@@ -1,24 +1,28 @@
 #!/usr/bin/env python
 """bench.py -- headline benchmark: k-means assignment step, points/sec, 8M x 256 fp32 @ 1024 clusters.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--points P]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--points P] [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[1] / configs[3]): P = 8 000 000 samples IN TOTAL (U[0,1), the reference's own
 benchmark distribution), 256 features, 1024 centroids = rows of the samples.  With N GPUs (one process per GPU
 under torchrun) the samples are range-partitioned, P/N rows per rank -> "scaling": "strong".
 
 A "step" is ONE assignment pass of the hot path (the reference's kmeans_assign_lloyd, src/kmeans.cu:293-364;
-here: tcgen05 distance filter + exact fp32 re-check + fused bookkeeping) over the rank's shard, resident in HBM:
+here: wgmma distance filter + exact fp32 re-check + fused bookkeeping) over the rank's shard, resident in HBM:
 `value` = P / max-over-ranks(device time per step) (SURVEY.md 8d: the metric is the assignment step).  The same
 run also times the FULL Lloyd iteration -- assign + per-cluster partial sums + NCCL all-reduce of the K*D fp32
 sums and K integer counts + normalise (BASELINE configs[3]) -- and reports it per phase under `iteration`.
 
 Other keys: `e2e` (the same pass through the reference-facing C ABI kmeans_cuda() with pinned HOST buffers: H2D
-of the samples and D2H of the assignments inside the timed region), `roofline` (the tcgen05 kernel, CUDA events
-around its launches, against the measured bf16 tensor peak of MEASURED_PEAKS.json), `cpu_baseline` (scikit-learn
+of the samples and D2H of the assignments inside the timed region), `roofline` (the wgmma kernel, CUDA events
+around its launches, against the bf16 tensor peak of MEASURED_PEAKS.json, else the H100 SXM data sheet), `cpu_baseline` (scikit-learn
 KMeans labelling on all host cores, the CPU reference north_star names; the C oracle port is nested), `clocks`.
 
-`--impl reference` times the UNMODIFIED reference (oracle/_ref/libKMCUDA.so, src-d/kmcuda rebuilt for sm_100 --
+`--dump-outputs DIR` writes what the last timed step computed, the assignments a caller receives, as
+DIR/assignments.npy (float32; DIR/assignments_rank<r>.npy with several ranks).  The inputs are seeded, so two builds
+can be compared output for output.
+
+`--impl reference` times the UNMODIFIED reference (oracle/_ref/libKMCUDA.so, src-d/kmcuda rebuilt for sm_90 --
 the reference has no CPU implementation, it is a CUDA library) through the same C ABI on the same P points with
 device mask (1 << N) - 1: `value` with device-resident inputs (device_ptrs = 0), `e2e` with pinned host buffers.
 If that library cannot be loaded the CPU oracle port is timed instead.
@@ -56,7 +60,7 @@ WORKLOAD = ("k-means assignment step, %d x %d fp32 samples in total (U[0,1)) @ %
 IMPORT = 3
 # kernels of this library per assignment pass (L2, tensor-core path): tc_prep_fused_kernel (||c||^2, mean, centred
 # norms, scale, fp16 table in one launch), tc_assign_kernel, recheck_pairs, recheck_reduce, exact_rows_few, exact_pass
-# (row list), finalize_rows (profiles/r02_launches_iteration.csv lists them, next to the update's kernels)
+# (row list), finalize_rows
 LAUNCHES_PER_ASSIGN = 7
 
 
@@ -72,7 +76,7 @@ def shard_range(total, rank, world):
 
 
 class ClockSampler:
-    """SM clock / power / throttle reasons DURING the timed region (B200_PROFILING.md's clocks line).
+    """SM clock / power / throttle reasons DURING the timed region.
 
     The timed region of the default run is ~0.1 s, shorter than nvidia-smi's start-up and coarser than its averaged
     readings, so NVML is polled in-process by a thread (~1 ms period) and only the samples between the two `mark()`
@@ -243,9 +247,10 @@ class ClockSampler:
 
 def measured_peaks():
     try:
-        return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
+        return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "MEASURED_PEAKS.json (measured)"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        # NVIDIA H100 SXM data sheet (700 W): HBM3 bandwidth, dense bf16 tensor rate
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet"
 
 
 def cpu_baseline():
@@ -352,7 +357,7 @@ def run_reference(args):
         torch.cuda.empty_cache()
         e2e_steps = max(1, min(steps, 3))
         dte = time_c_abi(ref, n, Xh.data_ptr(), Ch.ctypes.data, Ah.data_ptr(), mask, -1, e2e_steps, 1)
-        note = ("unmodified src-d/kmcuda rebuilt for sm_100 (oracle/_ref), device mask 0x%x, kmeans_cuda(import, "
+        note = ("unmodified src-d/kmcuda rebuilt for sm_90 (oracle/_ref), device mask 0x%x, kmeans_cuda(import, "
                 "tolerance=1, yinyang_t=0) = one assign pass on all %d points; `value`: device-resident inputs "
                 "(device_ptrs=0), %d timed calls; `e2e`: pinned host buffers, %d calls" % (mask, n, steps, e2e_steps))
         v = n / dt
@@ -377,6 +382,21 @@ def run_reference(args):
                      "cpu_baseline": {"value": v, "unit": UNIT, "cores": cores, "kind": "port", "sample": note},
                      "e2e": {"value": v, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}})
     emit(line)
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(directory, name, values, world=1):
+    """values: 1-D integer / float array; stored as float32.  Each of the `world` rank files gets an equal share of the
+    64 MB total; beyond it a fixed seeded sample of the rows is stored."""
+    os.makedirs(directory, exist_ok=True)
+    v = np.asarray(values)
+    share = DUMP_LIMIT_BYTES // max(1, world)
+    if v.size * 4 > share:
+        keep = np.sort(np.random.default_rng(0).choice(v.size, share // 4, replace=False))
+        v = v[keep]
+    np.save(os.path.join(directory, name + ".npy"), v.astype(np.float32))
 
 
 def run_ours(args):
@@ -441,6 +461,9 @@ def run_ours(args):
     kt = sh.kernel_times(min(args.steps, 64))
     kernel_ms = max_over_ranks(sum(kt) / len(kt))
     a_ref = a.clone()
+    if getattr(args, "dump_outputs", None):
+        dump_outputs(args.dump_outputs, "assignments" if world == 1 else "assignments_rank%d" % rank, a_ref.cpu().numpy(),
+                     world)
 
     if args.skip_extras:
         if rank == 0:
@@ -555,7 +578,7 @@ def run_ours(args):
 
     if rank == 0:
         peaks, peak_kind = measured_peaks()
-        peak_tf = float(peaks.get("bf16_tflops", 1590.0))
+        peak_tf = float(peaks.get("bf16_tflops", 989.0))
         flops = 2.0 * n * K * D
         achieved = flops / (kernel_ms * 1e-3) / 1e12
         traffic = None
@@ -586,8 +609,7 @@ def run_ours(args):
             "gpu_launches": args.steps * LAUNCHES_PER_ASSIGN,
             "roofline": {"bound": "tensor", "kernel": "tc_assign_kernel", "achieved": achieved, "peak": peak_tf,
                          "unit": "TFLOP/s", "frac": achieved / peak_tf, "traffic": traffic,
-                         "peak_source": "%s bf16_tflops (burst) of MEASURED_PEAKS.json; fp16 and bf16 share the "
-                                        "tcgen05 rate" % peak_kind,
+                         "peak_source": "bf16_tflops of %s; fp16 and bf16 share the tensor-core rate" % peak_kind,
                          "kernel_ms": kernel_ms, "algorithmic_flops_per_launch": flops,
                          "algorithmic_hbm_bytes_per_launch": n * (D * 4 + 4),
                          "whole_step_frac": 2.0 * n * K * D / (ms_per_step * 1e-3) / 1e12 / peak_tf},
@@ -608,8 +630,12 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--points", type=int, default=N_POINTS, help="samples IN TOTAL (default: the headline 8M)")
     ap.add_argument("--skip-extras", action="store_true", help="profiling runs: no iteration / e2e / cpu_baseline legs")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the assignments of the last timed step to DIR/assignments.npy (float32)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else max(args.warmup, 1)
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs dumps this library's outputs; it does not apply to --impl reference")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -1,5 +1,5 @@
 /*
- * kmcuda.h -- public C ABI of the B200-native libKMCUDA.
+ * kmcuda.h -- public C ABI of the H100-native libKMCUDA.
  *
  * This header re-states, declaration for declaration, the drop-in boundary of src-d/kmcuda
  * (reference: src/kmcuda.h).  Every enum value and every argument position crosses the ABI and is

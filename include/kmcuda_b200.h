@@ -1,5 +1,5 @@
 /*
- * kmcuda_b200.h -- shard-level C ABI of the B200-native libKMCUDA (extension, not in the reference).
+ * kmcuda_b200.h -- shard-level C ABI of the H100-native libKMCUDA (extension, not in the reference).
  *
  * The reference is single-process multi-GPU: one kmeans_cuda() call drives every device in the mask
  * and exchanges results with cudaMemcpyPeerAsync (reference src/private.h:177-183, src/kmeans.cu:
@@ -44,7 +44,7 @@ KMCUDAResult kmcuda_b200_assign(kmcuda_b200_shard *shard, uint32_t samples_size,
                                 const float *centroids, uint32_t *assignments,
                                 uint32_t *assignments_prev, uint32_t *changed, void *stream);
 
-/* 1 if the last assign pass ran on the tcgen05 filter + exact re-check, 0 if on the exact SIMT
+/* 1 if the last assign pass ran on the tensor-core (wgmma) filter + exact re-check, 0 if on the exact SIMT
  * kernel; also reports how many samples needed the re-check / the full exact fallback. */
 int32_t kmcuda_b200_last_pass_info(kmcuda_b200_shard *shard, uint32_t *rechecked, uint32_t *overflowed);
 

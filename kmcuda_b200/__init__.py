@@ -1,4 +1,4 @@
-"""kmcuda_b200 -- B200-native (sm_100a) implementation of kmcuda's batched-distance hot path.
+"""kmcuda_b200 -- H100-native (sm_90a) implementation of kmcuda's batched-distance hot path.
 
 Python surface = the reference's `libKMCUDA` module (reference src/python.cc:33-54):
 

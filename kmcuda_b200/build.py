@@ -1,4 +1,4 @@
-"""In-tree build of libKMCUDA.so for sm_100a (nvcc cross-compiles without a GPU).
+"""In-tree build of libKMCUDA.so for sm_90a (nvcc cross-compiles without a GPU).
 
     python kmcuda_b200/build.py            # incremental (run by path: importing the package needs the built library)
     python kmcuda_b200/build.py --force
@@ -23,7 +23,7 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 CU_SOURCES = ["simt_kernels.cu", "knn_kernels.cu", "assign_tc.cu", "yinyang.cu", "shard.cu", "exchange.cu", "api.cu"]
 CC_SOURCES = ["py_module.cc"]
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fno-strict-aliasing", "-I" + os.path.join(ROOT, "include"),
               "-I" + CSRC]
 

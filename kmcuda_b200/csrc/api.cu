@@ -139,8 +139,8 @@ static KMCUDAResult list_devices(uint32_t device, int verbosity, std::vector<int
     }
     cudaDeviceProp props;
     if (cudaGetDeviceProperties(&props, dev) != cudaSuccess) continue;
-    if (props.major < 10) {
-      KMB_INFO("compute capability mismatch for device %d: this build targets sm_100a, have %d.%d\n",
+    if (props.major != 9 || props.minor != 0) {   // sm_90a code runs on compute capability 9.0 only
+      KMB_INFO("compute capability mismatch for device %d: this build targets sm_90a, have %d.%d\n",
                dev, props.major, props.minor);
       continue;
     }

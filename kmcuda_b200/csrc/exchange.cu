@@ -223,7 +223,7 @@ KMCUDAResult kmcuda_b200_exchange_reduce(kmcuda_b200_exchange* ex, float* total_
   for (int r = 0; r < ex->world; r++) pp.base[r] = ex->peer[r];
   const size_t nsums = static_cast<size_t>(ex->K) * ex->D;
   const size_t nvec4 = nsums / 4;
-  const unsigned grid = static_cast<unsigned>(std::min<size_t>(148, (nvec4 + 255) / 256 + 1));
+  const unsigned grid = static_cast<unsigned>(std::min<size_t>(kmb::device_sms(), (nvec4 + 255) / 256 + 1));
   uint32_t* d_err = reinterpret_cast<uint32_t*>(ex->local + ex->off_err);
   kmb::exchange_reduce_kernel<<<grid, 256, 0, st>>>(pp, ex->off_sums[b], ex->off_counts[b], ex->off_flags, ex->iter,
                                                      nvec4, nsums, ex->K, total_sums, total_counts, d_err);

@@ -204,7 +204,7 @@ cudaError_t launch_knn_search(int metric, int k, const float* X, const float* C,
   if (q_length == 0) return cudaSuccess;
   const int smem_d = D <= kKnnMaxSmemD ? D : 0;
   const size_t smem = static_cast<size_t>(kKnnWarps) * smem_d * sizeof(float);
-  const unsigned grid = rows ? 148u * 8u : static_cast<unsigned>(std::min<size_t>(cdivk(q_length, kKnnWarps), 148u * 64u));
+  const unsigned grid = rows ? device_sms() * 8u : static_cast<unsigned>(std::min<size_t>(cdivk(q_length, kKnnWarps), device_sms() * 64u));
   cudaError_t e;
   if (metric == 1) {
     if ((e = cudaFuncSetAttribute(knn_warp_search_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,

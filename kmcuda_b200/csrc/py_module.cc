@@ -378,7 +378,7 @@ PyObject* py_knn_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
   return Py_BuildValue("K", static_cast<unsigned long long>(reinterpret_cast<uintptr_t>(neighbors)));
 }
 
-char module_doc[] = "K-means and K-nn on NVIDIA B200 (drop-in for src-d/kmcuda's libKMCUDA).";
+char module_doc[] = "K-means and K-nn on NVIDIA H100 (drop-in for src-d/kmcuda's libKMCUDA).";
 char kmeans_doc[] = "kmeans_cuda(samples, clusters, tolerance=.01, init=\"k-means++\", yinyang_t=.1, metric=\"L2\", "
                     "average_distance=False, seed=time(), device=0, verbosity=0) -> (centroids, assignments[, avg])";
 char knn_doc[] = "knn_cuda(k, samples, centroids, assignments, metric=\"L2\", device=0, verbosity=0) -> neighbors";

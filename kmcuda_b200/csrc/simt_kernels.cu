@@ -14,6 +14,16 @@
 
 namespace kmb {
 
+unsigned device_sms() {
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+      n <= 0) {
+    cudaGetLastError();
+    n = 132;   // H100 SXM
+  }
+  return static_cast<unsigned>(n);
+}
+
 static inline unsigned cdiv(size_t a, size_t b) { return static_cast<unsigned>((a + b - 1) / b); }
 
 // row lists up to this length are handled one CTA per row (exact_rows_few_kernel)
@@ -264,7 +274,7 @@ static cudaError_t launch_exact_pass(const float* X, const float* C, const float
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        static_cast<int>(cfg.smem));
   if (e != cudaSuccess) return e;
-  unsigned grid = d_nrows ? 148 * 2 : cdiv(n, cfg.rb);
+  unsigned grid = d_nrows ? device_sms() * 2 : cdiv(n, cfg.rb);
   if (grid == 0) return cudaSuccess;
   kern<<<grid, cfg.rb * cfg.tpr, cfg.smem, st>>>(X, C, csq, n, D, K, rows, d_nrows, result, cfg.use_smem, cfg.rb, G,
                                                  assign, groups, bounds);
@@ -276,8 +286,8 @@ cudaError_t launch_assign_exact(int metric, const float* X, const float* C, cons
                                 const uint32_t* d_nrows, uint32_t* result, cudaStream_t st) {
   if (d_nrows) {  // list mode: short lists go to the one-CTA-per-row kernel (decided on the device)
     const size_t smem = sizeof(float) * D;
-    if (metric == 1) exact_rows_few_kernel<1><<<148 * 4, 512, smem, st>>>(X, C, csq, D, K, rows, d_nrows, result);
-    else exact_rows_few_kernel<0><<<148 * 4, 512, smem, st>>>(X, C, csq, D, K, rows, d_nrows, result);
+    if (metric == 1) exact_rows_few_kernel<1><<<device_sms() * 4, 512, smem, st>>>(X, C, csq, D, K, rows, d_nrows, result);
+    else exact_rows_few_kernel<0><<<device_sms() * 4, 512, smem, st>>>(X, C, csq, D, K, rows, d_nrows, result);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
   }
@@ -719,7 +729,7 @@ __global__ void peer_min_u32_kernel(const PeerU32 pb, size_t count, uint32_t* __
   }
 }
 cudaError_t launch_peer_min_u32(const PeerU32& pb, size_t count, uint32_t* out, cudaStream_t st) {
-  const unsigned grid = static_cast<unsigned>(std::min<size_t>(148 * 8, (count + 255) / 256 + 1));
+  const unsigned grid = static_cast<unsigned>(std::min<size_t>(device_sms() * 8, (count + 255) / 256 + 1));
   peer_min_u32_kernel<<<grid, 256, 0, st>>>(pb, count, out);
   return cudaGetLastError();
 }
@@ -728,7 +738,7 @@ cudaError_t launch_peer_reduce(const PeerBuffers& pb, uint32_t K, int D, float* 
                                cudaStream_t st) {
   const size_t nsums = static_cast<size_t>(K) * D;
   const size_t nvec4 = nsums / 4;
-  const unsigned grid = static_cast<unsigned>(std::min<size_t>(148 * 4, (nvec4 + 255) / 256 + 1));
+  const unsigned grid = static_cast<unsigned>(std::min<size_t>(device_sms() * 4, (nvec4 + 255) / 256 + 1));
   peer_reduce_kernel<<<grid, 256, 0, st>>>(pb, nvec4, nsums, K, out_sums, out_counts);
   return cudaGetLastError();
 }
@@ -1049,17 +1059,17 @@ __global__ void fill_u32_kernel(uint32_t* p, uint32_t v, size_t n) {
 
 cudaError_t launch_half_to_float(const void* src, float* dst, size_t n, cudaStream_t st) {
   if (!n) return cudaSuccess;
-  half_to_float_kernel<<<min(cdiv(n, 256), 148u * 32u), 256, 0, st>>>(static_cast<const __half*>(src), dst, n);
+  half_to_float_kernel<<<min(cdiv(n, 256), device_sms() * 32u), 256, 0, st>>>(static_cast<const __half*>(src), dst, n);
   return cudaGetLastError();
 }
 cudaError_t launch_float_to_half(const float* src, void* dst, size_t n, cudaStream_t st) {
   if (!n) return cudaSuccess;
-  float_to_half_kernel<<<min(cdiv(n, 256), 148u * 32u), 256, 0, st>>>(src, static_cast<__half*>(dst), n);
+  float_to_half_kernel<<<min(cdiv(n, 256), device_sms() * 32u), 256, 0, st>>>(src, static_cast<__half*>(dst), n);
   return cudaGetLastError();
 }
 cudaError_t launch_fill_u32(uint32_t* p, uint32_t v, size_t n, cudaStream_t st) {
   if (!n) return cudaSuccess;
-  fill_u32_kernel<<<min(cdiv(n, 256), 148u * 32u), 256, 0, st>>>(p, v, n);
+  fill_u32_kernel<<<min(cdiv(n, 256), device_sms() * 32u), 256, 0, st>>>(p, v, n);
   return cudaGetLastError();
 }
 

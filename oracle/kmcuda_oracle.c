@@ -8,7 +8,7 @@
  * reference's fp16x2 path accumulates in fp16 and has no bit-wise parity contract (SURVEY.md 7.2).
  *
  * Parity pin: on the GPU box this restatement is compared bit-for-bit against the UNMODIFIED
- * reference rebuilt for sm_100 (oracle/_ref/libKMCUDA.so, see oracle/build_ref.sh) by
+ * reference rebuilt for sm_90 (oracle/_ref/libKMCUDA.so, see oracle/build_ref.sh) by
  * tests/test_parity_gpu.py::test_oracle_matches_reference_*; on the CPU it is pinned against
  * scikit-learn the same way the reference's own test.py pins the reference (tests/test_oracle_cpu.py).
  * Cosine uses the host libm acosf, which is NOT bit-specified to equal CUDA's acosf: cosine results

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""A/B timing of builds of libKMCUDA.so on the headline shape (run on the B200 box).  Checker script: it lives
+"""A/B timing of builds of libKMCUDA.so on the headline shape (run on an H100).  Checker script: it lives
 under tests/ because it loads the reference library through oracle/ (not collected by pytest).
 
     python tests/ab_kernel.py [name=path/to/libKMCUDA.so ...] [--n 8000000] [--env KEY=VAL,...]

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     # The library continues a Yinyang run with Lloyd passes once a Yinyang iteration proves slower than a Lloyd
     # iteration of the same run (identical results).  The tests that exercise the Yinyang kernels need them to run:
     # the switch is off for the suite and on in the one test that checks it.

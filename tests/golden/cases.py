@@ -43,3 +43,22 @@ def make_assign_case(n, d, k, seed, kind):
     else:
         C += (rng.standard_normal(C.shape) * 0.01 * np.abs(C).mean()).astype(np.float32)
     return np.ascontiguousarray(X), np.ascontiguousarray(C)
+
+
+HEADLINE_SAMPLE = 65536     # rows of the 8M headline pass whose reference assignments are stored
+
+
+def headline_8m():
+    """8 000 000 x 256 U[0,1) samples (seed 777, the reference README's benchmark), 1024 centroids = rows of them"""
+    n, d, k = 8000000, 256, 1024
+    rng = np.random.default_rng(777)
+    X = np.empty((n, d), np.float32)
+    for i in range(0, n, 1000000):               # chunked generation keeps the host RSS at the matrix itself
+        X[i:i + 1000000] = rng.random((1000000, d), dtype=np.float32)
+    C0 = X[rng.choice(n, k, replace=False)].copy()
+    return X, C0
+
+
+def headline_rows():
+    """the fixed sample of headline rows (sorted) that tests/golden/headline_8m.npz covers"""
+    return np.sort(np.random.default_rng(2024).choice(8000000, HEADLINE_SAMPLE, replace=False))

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Secondary configurations of BASELINE.json (C1, C2, C3, C5) on one B200: this library next to the
+"""Secondary configurations of BASELINE.json (C1, C2, C3, C5) on one H100: this library next to the
 unmodified reference (oracle/_ref/libKMCUDA.so), same inputs, same C-ABI call, wall clock around the call.
 
     python tests/secondary_configs.py [c1 c2 c3 c5 ...] [--out gpurun_out/secondary.json]
@@ -145,9 +145,10 @@ def c3_child(n_full, tol):
     print("C3_USED_CLUSTERS %d" % len(np.unique(A)), flush=True)
 
 
-def c3(ours, ref, res, n_full=4000000, n_ref=100000, tol=0.0005):
-    """C3 as specified: Yinyang, angular, fp16 samples, 4M x 480 @ 40000, yinyang_t = 0.1 (G = 4000, 64 GB of
-    bounds).  The reference needs days to converge here (README.md:60-62); the run stops at `tol` reassignments so
+def c3(ours, ref, res, n_full=2000000, n_ref=100000, tol=0.0005):
+    """C3 sized for one 80 GB H100: Yinyang, angular, fp16 samples, 2M x 480 @ 40000, yinyang_t = 0.1 (G = 4000, 32 GB
+    of bounds; the 4M rows of the original configuration would need 64 GB of bounds next to the samples, the
+    centroids and the pass's work buffers).  The reference needs days to converge here (README.md:60-62); the run stops at `tol` reassignments so
     that a few Yinyang iterations (after the Lloyd draft phase and one bounds refresh) are timed."""
     import subprocess
     D, K = 480, 40000
@@ -165,8 +166,8 @@ def c3(ours, ref, res, n_full=4000000, n_ref=100000, tol=0.0005):
     if r.returncode != 0:
         out["stderr_tail"] = r.stderr[-1500:]
     out["hbm_floor_note"] = ("per Yinyang iteration the bounds stream is 2 * (G + 1) * 4 B per sample = %.1f GB; at the "
-                             "measured 6.57 TB/s that is %.1f ms" % (2 * 4001 * 4 * n_full / 1e9,
-                                                                      2 * 4001 * 4 * n_full / 6.5725e12 * 1e3))
+                             "H100 SXM data sheet's 3.35 TB/s that is %.1f ms" % (2 * 4001 * 4 * n_full / 1e9,
+                                                                                 2 * 4001 * 4 * n_full / 3.35e12 * 1e3))
     # agreement with the reference on a sub-sample, one assignment step (the reference accumulates fp16 data in fp16,
     # this library works on the exactly widened values: statistical agreement, SURVEY.md a2)
     X, C0 = _c3_data(n_ref, n_ref, D, K, np.random.default_rng(777))

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: `pytest -m gpu`).  Everything goes through the C ABI of
+"""GPU parity tests (run on an H100: `pytest -m gpu`).  Everything goes through the C ABI of
 kmcuda_b200/libKMCUDA.so; the oracle (oracle/) and the rebuilt reference (oracle/_ref) are checkers only.
 
 Bars: bit-exact for assignments / neighbour indices (the tensor-core filter + exact re-check is
@@ -72,7 +72,7 @@ def test_oracle_matches_reference(ref):
 @pytest.mark.parametrize("force_exact", ["0", "1"])
 def test_assign_matches_golden(ours, name, force_exact, monkeypatch):
     """one assignment pass (tolerance=1 trick, reference src/test.py:512-519) == golden, bit for bit;
-    force_exact=0 takes the tcgen05 filter + re-check wherever the shape allows it"""
+    force_exact=0 takes the wgmma filter + re-check wherever the shape allows it"""
     monkeypatch.setenv("KMCUDA_B200_FORCE_EXACT", force_exact)
     X, C = cases.make_assign_case(*cases.ASSIGN_CASES[name])
     got = one_pass(ours, X, C)
@@ -98,7 +98,7 @@ def _shard_pass(X, C, assign=None, metric="L2", force_exact=False):
 
 
 def test_tensor_core_path_runs_and_matches_reference_100k(ref):
-    """C1-sized pass: the tcgen05 path must be the one that runs, and equal the reference kernel"""
+    """C1-sized pass: the tensor-core path must be the one that runs, and equal the reference kernel"""
     rng = np.random.default_rng(777)
     X = rng.random((100000, 256), dtype=np.float32)
     C = X[rng.choice(len(X), 1024, replace=False)].copy()
@@ -118,10 +118,12 @@ def _unit(a):
 
 @pytest.mark.parametrize("n,d,k,metric", [(20000, 256, 500, "cos"), (20000, 480, 2000, "L2"),
                                           (20000, 480, 2000, "cos"), (30000, 64, 20000, "L2"),
-                                          (9000, 324, 700, "L2")])
+                                          (9000, 324, 700, "L2"), (20000, 240, 2000, "L2"),
+                                          (20000, 240, 2000, "cos"), (9000, 196, 700, "L2")])
 def test_tensor_core_wide_shapes_match_reference(ref, n, d, k, metric):
-    """cosine, D up to 512 (single A buffer in TMEM) and K >> 1024 (chunk-list compaction) through the
-    tcgen05 filter: bit-identical to the reference kernel"""
+    """cosine, D up to 512 (single A buffer in shared memory; above 256 the shallow pipeline with quad-shuffle
+    regrouping), ragged last K-blocks and K >> 1024 (chunk-list compaction) through the wgmma filter: bit-identical
+    to the reference kernel"""
     rng = np.random.default_rng(n + d + k)
     X = rng.standard_normal((n, d)).astype(np.float32)
     if metric == "cos":
@@ -297,7 +299,7 @@ def _mixture(n, d, k, seed, sigma=0.25):
 
 @pytest.mark.parametrize("n,d,k,metric", [(60000, 64, 256, 0), (40000, 100, 120, 0), (30000, 32, 64, 1)])
 def test_yinyang_tensor_core_local_step_equals_reference_order_scan(ours, ref, n, d, k, metric, monkeypatch):
-    """Yinyang iterations: the tcgen05 candidate pass + exact finish (yinyang.cu) must give the same run as the
+    """Yinyang iterations: the tensor-core candidate pass + exact finish (yinyang.cu) must give the same run as the
     reference-order per-row scan (KMCUDA_B200_FORCE_EXACT=1), and both the same as the reference library"""
     rng = np.random.default_rng(42 + d)
     X = rng.random((n, d), dtype=np.float32) if metric == 0 else rng.standard_normal((n, d)).astype(np.float32)
@@ -421,7 +423,7 @@ def _knn(lib, k, X, C, A, metric=0):
 @pytest.mark.parametrize("kind,n,d,kc,k", [("uniform", 30000, 48, 200, 10), ("mixture", 60000, 64, 300, 10),
                                            ("mixture", 50000, 256, 100, 3), ("uniform", 20000, 100, 50, 15)])
 def test_knn_tensor_core_path_matches_reference(ours, ref, capfd, monkeypatch, kind, n, d, kc, k):
-    """knn_cuda through the tcgen05 candidate pass (cluster-sorted tiles, two passes, exact re-check + selection):
+    """knn_cuda through the tensor-core candidate pass (cluster-sorted tiles, two passes, exact re-check + selection):
     same neighbours as the reference library, and as a float64 brute force on a sample of the queries"""
     rng = np.random.default_rng(n + d)
     if kind == "uniform":
