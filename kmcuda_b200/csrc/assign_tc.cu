@@ -14,8 +14,8 @@
 //   consumer warps  : two warpgroups, one per 64-row half of the tile; each issues wgmma m64n128k16 (A and B
 //                     from shared memory, fp32 accumulators in its registers) over every K-block, plus one
 //                     extra K=16 step that adds -||c||^2/2 as three fp16 terms against constant ones, so
-//                     acc = x.c - ||c||^2/2.  The accumulator fragment is regrouped through a small per-warp
-//                     shared-memory buffer so that every thread holds 64 consecutive columns of one row; then
+//                     acc = x.c - ||c||^2/2.  The accumulator fragment is regrouped with quad shuffles so
+//                     that every thread holds 64 consecutive columns of one row; then
 //                     the running row maximum M is updated and every column whose value is within `margin`
 //                     of M is recorded (bit mask per 32-column chunk); margin is a rigorous bound on
 //                     |approx - exact| derived from the actual rounding residuals (Cauchy-Schwarz), so the
@@ -25,8 +25,9 @@
 //   bit-identical to the reference kernel's, ties included.
 //
 // Shared memory (227 KB per block on H100) holds the whole fp16 A operand of a tile (16 KB per 64 features), so
-// the tensor-core path serves D <= 512; two A buffers for D <= 128, so the next tile is converted while the
-// current one is multiplied.  For D > 256 the pipeline is shallower (see smem_layout).
+// the tensor-core path serves D <= 512.  The A region is a ring of K-block slots with room for more than one tile
+// (D <= 256), so the next tile's first K-blocks are converted while the current one is multiplied.  For D > 256 the
+// pipeline is shallower (see smem_layout).
 //
 // The same kernel template serves two more callers (MODE template parameter, see tc::Params):
 //   MODE 1  Yinyang local step (reference kmeans.cu:584-672): the samples are a compacted row list; candidates =
@@ -69,8 +70,6 @@ constexpr int B_STAGE_BYTES = B_KB_BYTES;
 constexpr int AUG_A_BYTES = TM * 32;    // 4 KiB  (K=16 fp16, no swizzle)
 constexpr int AUG_B_BYTES = TN * 32;    // 4 KiB
 constexpr int LIST_LEN = 5;             // entries per epilogue thread: one per n-tile that held a candidate (max, 2 x 32-bit mask, n-tile)
-constexpr int XPOSE_STRIDE = 36;        // floats per row of a warp's regrouping buffer (16 rows x 2 halves x 16 columns, padded)
-constexpr int XPOSE_WARP_BYTES = 16 * XPOSE_STRIDE * 4;
 // Knock-out builds (timing experiments only, results are garbage): 1 = the epilogue does not read the accumulators,
 // 2 = no MMA is issued, 3 = converters do no work, 5 = the B / bias copies are not issued, 7 = the epilogue loads the
 // accumulators but skips the ALU work on them.  Which of them shortens the kernel says what bounds it.
@@ -109,22 +108,27 @@ struct Stats {       // written by the centroid prep kernels, read by the main k
 
 constexpr uint32_t LIST_ARRAY = 2 * LIST_LEN * 256 * 4;   // bytes of one of the four list arrays (both tile parities)
 struct SmemLayout {  // byte offsets from the 1024-aligned dynamic smem base
-  uint32_t a, b, aug_a, aug_b, list, norms, fin, mu, xpose, bars, total;
+  uint32_t a, b, aug_a, aug_b, list, norms, fin, mu, bars, total;
 };
 
-// Per-shape pipeline depths.  D <= 256: A region of 4 K-blocks (two buffers for D <= 128), 4 B stages, 2 bias buffers,
-// 4-deep norms ring, accumulators regrouped through a per-warp buffer.  D > 256: the 128 KiB A tile leaves 2 B stages,
-// 1 bias buffer and a 2-deep norms ring (enough with one A buffer: the converters cannot run more than one segment ahead),
-// and the accumulators are regrouped with quad shuffles instead of the 18 KiB buffer.
+// Per-shape pipeline depths.  The A region is a ring of a_slots(nkb) K-block slots that the converters fill K-block by
+// K-block, across tile boundaries: with more slots than K-blocks per tile, the next tile's first K-blocks are converted
+// while the current tile is still being multiplied.  D <= 128: 4 slots (two tiles or more), 4 B stages, 2 bias buffers.
+// D 129-256: 5-6 slots, 4 B stages, 1 bias buffer.  D > 256: the 128 KiB region (8 slots) leaves 2 B stages and 1 bias
+// buffer.  The norms ring must be deeper than the number of segments the converters can run ahead (see layouts_fit).
 __host__ __device__ constexpr bool wide_nkb(int nkb) { return nkb > WIDE_NKB; }
 __host__ __device__ constexpr int b_stages(int nkb) { return wide_nkb(nkb) ? 2 : B_STAGES; }
-__host__ __device__ constexpr int aug_bufs(int nkb) { return wide_nkb(nkb) ? 1 : 2; }
-__host__ __device__ constexpr int norm_depth(int nkb) { return wide_nkb(nkb) ? 2 : 4; }
+__host__ __device__ constexpr int aug_bufs(int nkb) { return nkb <= 2 ? 2 : 1; }
+__host__ __device__ constexpr int a_slots(int nkb) { return nkb <= 2 ? 4 : nkb == 3 ? 5 : nkb == 4 ? 6 : MAX_NKB; }
+// The converters write the norms of segment f + depth after waiting for the slot of its last K-block, i.e. after every
+// consumer warp released K-block (f + depth + 1) * nkb - 1 - a_slots; that K-block belongs to segment f + 1 or later
+// (so each warp has read the norms of f) exactly when depth * nkb > a_slots.
+__host__ __device__ constexpr int norm_depth(int nkb) { return a_slots(nkb) / nkb + 1; }
 
 __host__ __device__ constexpr SmemLayout smem_layout(int nkb) {
   SmemLayout L{};
   uint32_t o = 0;
-  L.a = o; o += (wide_nkb(nkb) ? MAX_NKB : WIDE_NKB) * A_KB_BYTES;
+  L.a = o; o += a_slots(nkb) * A_KB_BYTES;
   L.b = o; o += b_stages(nkb) * B_STAGE_BYTES;
   L.aug_a = o; o += AUG_A_BYTES;
   L.aug_b = o; o += aug_bufs(nkb) * AUG_B_BYTES;
@@ -135,14 +139,18 @@ __host__ __device__ constexpr SmemLayout smem_layout(int nkb) {
   L.fin = o; o += 2 * 5 * 256 * 4;    // [tile parity][M|cnt|flags|margin|M2][epilogue thread]
   L.norms = o; o += norm_depth(nkb) * 4 * TM * 4;   // [segment % depth][x|d][row]  x~^2 | residual^2 | (k-NN) exact s^2|x-c|^2 | (k-NN) s^2(|x|+|c|)^2
   L.mu = o; o += MAX_NKB * KB * 4;    // -mu * s per feature (zero padded): the converters' centring term
-  L.xpose = o; o += wide_nkb(nkb) ? 0 : N_EPI_WARPS * XPOSE_WARP_BYTES;
   L.bars = o; o += 64 * 8;
   L.total = o;
   return L;
 }
 static_assert(4 * LIST_ARRAY + 2 * 5 * 256 * 4 >= 48 * 256 * 4, "k-NN scratch overlaps the norms");
-static_assert(smem_layout(MAX_NKB).total + 1024 <= 232448 && smem_layout(WIDE_NKB).total + 1024 <= 232448,
-              "227 KiB of shared memory per block on H100");
+__host__ __device__ constexpr bool layouts_fit() {
+  for (int k = 1; k <= MAX_NKB; k++)
+    if (smem_layout(k).total + 1024 > 232448 || a_slots(k) < k || a_slots(k) > MAX_NKB || norm_depth(k) * k <= a_slots(k))
+      return false;
+  return true;
+}
+static_assert(layouts_fit(), "227 KiB of shared memory per block on H100; a whole tile in the A ring; norms ring depth");
 
 // barrier indices inside the bars[] array
 enum {
@@ -150,9 +158,9 @@ enum {
   BAR_B_EMPTY = BAR_B_FULL + B_STAGES,        // [B_STAGES]
   BAR_AUG_FULL = BAR_B_EMPTY + B_STAGES,      // [2]
   BAR_AUG_EMPTY = BAR_AUG_FULL + 2,           // [2]
-  BAR_A_FULL = BAR_AUG_EMPTY + 2,             // [2][MAX_NKB]
-  BAR_A_FREE = BAR_A_FULL + 2 * MAX_NKB,      // [2]
-  BAR_EMIT_FULL = BAR_A_FREE + 2,             // [2] epilogue -> emitter (per tile parity)
+  BAR_A_FULL = BAR_AUG_EMPTY + 2,             // [a_slots] converters -> consumers, per A slot
+  BAR_A_FREE = BAR_A_FULL + MAX_NKB,          // [a_slots] consumers -> converters, per A slot
+  BAR_EMIT_FULL = BAR_A_FREE + MAX_NKB,       // [2] epilogue -> emitter (per tile parity)
   BAR_EMIT_EMPTY = BAR_EMIT_FULL + 2,         // [2]
   BAR_COUNT = BAR_EMIT_EMPTY + 2
 };
@@ -800,8 +808,7 @@ template <int NKB, int MODE>
 __global__ void __launch_bounds__(N_THREADS, 1)
 tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
   static_assert(NKB <= MAX_NKB, "the A operand of a tile must fit its shared-memory region");
-  constexpr bool WIDE = wide_nkb(NKB);
-  constexpr int BST = b_stages(NKB), AUGB = aug_bufs(NKB), NDEPTH = norm_depth(NKB);
+  constexpr int BST = b_stages(NKB), AUGB = aug_bufs(NKB), NDEPTH = norm_depth(NKB), ASLOTS = a_slots(NKB);
   // 1024-byte alignment (128B-swizzle atoms) by an OFFSET into the shared array: the pointer keeps its shared address
   // space, so every access below is LDS / STS
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -811,7 +818,6 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
   const uint32_t bars_u32 = ptx::smem_u32(bars);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   constexpr int nkb = NKB;
-  constexpr int NBUF = NKB <= WIDE_NKB / 2 ? 2 : 1;   // A operand buffers in the A region
   // The error bound needs |x~| (the fp16-rounded operand row) and the rounding residual |a - x~|; the converters MEASURE
   // both.  KMB_ANALYTIC_RESIDUAL=1 (A/B build) bounds them from |a|^2 alone in the streaming modes 0 and 3 -- round-to-
   // nearest into fp16 moves a normal value by at most 2^-11 |a_i|, a subnormal one by at most 2^-25 -- which takes the
@@ -844,10 +850,12 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
     for (int s = 0; s < 2; s++) {
       ptx::mbar_init(&bars[BAR_AUG_FULL + s], 1);
       ptx::mbar_init(&bars[BAR_AUG_EMPTY + s], N_EPI_WARPS);
-      ptx::mbar_init(&bars[BAR_A_FREE + s], N_EPI_WARPS);
       ptx::mbar_init(&bars[BAR_EMIT_FULL + s], N_EPI_WARPS);
       ptx::mbar_init(&bars[BAR_EMIT_EMPTY + s], N_EMIT_WARPS);
-      for (int kb = 0; kb < MAX_NKB; kb++) ptx::mbar_init(&bars[BAR_A_FULL + s * MAX_NKB + kb], N_CONV_WARPS);
+    }
+    for (int s = 0; s < ASLOTS; s++) {
+      ptx::mbar_init(&bars[BAR_A_FULL + s], N_CONV_WARPS);
+      ptx::mbar_init(&bars[BAR_A_FREE + s], N_EPI_WARPS);
     }
     ptx::fence_mbar_init();
   }
@@ -870,8 +878,19 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
       for (uint32_t tile = tile_begin; tile < tile_end; tile += gridDim.x) {
         for (BlockIter<MODE> it(p, tile); it.valid(); it.next()) {
           const int n = static_cast<int>(it.cur);
-          // the bias block first: it is consumed last, and its buffer was released two n-tiles ago, so the copy is
-          // in flight for a whole n-tile before the consumers ask for it
+#pragma unroll
+          for (int kb = 0; kb < NKB; kb++) {
+            TC_WAIT(BAR_B_EMPTY + bs, bph ^ 1, 1);
+#if KMB_KO == 5
+            ptx::mbar_arrive(&bars[BAR_B_FULL + bs]);
+#else
+            ptx::mbar_arrive_expect_tx(&bars[BAR_B_FULL + bs], B_KB_BYTES);
+            ptx::tma_load_2d(smem + L.b + bs * B_STAGE_BYTES, &tmap_b, kb * KB, n * TN, &bars[BAR_B_FULL + bs]);
+#endif
+            if (++bs == BST) { bs = 0; bph ^= 1; }
+          }
+          // the bias block after the K-blocks: it is consumed last, and with one buffer its release (the end of the
+          // previous n-tile) must not hold back the centroid stages of this one
           const int as = ac % AUGB;
           const uint32_t aph = (ac / AUGB) & 1;
           TC_WAIT(BAR_AUG_EMPTY + as, aph ^ 1, 2);
@@ -884,17 +903,6 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
                          AUG_B_BYTES, &bars[BAR_AUG_FULL + as]);
 #endif
           ac++;
-#pragma unroll
-          for (int kb = 0; kb < NKB; kb++) {
-            TC_WAIT(BAR_B_EMPTY + bs, bph ^ 1, 1);
-#if KMB_KO == 5
-            ptx::mbar_arrive(&bars[BAR_B_FULL + bs]);
-#else
-            ptx::mbar_arrive_expect_tx(&bars[BAR_B_FULL + bs], B_KB_BYTES);
-            ptx::tma_load_2d(smem + L.b + bs * B_STAGE_BYTES, &tmap_b, kb * KB, n * TN, &bars[BAR_B_FULL + bs]);
-#endif
-            if (++bs == BST) { bs = 0; bph ^= 1; }
-          }
         }
       }
     }
@@ -903,7 +911,7 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
     const int q = warp & 3;
     const int row = q * 32 + lane;          // this thread's sample row within the tile
     const float s = p.stats->scale;
-    uint32_t si = 0;
+    uint32_t si = 0, as = 0, aph = 0;       // segments converted; A ring slot and phase of the next K-block
     for (uint32_t tile = tile_begin; tile < tile_end; tile += gridDim.x) {
       if (MODE == 2 && p.knn_nblk[tile] == 0) continue;
       const float* xrow = nullptr;
@@ -921,9 +929,6 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
         xrow = p.X + static_cast<size_t>(min(p.rows[tile * TM + row], p.n - 1)) * p.D;
       const uint32_t nseg = MODE == 2 ? p.knn_rcount[tile] : 1u;
       for (uint32_t seg = 0; seg < nseg; seg++, si++) {
-        const int abuf = si % NBUF;
-        TC_WAIT(BAR_A_FREE + abuf, ((si / NBUF) & 1) ^ 1, 7);   // wgmmas of the previous user of this buffer are done
-        uint8_t* a_row = smem + L.a + abuf * (NKB * A_KB_BYTES) + row * 128;
         // ||x~||^2 and ||s(x - mu) - x~||^2 as even/odd partial sums
         uint64_t nx2 = 0ull, nd2 = 0ull;
         const uint64_t s2 = ptx::pack2(s, s);
@@ -984,12 +989,16 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
               pk[half * 16 + c * 2 + 1] = *reinterpret_cast<uint32_t*>(&h1);
             }
           }
+          // only the stores wait for the slot: the loads of this K-block, possibly of the next tile, are already in
+          // flight while the consumers still multiply with the slot's previous K-block
+          TC_WAIT(BAR_A_FREE + as, aph ^ 1, 7);
 #if KMB_KO != 3
           // the row's 128 bytes of this K-block: 16-byte chunk c (features 8c .. 8c+7) at chunk position c ^ (row % 8)
           // (the 128-byte swizzle of a K-major wgmma operand; also spreads the warp's stores over all banks)
+          uint8_t* a_row = smem + L.a + as * A_KB_BYTES + row * 128;
 #pragma unroll
           for (int c = 0; c < 8; c++)
-            *reinterpret_cast<uint4*>(a_row + kb * A_KB_BYTES + ((c ^ (row & 7)) << 4)) =
+            *reinterpret_cast<uint4*>(a_row + ((c ^ (row & 7)) << 4)) =
                 make_uint4(pk[4 * c], pk[4 * c + 1], pk[4 * c + 2], pk[4 * c + 3]);
 #else
           (void)pk;
@@ -1008,22 +1017,22 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
           }
           ptx::fence_proxy_async_smem();   // the generic-proxy stores above are read by wgmma (async proxy)
           __syncwarp();
-          if (lane == 0) ptx::mbar_arrive(&bars[BAR_A_FULL + abuf * MAX_NKB + kb]);
+          if (lane == 0) ptx::mbar_arrive(&bars[BAR_A_FULL + as]);
+          if (++as == ASLOTS) { as = 0; aph ^= 1; }
         }
       }
     }
   } else if (warp >= FIRST_EPI_WARP && warp < FIRST_EPI_WARP + N_EPI_WARPS) {
     // ================================ consumers: wgmma + epilogue ================================
     // Warpgroup g multiplies rows g*64 .. g*64+63 of the tile with all 128 columns of an n-tile; its warp wq holds the
-    // accumulators of rows g*64 + wq*16 .. +15.  After regrouping, each lane owns one row and one 64-column half of
-    // every n-tile: through the buffer, lane l takes row g*64 + wq*16 + l % 16 and half l / 16; with quad shuffles
-    // (D > 256), lane l takes the row it already holds, g*64 + wq*16 + l / 4 + 8 * (l % 2), and half (l % 4) / 2.
+    // accumulators of rows g*64 + wq*16 .. +15.  After regrouping with quad shuffles, each lane owns one row and one
+    // 64-column half of every n-tile: lane l takes the row it already holds, g*64 + wq*16 + l / 4 + 8 * (l % 2), and
+    // half (l % 4) / 2.
     const int e = warp - FIRST_EPI_WARP;       // 0..7
     const int g = e >> 2, wq = e & 3;
-    const int h = WIDE ? (lane & 3) >> 1 : lane >> 4;   // column half of every 128-column n-tile
-    const int row = g * 64 + wq * 16 + (WIDE ? (lane >> 2) + 8 * (lane & 1) : lane & 15);
+    const int h = (lane & 3) >> 1;             // column half of every 128-column n-tile
+    const int row = g * 64 + wq * 16 + (lane >> 2) + 8 * (lane & 1);
     const int slot = h * TM + row;             // 0..255
-    float* xp = reinterpret_cast<float*>(smem + L.xpose + e * XPOSE_WARP_BYTES);   // (not used when WIDE)
     // K-major 128-byte-swizzled operands: 8-row groups 1024 bytes apart; +32 bytes (2 in the address field) per K=16
     const uint64_t adesc0 = ptx::make_smem_desc(ptx::smem_u32(smem + L.a + g * (64 * 128)), 16, 1024, 1);
     const uint64_t bdesc0 = ptx::make_smem_desc(ptx::smem_u32(smem + L.b), 16, 1024, 1);
@@ -1032,6 +1041,7 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
     const uint64_t aug_bd0 = ptx::make_smem_desc(ptx::smem_u32(smem + L.aug_b), TN * 16, 128, 0);
     uint32_t bs = 0, bph = 0;                  // B ring stage / phase
     uint32_t a_ready_si = 0xFFFFFFFFu;         // segment whose A operand this warp has already waited for
+    uint32_t a0 = 0, aph0 = 0;                 // A ring slot and phase of the current segment's first K-block
     const float cmax = p.stats->cmax, dcmax = p.stats->dcmax;
     const float mun = MODE == 2 ? 0.f : p.stats->mun;
     const float knn_extra = MODE == 2 ? p.stats->knn_extra : 0.f;
@@ -1090,31 +1100,40 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
         const int n = static_cast<int>(it.cur);
         const int buf = ac % AUGB;
         const uint32_t aph = (ac / AUGB) & 1;
-        const uint32_t abuf = si % NBUF;
         const bool need_a = a_ready_si != si;      // first n-tile of this segment
+        const bool free_a = it.seg_last();         // last n-tile of this segment: release each A slot once read
         a_ready_si = si;
         __syncwarp();                              // wgmma is .aligned: the warp issues it converged
         float acc[64];
+        uint32_t sa_prev = 0;                      // A slot of the previous K-block
 #pragma unroll
         for (int kb = 0; kb < NKB; kb++) {
-          if (need_a) TC_WAIT(BAR_A_FULL + abuf * MAX_NKB + kb, (si / NBUF) & 1, 4);
+          // K-block kb of the segment sits in slot a0 + kb of the ring (at most one wrap: NKB <= ASLOTS)
+          const bool wrap = a0 + kb >= static_cast<uint32_t>(ASLOTS);
+          const uint32_t sa = wrap ? a0 + kb - ASLOTS : a0 + kb;
+          if (need_a) TC_WAIT(BAR_A_FULL + sa, wrap ? aph0 ^ 1 : aph0, 4);
           TC_WAIT(BAR_B_FULL + bs, bph, 5);
           __syncwarp();
 #if KMB_KO != 2
           ptx::wgmma_fence_acc(acc);
           ptx::wgmma_fence();
-          const uint64_t ad = adesc0 + (((abuf * NKB + kb) * A_KB_BYTES) >> 4);
+          const uint64_t ad = adesc0 + ((sa * A_KB_BYTES) >> 4);
           const uint64_t bd = bdesc0 + ((bs * B_STAGE_BYTES) >> 4);
 #pragma unroll
           for (int k = 0; k < 4; k++) ptx::wgmma_m64n128k16(acc, ad + 2 * k, bd + 2 * k, (kb | k) ? 1u : 0u);
           ptx::wgmma_commit();
           ptx::wgmma_fence_acc(acc);
 #endif
-          // the previous K-block's group has retired once at most one group is pending: release its B stage
+          // the previous K-block's group has retired once at most one group is pending: release its B stage (and,
+          // in the segment's last n-tile, its A slot)
           if (kb > 0) {
             ptx::wgmma_wait<1>();
-            if (lane == 0) ptx::mbar_arrive(&bars[BAR_B_EMPTY + (bs ? bs - 1 : BST - 1)]);
+            if (lane == 0) {
+              ptx::mbar_arrive(&bars[BAR_B_EMPTY + (bs ? bs - 1 : BST - 1)]);
+              if (free_a) ptx::mbar_arrive(&bars[BAR_A_FREE + sa_prev]);
+            }
           }
+          sa_prev = sa;
           if (++bs == BST) { bs = 0; bph ^= 1; }
         }
         // bias step: acc += ones(64x16) * bias(128x16)^T  (both operands no-swizzle K-major smem blocks)
@@ -1133,39 +1152,16 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
         if (lane == 0) {
           ptx::mbar_arrive(&bars[BAR_B_EMPTY + (bs ? bs - 1 : BST - 1)]);
           ptx::mbar_arrive(&bars[BAR_AUG_EMPTY + buf]);
-          if (it.seg_last()) ptx::mbar_arrive(&bars[BAR_A_FREE + abuf]);   // the converters may refill the A buffer
+          if (free_a) ptx::mbar_arrive(&bars[BAR_A_FREE + sa_prev]);
         }
-        // regroup: acc[j*4 + hh*2 + e2] is (row wq*16 + hh*8 + lane/4, column 8j + 2*(lane%4) + e2); four rounds through
-        // the warp's buffer, each moving 16 columns of both halves, give this thread columns h*64 .. h*64+63 of its row
+        if (free_a) {   // the next segment starts NKB slots further on
+          a0 += NKB;
+          if (a0 >= static_cast<uint32_t>(ASLOTS)) { a0 -= ASLOTS; aph0 ^= 1; }
+        }
+        // regroup: this thread gets columns h*64 .. h*64+63 of its row (quad shuffles, see regroup_quad)
         uint32_t r0[32], r1[32];
 #if KMB_KO != 1
-        if (WIDE) regroup_quad(acc, lane, r0, r1);
-        else
-#pragma unroll
-        for (int ps = 0; ps < 4; ps++) {
-#pragma unroll
-          for (int hf = 0; hf < 2; hf++)
-#pragma unroll
-            for (int jj = 0; jj < 2; jj++)
-#pragma unroll
-              for (int hh = 0; hh < 2; hh++) {
-                const int j = hf * 8 + ps * 2 + jj;
-                *reinterpret_cast<float2*>(xp + (hh * 8 + (lane >> 2)) * XPOSE_STRIDE + hf * 16 + jj * 8 + 2 * (lane & 3)) =
-                    make_float2(acc[j * 4 + hh * 2], acc[j * 4 + hh * 2 + 1]);
-              }
-          __syncwarp();
-          const float4* src = reinterpret_cast<const float4*>(xp + (lane & 15) * XPOSE_STRIDE + h * 16);
-          uint32_t* dst = (ps < 2 ? r0 : r1) + (ps & 1) * 16;
-#pragma unroll
-          for (int c = 0; c < 4; c++) {
-            const float4 v = src[c];
-            dst[4 * c] = __float_as_uint(v.x);
-            dst[4 * c + 1] = __float_as_uint(v.y);
-            dst[4 * c + 2] = __float_as_uint(v.z);
-            dst[4 * c + 3] = __float_as_uint(v.w);
-          }
-          __syncwarp();
-        }
+        regroup_quad(acc, lane, r0, r1);
 #else
         for (int jj = 0; jj < 32; jj++) {   // stand-in values: strictly decreasing, 64 apart -> one candidate per row
           r0[jj] = __float_as_uint(-64.f * static_cast<float>(n * 128 + h * 64 + jj + 1));
@@ -1223,7 +1219,7 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
             mmax = fmaxf(mmax, margin);
             if (p.knn_first_pass && seg == 1) {
               // threshold sweep done: both column halves of the row adopt the merged top-kk (the partner half is
-              // lane ^ 16 of the same warp)
+              // lane ^ 2 of the same warp)
               float mg[KNN_MAX_KK];
               __syncwarp();
               knn_select_buckets(topk + 16 * 256, reinterpret_cast<float*>(smem + L.list) + ((1 - h) * TM + row) + 16 * 256,
