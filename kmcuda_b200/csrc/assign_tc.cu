@@ -14,10 +14,11 @@
 //   consumer warps  : two warpgroups, one per 64-row half of the tile; each issues wgmma m64n128k16 (A and B
 //                     from shared memory, fp32 accumulators in its registers) over every K-block, plus one
 //                     extra K=16 step that adds -||c||^2/2 as three fp16 terms against constant ones, so
-//                     acc = x.c - ||c||^2/2.  The accumulator fragment is regrouped with quad shuffles so
-//                     that every thread holds 64 consecutive columns of one row; then
-//                     the running row maximum M is updated and every column whose value is within `margin`
-//                     of M is recorded (bit mask per 32-column chunk); margin is a rigorous bound on
+//                     acc = x.c - ||c||^2/2.  The epilogue works on the accumulator fragment as it lands: a
+//                     lane holds 32 columns of each of two rows, and the four lanes of a quad hold all 128
+//                     columns of their rows.  The running row maximum M is updated (quad all-reduce of the
+//                     lanes' chunk maxima) and every column whose value is within `margin` of M is recorded (a
+//                     32-bit mask per row and lane, decoded into columns by the emitters); margin is a rigorous bound on
 //                     |approx - exact| derived from the actual rounding residuals (Cauchy-Schwarz), so the
 //                     reference's fp32 winner is guaranteed to be among the recorded candidates.
 //   rows with one candidate are final; rows with several go to the exact re-check queue; rows with
@@ -69,7 +70,9 @@ constexpr int B_KB_BYTES = TN * 128;    // one K-block of the centroid tile: 16 
 constexpr int B_STAGE_BYTES = B_KB_BYTES;
 constexpr int AUG_A_BYTES = TM * 32;    // 4 KiB  (K=16 fp16, no swizzle)
 constexpr int AUG_B_BYTES = TN * 32;    // 4 KiB
-constexpr int LIST_LEN = 5;             // entries per epilogue thread: one per n-tile that held a candidate (max, 2 x 32-bit mask, n-tile)
+constexpr int LIST_LEN = 5;             // entries per epilogue thread: one per n-tile in which one of its two rows held a
+                                        // candidate (2 x row maximum, 2 x 32-bit mask, 16-bit n-tile)
+constexpr int LIST_ARRAYS = 4;
 // Knock-out builds (timing experiments only, results are garbage): 1 = the epilogue does not read the accumulators,
 // 2 = no MMA is issued, 3 = converters do no work, 5 = the B / bias copies are not issued, 7 = the epilogue loads the
 // accumulators but skips the ALU work on them.  Which of them shortens the kernel says what bounds it.
@@ -106,7 +109,11 @@ struct Stats {       // written by the centroid prep kernels, read by the main k
   float knn_extra;      // k-NN, angular metric served through the L2 pass: s^2 * max |1 - ||y||^2| (see tc_knn_search)
 };
 
-constexpr uint32_t LIST_ARRAY = 2 * LIST_LEN * 256 * 4;   // bytes of one of the four list arrays (both tile parities)
+constexpr uint32_t LIST_ARRAY = 2 * LIST_LEN * 256 * 4;   // bytes of one of the four 32-bit list arrays (both tile parities)
+constexpr uint32_t LIST_NT_BYTES = 2 * LIST_LEN * 256 * 2; // the n-tile array (16 bit: nt <= 16383, see tc_supported)
+// per-tile state in the fin region, in words from the parity's base: M, margin, M2 per row; per epilogue thread its list
+// length (bits 0-7) and flags (R0 in bits 8-15, R1 in bits 16-23)
+enum { FIN_M = 0, FIN_MARGIN = TM, FIN_M2 = 2 * TM, FIN_STATE = 3 * TM, FIN_WORDS = 3 * TM + 256 };
 struct SmemLayout {  // byte offsets from the 1024-aligned dynamic smem base
   uint32_t a, b, aug_a, aug_b, list, norms, fin, mu, bars, total;
 };
@@ -132,18 +139,18 @@ __host__ __device__ constexpr SmemLayout smem_layout(int nkb) {
   L.b = o; o += b_stages(nkb) * B_STAGE_BYTES;
   L.aug_a = o; o += AUG_A_BYTES;
   L.aug_b = o; o += aug_bufs(nkb) * AUG_B_BYTES;
-  // candidate lists: 4 arrays (entry maximum | mask of columns 0-31 | mask of columns 32-63 | n-tile) of
-  // [tile parity][entry][epilogue thread] words, LIST_ARRAY bytes apart.  MODE 2 reuses [list, norms) as its top-kk /
-  // bucket scratch: 48 rows x 256 x 4 bytes (static_assert below)
-  L.list = o; o += 4 * LIST_ARRAY;
-  L.fin = o; o += 2 * 5 * 256 * 4;    // [tile parity][M|cnt|flags|margin|M2][epilogue thread]
+  // candidate lists (MODE 0 / 1): 4 arrays (maximum of row R0 | of row R1 | mask of R0 | mask of R1) of
+  // [tile parity][entry][epilogue thread] words, LIST_ARRAY bytes apart, then the n-tiles as 16-bit [parity][entry][thread].
+  // MODE 2 reuses [list, norms) as its top-kk / bucket scratch: 48 rows x 256 x 4 bytes (static_assert below)
+  L.list = o; o += LIST_ARRAYS * LIST_ARRAY + LIST_NT_BYTES;
+  L.fin = o; o += 2 * FIN_WORDS * 4;  // [tile parity][FIN_*]
   L.norms = o; o += norm_depth(nkb) * 4 * TM * 4;   // [segment % depth][x|d][row]  x~^2 | residual^2 | (k-NN) exact s^2|x-c|^2 | (k-NN) s^2(|x|+|c|)^2
   L.mu = o; o += MAX_NKB * KB * 4;    // -mu * s per feature (zero padded): the converters' centring term
   L.bars = o; o += 64 * 8;
   L.total = o;
   return L;
 }
-static_assert(4 * LIST_ARRAY + 2 * 5 * 256 * 4 >= 48 * 256 * 4, "k-NN scratch overlaps the norms");
+static_assert(LIST_ARRAYS * LIST_ARRAY + LIST_NT_BYTES + 2 * FIN_WORDS * 4 >= 48 * 256 * 4, "k-NN scratch overlaps the norms");
 __host__ __device__ constexpr bool layouts_fit() {
   for (int k = 1; k <= MAX_NKB; k++)
     if (smem_layout(k).total + 1024 > 232448 || a_slots(k) < k || a_slots(k) > MAX_NKB || norm_depth(k) * k <= a_slots(k))
@@ -679,20 +686,19 @@ __device__ __forceinline__ uint32_t commit_assignment(uint32_t* __restrict__ ass
   return 1u;
 }
 
-// in-place compaction of one epilogue thread's chunk list: entries whose chunk maximum fell below the
-// current threshold can never hold a candidate (the threshold only rises)
-__device__ __forceinline__ uint32_t compact_list(uint32_t* lst, uint32_t cnt, float thr) {
-  // lst = this thread's column of the entry arrays (stride 256 words per entry, LIST_ARRAY bytes between arrays)
+// in-place compaction of one epilogue thread's list: an entry whose chunk maxima of both rows fell below their rows'
+// current thresholds can never hold a candidate (the thresholds only rise)
+__device__ __forceinline__ uint32_t compact_list(uint32_t* lst, uint16_t* lnt, uint32_t cnt, float thr0, float thr1) {
+  // lst / lnt = this thread's column of the entry arrays / of the n-tiles (stride 256 per entry, LIST_ARRAY bytes
+  // between arrays)
   constexpr uint32_t A = LIST_ARRAY / 4;
   uint32_t w = 0;
+#pragma unroll 1
   for (uint32_t i = 0; i < cnt; i++) {
-    const uint32_t cmb = lst[i * 256];
-    if (__uint_as_float(cmb) >= thr) {
+    if (__uint_as_float(lst[i * 256]) >= thr0 || __uint_as_float(lst[A + i * 256]) >= thr1) {
       if (w != i) {
-        lst[w * 256] = cmb;
-        lst[A + w * 256] = lst[A + i * 256];
-        lst[2 * A + w * 256] = lst[2 * A + i * 256];
-        lst[3 * A + w * 256] = lst[3 * A + i * 256];
+        for (int k = 0; k < LIST_ARRAYS; k++) lst[k * A + w * 256] = lst[k * A + i * 256];
+        lnt[w * 256] = lnt[i * 256];
       }
       w++;
     }
@@ -772,6 +778,7 @@ __device__ __noinline__ uint32_t knn_append(uint4* ent, uint32_t cnt, float kth,
   return cnt + 1;
 }
 
+// MODE 2 / 3 only (their epilogues take maxima over 4 consecutive columns and fold group runs of a 64-column half).
 // Regrouping of one warp's m64n128 accumulator fragment without shared memory: acc[j*4 + hh*2 + e] is (row
 // hh*8 + lane/4, column 8j + 2t + e) with t = lane % 4.  The four lanes of a quad hold the same two rows; lane t takes
 // combination c = t of (row hh = c % 2, half c / 2) and receives its 16 columns from each quad partner s (columns
@@ -1025,14 +1032,18 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
   } else if (warp >= FIRST_EPI_WARP && warp < FIRST_EPI_WARP + N_EPI_WARPS) {
     // ================================ consumers: wgmma + epilogue ================================
     // Warpgroup g multiplies rows g*64 .. g*64+63 of the tile with all 128 columns of an n-tile; its warp wq holds the
-    // accumulators of rows g*64 + wq*16 .. +15.  After regrouping with quad shuffles, each lane owns one row and one
-    // 64-column half of every n-tile: lane l takes the row it already holds, g*64 + wq*16 + l / 4 + 8 * (l % 2), and
-    // half (l % 4) / 2.
+    // accumulators of rows g*64 + wq*16 .. +15.  MODE 0 / 1 run the epilogue on that fragment as it lands: lane l holds
+    // rows R0 = g*64 + wq*16 + l / 4 and R1 = R0 + 8 at columns 8j + 2t + e (t = l % 4, j < 16, e < 2), so the four
+    // lanes of a quad hold all 128 columns of their two rows.  MODE 2 / 3 regroup the fragment with quad shuffles
+    // first: each lane then owns one row and one 64-column half of every n-tile, lane l takes the row it already
+    // holds, g*64 + wq*16 + l / 4 + 8 * (l % 2), and half (l % 4) / 2.
     const int e = warp - FIRST_EPI_WARP;       // 0..7
     const int g = e >> 2, wq = e & 3;
-    const int h = (lane & 3) >> 1;             // column half of every 128-column n-tile
+    const int h = (lane & 3) >> 1;             // MODE 2 / 3: column half of every 128-column n-tile
     const int row = g * 64 + wq * 16 + (lane >> 2) + 8 * (lane & 1);
     const int slot = h * TM + row;             // 0..255
+    const int qrow = g * 64 + wq * 16 + (lane >> 2);   // MODE 0 / 1: R0
+    const int lid = e * 32 + lane;                     // MODE 0 / 1: this thread's column of the lists, 0..255
     // K-major 128-byte-swizzled operands: 8-row groups 1024 bytes apart; +32 bytes (2 in the address field) per K=16
     const uint64_t adesc0 = ptx::make_smem_desc(ptx::smem_u32(smem + L.a + g * (64 * 128)), 16, 1024, 1);
     const uint64_t bdesc0 = ptx::make_smem_desc(ptx::smem_u32(smem + L.b), 16, 1024, 1);
@@ -1042,9 +1053,6 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
     uint32_t bs = 0, bph = 0;                  // B ring stage / phase
     uint32_t a_ready_si = 0xFFFFFFFFu;         // segment whose A operand this warp has already waited for
     uint32_t a0 = 0, aph0 = 0;                 // A ring slot and phase of the current segment's first K-block
-    const float cmax = p.stats->cmax, dcmax = p.stats->dcmax;
-    const float mun = MODE == 2 ? 0.f : p.stats->mun;
-    const float knn_extra = MODE == 2 ? p.stats->knn_extra : 0.f;
     // cosine: every dot >= 1 is clamped to angle 0 by the reference, so all of them tie -> the threshold
     // never rises above s^2 * 1 (the accumulator holds s^2 * dot)
     const float cap = p.metric == 1 ? p.stats->scale * p.stats->scale : INFINITY;
@@ -1052,12 +1060,19 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
     for (uint32_t tile = tile_begin; tile < tile_end; tile += gridDim.x) {
       if (MODE == 2 && p.knn_nblk[tile] == 0) continue;
       const int par = ti & 1;
-      uint32_t* lst = reinterpret_cast<uint32_t*>(smem + L.list) + par * LIST_LEN * 256 + slot;   // this thread's entries
-      float* fin = reinterpret_cast<float*>(smem + L.fin) + par * 5 * 256;
+      uint32_t* lst = reinterpret_cast<uint32_t*>(smem + L.list) + par * LIST_LEN * 256 + lid;   // this thread's entries
+      uint16_t* lnt = reinterpret_cast<uint16_t*>(smem + L.list + LIST_ARRAYS * LIST_ARRAY) + par * LIST_LEN * 256 + lid;
+      float* fin = reinterpret_cast<float*>(smem + L.fin) + par * FIN_WORDS;
       // the emitter warps must have consumed this parity's lists (tile ti-2)
       if (MODE < 2) TC_WAIT(BAR_EMIT_EMPTY + par, ((ti >> 1) & 1) ^ 1, 11);
-      float M = -INFINITY, M2 = -INFINITY, margin = 0.f;   // M2: MODE 1, second largest chunk maximum
-      uint32_t cnt = 0, flags = 0;
+      float M = -INFINITY, margin = 0.f;   // MODE 2 / 3
+      // MODE 0 / 1, per row R0 / R1 (the same in the four lanes of a quad): running maximum and MODE 1 lower bound of
+      // the second best score.  The rest of the state lives in fin, where the emitters read it, rather than in registers
+      // across the n-tile loop: the row margins, this thread's list length and its flags (FIN_STATE).
+      float Mr[2] = {-INFINITY, -INFINITY}, M2r[2] = {-INFINITY, -INFINITY};
+      uint32_t* const fst = reinterpret_cast<uint32_t*>(fin) + FIN_STATE + lid;
+      if (MODE < 2) *fst = 0u;
+      uint32_t cnt = 0, flags = 0;       // MODE 2 / 3
       // MODE 2: this half-row's persistent state (global) and its top-kk column (the list_cm region is free)
       float* topk = reinterpret_cast<float*>(smem + L.list) + slot;   // [kk][256], kk <= 16 rows of the scratch
       uint32_t kslot = 0;
@@ -1158,63 +1173,80 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
           a0 += NKB;
           if (a0 >= static_cast<uint32_t>(ASLOTS)) { a0 -= ASLOTS; aph0 ^= 1; }
         }
-        // regroup: this thread gets columns h*64 .. h*64+63 of its row (quad shuffles, see regroup_quad)
-        uint32_t r0[32], r1[32];
-#if KMB_KO != 1
-        regroup_quad(acc, lane, r0, r1);
-#else
-        for (int jj = 0; jj < 32; jj++) {   // stand-in values: strictly decreasing, 64 apart -> one candidate per row
-          r0[jj] = __float_as_uint(-64.f * static_cast<float>(n * 128 + h * 64 + jj + 1));
-          r1[jj] = __float_as_uint(-64.f * static_cast<float>(n * 128 + h * 64 + 32 + jj + 1));
-        }
+#if KMB_KO == 1
+        if (MODE < 2)   // stand-in values: strictly decreasing along the row, 64 apart -> one candidate per row
+#pragma unroll
+          for (int j = 0; j < 16; j++)
+#pragma unroll
+            for (int q = 0; q < 4; q++)
+              acc[j * 4 + q] = -64.f * static_cast<float>(n * TN + 8 * j + 2 * (lane & 3) + (q & 1) + 1);
 #endif
         if (it.seg_first()) {
           const float* norms = reinterpret_cast<const float*>(smem + L.norms) + (si % NDEPTH) * 4 * TM;
-          // rigorous bound on |acc - (s^2 x.c - s^2||c||^2/2)| (see header): Cauchy-Schwarz on the
+          // (loaded here, once per segment, rather than held in registers across the n-tile loop)
+          const float cmax = p.stats->cmax, dcmax = p.stats->dcmax;
+          const float mun = MODE == 2 ? 0.f : p.stats->mun;
+          const float knn_extra = MODE == 2 ? p.stats->knn_extra : 0.f;
+          // rigorous bound on |acc - (s^2 x.c - s^2||c||^2/2)| of tile row r (see header): Cauchy-Schwarz on the
           // actual rounding residuals + accumulation + the reference's own rounding slack
-          float nx, nd;
-          if (MEASURED_RESIDUAL) {
-            nx = __fsqrt_ru(norms[row]) * 1.0001f;
-            nd = __fsqrt_ru(norms[TM + row]) * 1.0001f;
+          auto row_margin = [&](int r, uint32_t& fl) {
+            float nx, nd;
+            if (MEASURED_RESIDUAL) {
+              nx = __fsqrt_ru(norms[r]) * 1.0001f;
+              nd = __fsqrt_ru(norms[TM + r]) * 1.0001f;
+            } else {
+              // norms[r] = |a|^2 (fp32 sum, relative error < 1e-4): |a - x~| <= 2^-11 |a| + sqrt(Dp) 2^-25, |x~| <= |a| + |a - x~|
+              const float na = __fsqrt_ru(norms[r]) * 1.0001f;
+              nd = na * 4.8834e-4f + __fsqrt_ru(static_cast<float>(p.nkb * KB)) * 2.99e-8f;
+              nx = na + nd;
+              // an element beyond the fp16 range would have become Inf in the operand: such rows take the exact pass
+              if (!(na < 65000.f)) fl |= 1u;
+            }
+            const float xn = nx + nd;
+            float E = nx * dcmax + nd * cmax + nd * dcmax;
+            E += static_cast<float>(p.nkb * KB + 16) * 2.4e-7f * nx * cmax;   // fp32 accumulation in the tensor core
+            // reference Kahan/rd rounding + bias split + fp32 centring of both operands: the reference works on the
+            // UNCENTRED vectors, whose norms are bounded by the centred ones + ||mu||
+            const float xu = xn + mun, cu = cmax + mun;
+            if (MODE == 0) {
+              // the reference ranks with fma_rd(-2, Kahan dot, csq): |error| <= 1.2e-7 cu^2 + 2.4e-7 xu cu in score units
+              // (2^-23 per directed rounding, Kahan sums to ~1 ulp); 2.5x - 5x of that is allowed for
+              E += 6.0e-7f * (cu * cu + xu * cu);
+            } else if (MODE == 2) {
+              E += 2.0e-6f * (cu * cu + xu * cu) + 2.0e-6f * xu * xu;
+            } else {
+              // MODE 1 / 3 decide on TRUE distances sqrt(Kahan sum (x - c)^2): their rounding is relative to |x - c|^2 <=
+              // (|x^| + |c^|)^2 (the subtraction cancels the common offset exactly), plus the fp32 centring of both operands
+              E += 2.0e-6f * (xn + cmax) * (xn + cmax) + 2.4e-7f * (xn * cmax + cmax * cmax);
+            }
+            if (MODE == 3) {
+              xa2lo = norms[r] * (1.f - 1.0e-4f);                          // lower bound of |s (x - mu)|^2 (fp32 summation error)
+              // scores this low are not separable from the padding sentinel (-65504): such rows take the exact pass
+              if (!(nx * cmax < 6.0e4f)) fl |= 1u;
+            }
+            if (MODE == 2) {
+              goff = 0.5f * norms[2 * TM + r];
+              // centring x - c_B and y - c_B rounds in fp32 (relative to |x|+|c|), and the row constant is subtracted
+              // from scores of its own magnitude
+              E += 1.2e-7f * (__fsqrt_ru(norms[3 * TM + r]) * cmax + p.stats->yabs * xn) + 4.8e-7f * (goff + xn * cmax);
+            }
+            float mg = 2.f * E * 1.001f + 1e-30f;
+            if (MODE == 2) mg += knn_extra;
+            if (!(mg < 1.0e30f)) fl |= 1u;                                  // NaN / Inf somewhere in the row
+            return mg;
+          };
+          if (MODE < 2) {
+#pragma unroll
+            for (int hh = 0; hh < 2; hh++) {
+              uint32_t fl = 0;
+              const float mg = row_margin(qrow + 8 * hh, fl);
+              if ((lane & 3) == 0) fin[FIN_MARGIN + qrow + 8 * hh] = mg;
+              *fst |= fl << (8 + 8 * hh);
+            }
+            __syncwarp();
           } else {
-            // norms[row] = |a|^2 (fp32 sum, relative error < 1e-4): |a - x~| <= 2^-11 |a| + sqrt(Dp) 2^-25, |x~| <= |a| + |a - x~|
-            const float na = __fsqrt_ru(norms[row]) * 1.0001f;
-            nd = na * 4.8834e-4f + __fsqrt_ru(static_cast<float>(p.nkb * KB)) * 2.99e-8f;
-            nx = na + nd;
-            // an element beyond the fp16 range would have become Inf in the operand: such rows take the exact pass
-            if (!(na < 65000.f)) flags |= 1u;
+            margin = row_margin(row, flags);
           }
-          const float xn = nx + nd;
-          float E = nx * dcmax + nd * cmax + nd * dcmax;
-          E += static_cast<float>(p.nkb * KB + 16) * 2.4e-7f * nx * cmax;   // fp32 accumulation in the tensor core
-          // reference Kahan/rd rounding + bias split + fp32 centring of both operands: the reference works on the
-          // UNCENTRED vectors, whose norms are bounded by the centred ones + ||mu||
-          const float xu = xn + mun, cu = cmax + mun;
-          if (MODE == 0) {
-            // the reference ranks with fma_rd(-2, Kahan dot, csq): |error| <= 1.2e-7 cu^2 + 2.4e-7 xu cu in score units
-            // (2^-23 per directed rounding, Kahan sums to ~1 ulp); 2.5x - 5x of that is allowed for
-            E += 6.0e-7f * (cu * cu + xu * cu);
-          } else if (MODE == 2) {
-            E += 2.0e-6f * (cu * cu + xu * cu) + 2.0e-6f * xu * xu;
-          } else {
-            // MODE 1 / 3 decide on TRUE distances sqrt(Kahan sum (x - c)^2): their rounding is relative to |x - c|^2 <=
-            // (|x^| + |c^|)^2 (the subtraction cancels the common offset exactly), plus the fp32 centring of both operands
-            E += 2.0e-6f * (xn + cmax) * (xn + cmax) + 2.4e-7f * (xn * cmax + cmax * cmax);
-          }
-          if (MODE == 3) {
-            xa2lo = norms[row] * (1.f - 1.0e-4f);                          // lower bound of |s (x - mu)|^2 (fp32 summation error)
-            // scores this low are not separable from the padding sentinel (-65504): such rows take the exact pass
-            if (!(nx * cmax < 6.0e4f)) flags |= 1u;
-          }
-          if (MODE == 2) {
-            goff = 0.5f * norms[2 * TM + row];
-            // centring x - c_B and y - c_B rounds in fp32 (relative to |x|+|c|), and the row constant is subtracted
-            // from scores of its own magnitude
-            E += 1.2e-7f * (__fsqrt_ru(norms[3 * TM + row]) * cmax + p.stats->yabs * xn) + 4.8e-7f * (goff + xn * cmax);
-          }
-          margin = 2.f * E * 1.001f + 1e-30f;
-          if (MODE == 2) margin += knn_extra;
-          if (!(margin < 1.0e30f)) flags |= 1u;                            // NaN / Inf somewhere in the row
           if (MODE == 2) {
             mmax = fmaxf(mmax, margin);
             if (p.knn_first_pass && seg == 1) {
@@ -1230,12 +1262,108 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
             }
           }
         }
+        if (MODE < 2) {
+          // Lloyd / Yinyang candidate epilogue on the fragment as it lands: mask bit b = 2j + e of row hh (R0 / R1) is
+          // acc[j*4 + hh*2 + e], column 8j + 2t + e of the n-tile.  Any fixed column order would do: the running row
+          // maximum and the "within margin" bits do not depend on it, and the emitter decodes bits into columns.
 #ifdef KMB_DEBUG_SCORES   // bring-up builds only: 64 stores per n-tile bloat the hot loop's instruction footprint
-        if (MODE == 0 && p.dbg_scores) {
-          const uint64_t grow = static_cast<uint64_t>(tile) * TM + row;
-          float* dst = p.dbg_scores + grow * (static_cast<uint64_t>(nt) * TN) + n * TN + h * 64;
-          for (int jj = 0; jj < 32; jj++) dst[jj] = __uint_as_float(r0[jj]);
-          for (int jj = 0; jj < 32; jj++) dst[32 + jj] = __uint_as_float(r1[jj]);
+          if (MODE == 0 && p.dbg_scores)
+            for (int hh = 0; hh < 2; hh++) {
+              const uint64_t grow = static_cast<uint64_t>(tile) * TM + qrow + 8 * hh;
+              float* dst = p.dbg_scores + grow * (static_cast<uint64_t>(nt) * TN) + n * TN + 2 * (lane & 3);
+              for (int j = 0; j < 16; j++) {
+                dst[8 * j] = acc[j * 4 + hh * 2];
+                dst[8 * j + 1] = acc[j * 4 + hh * 2 + 1];
+              }
+            }
+#endif
+          if (it.seg_last()) si++;
+#if KMB_KO == 7
+          if (MODE == 0) {   // timing build: the accumulators are loaded, the ALU work on them is skipped
+            uint32_t x0 = 0, x1 = 0;
+#pragma unroll
+            for (int j = 0; j < 16; j += 4) { x0 ^= __float_as_uint(acc[j * 4]); x1 ^= __float_as_uint(acc[j * 4 + 2]); }
+            Mr[0] = fmaxf(Mr[0], __uint_as_float(x0 & 0x3fffffffu));
+            Mr[1] = fmaxf(Mr[1], __uint_as_float(x1 & 0x3fffffffu));
+            continue;
+          }
+#endif
+          float cm[2], thr[2];    // this lane's chunk maximum (32 columns) and the row's threshold
+          uint32_t mask[2];
+#pragma unroll
+          for (int hh = 0; hh < 2; hh++) {
+            auto v = [&](int b) { return acc[(b >> 1) * 4 + hh * 2 + (b & 1)]; };
+            // chunk maximum with three-input maxima: 15 instructions per 32 columns
+            float u[10];
+#pragma unroll
+            for (int i = 0; i < 10; i++) u[i] = ptx::fmax3(v(3 * i), v(3 * i + 1), v(3 * i + 2));
+            cm[hh] = fmaxf(ptx::fmax3(ptx::fmax3(u[0], u[1], u[2]), ptx::fmax3(u[3], u[4], u[5]), ptx::fmax3(u[6], u[7], u[8])),
+                           ptx::fmax3(u[9], v(30), v(31)));
+            if (MODE == 0) {
+              // quad all-reduce: the running maximum of the whole row
+              float qm = fmaxf(cm[hh], __shfl_xor_sync(0xffffffffu, cm[hh], 1));
+              qm = fmaxf(qm, __shfl_xor_sync(0xffffffffu, qm, 2));
+              Mr[hh] = fmaxf(Mr[hh], qm);
+              thr[hh] = fminf(Mr[hh], cap) - fin[FIN_MARGIN + qrow + 8 * hh];
+            } else {
+              // (largest, second largest) of the quad's four chunk maxima, merged into the row's running pair.  The
+              // chunks of the four lanes and of different n-tiles are disjoint column sets, so two distinct columns
+              // reach the second value of the pair: M2 is a lower bound of the row's second best score.  (Merged
+              // over the quad rather than kept per lane: the lane's own pair is valid too, but looser.)
+              const float o = __shfl_xor_sync(0xffffffffu, cm[hh], 1);
+              const float a1 = fmaxf(cm[hh], o), a2 = fminf(cm[hh], o);
+              const float b1 = __shfl_xor_sync(0xffffffffu, a1, 2), b2 = __shfl_xor_sync(0xffffffffu, a2, 2);
+              const float q1 = fmaxf(a1, b1), q2 = fmaxf(fminf(a1, b1), fmaxf(a2, b2));
+              M2r[hh] = ptx::fmax3(M2r[hh], q2, fminf(Mr[hh], q1));
+              Mr[hh] = fmaxf(Mr[hh], q1);
+              thr[hh] = fminf(M2r[hh], cap) - fin[FIN_MARGIN + qrow + 8 * hh];
+            }
+            // candidate mask: d = v - thr as packed pairs, then the sign bits are shifted in with one funnel shift per
+            // column; bit (31 - b) of (c0 << 16 | c1) = sign of d_b = "bit b is below the threshold".  NaN scores only
+            // occur in rows whose margin is not finite (flag 1).
+            const uint64_t nthr2 = ptx::pack2(-thr[hh], -thr[hh]);
+            uint32_t c0 = 0, c1 = 0;   // two 16-column chains (shorter dependency chains)
+#pragma unroll
+            for (int j = 0; j < 16; j++) {
+              float x, y;
+              ptx::unpack2(ptx::fadd2(ptx::pack2(v(2 * j), v(2 * j + 1)), nthr2), x, y);
+              if (j < 8) {
+                c0 = __funnelshift_l(__float_as_uint(x), c0, 1);
+                c0 = __funnelshift_l(__float_as_uint(y), c0, 1);
+              } else {
+                c1 = __funnelshift_l(__float_as_uint(x), c1, 1);
+                c1 = __funnelshift_l(__float_as_uint(y), c1, 1);
+              }
+            }
+            mask[hh] = __brev(~((c0 << 16) | c1));
+          }
+          // one entry per n-tile in which either row holds a candidate in this lane's columns
+          if (mask[0] | mask[1]) {
+            constexpr uint32_t A = LIST_ARRAY / 4;
+            uint32_t st = *fst, c = st & 0xffu;
+            if (c >= LIST_LEN - 1) c = compact_list(lst, lnt, c, thr[0], thr[1]);   // rare: drop entries below the risen thresholds
+            if (c < LIST_LEN) {
+              lst[c * 256] = __float_as_uint(cm[0]);
+              lst[A + c * 256] = __float_as_uint(cm[1]);
+              lst[2 * A + c * 256] = mask[0];
+              lst[3 * A + c * 256] = mask[1];
+              lnt[c * 256] = static_cast<uint16_t>(n);
+              c++;
+            } else {
+              st |= (mask[0] ? 2u << 8 : 0u) | (mask[1] ? 2u << 16 : 0u);   // the row's candidate set is incomplete
+            }
+            *fst = (st & ~0xffu) | c;
+          }
+          continue;
+        }
+        // MODE 2 / 3: this thread gets columns h*64 .. h*64+63 of its row (quad shuffles, see regroup_quad)
+        uint32_t r0[32], r1[32];
+#if KMB_KO != 1
+        regroup_quad(acc, lane, r0, r1);
+#else
+        for (int jj = 0; jj < 32; jj++) {   // stand-in values: strictly decreasing, 64 apart -> one candidate per row
+          r0[jj] = __float_as_uint(-64.f * static_cast<float>(n * 128 + h * 64 + jj + 1));
+          r1[jj] = __float_as_uint(-64.f * static_cast<float>(n * 128 + h * 64 + 32 + jj + 1));
         }
 #endif
         if (MODE == 3) {
@@ -1288,20 +1416,9 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
           if (it.seg_last()) si++;
           continue;
         }
-        // chunk maxima with three-input maxima (FMNMX3): 16 instructions per 32 columns
-        float t0[8], t1[8];      // MODE 2 only: maxima of the 4-column groups
-        float cm0, cm1;
-#if KMB_KO == 7
-        if (MODE == 0) {   // timing build: the accumulators are loaded, the ALU work on them is skipped
-          uint32_t x0 = 0, x1 = 0;
-#pragma unroll
-          for (int jj = 0; jj < 32; jj += 8) { x0 ^= r0[jj]; x1 ^= r1[jj]; }
-          M = fmaxf(M, __uint_as_float(x0 & x1 & 0x3fffffffu));
-          if (it.seg_last()) si++;
-          continue;
-        }
-#endif
         if (MODE == 2) {
+          // MODE 2: maxima of the 4-column groups and of the two 32-column chunks
+          float t0[8], t1[8];
 #pragma unroll
           for (int i = 0; i < 8; i++) {
             t0[i] = fmaxf(fmaxf(__uint_as_float(r0[4 * i]), __uint_as_float(r0[4 * i + 1])),
@@ -1309,34 +1426,8 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
             t1[i] = fmaxf(fmaxf(__uint_as_float(r1[4 * i]), __uint_as_float(r1[4 * i + 1])),
                           fmaxf(__uint_as_float(r1[4 * i + 2]), __uint_as_float(r1[4 * i + 3])));
           }
-          cm0 = fmaxf(fmaxf(fmaxf(t0[0], t0[1]), fmaxf(t0[2], t0[3])), fmaxf(fmaxf(t0[4], t0[5]), fmaxf(t0[6], t0[7])));
-          cm1 = fmaxf(fmaxf(fmaxf(t1[0], t1[1]), fmaxf(t1[2], t1[3])), fmaxf(fmaxf(t1[4], t1[5]), fmaxf(t1[6], t1[7])));
-        } else {
-          float u0[10], u1[10];
-#pragma unroll
-          for (int i = 0; i < 10; i++) {
-            u0[i] = ptx::fmax3(__uint_as_float(r0[3 * i]), __uint_as_float(r0[3 * i + 1]), __uint_as_float(r0[3 * i + 2]));
-            u1[i] = ptx::fmax3(__uint_as_float(r1[3 * i]), __uint_as_float(r1[3 * i + 1]), __uint_as_float(r1[3 * i + 2]));
-          }
-          const float w00 = ptx::fmax3(u0[0], u0[1], u0[2]), w01 = ptx::fmax3(u0[3], u0[4], u0[5]);
-          const float w02 = ptx::fmax3(u0[6], u0[7], u0[8]), w03 = ptx::fmax3(u0[9], __uint_as_float(r0[30]), __uint_as_float(r0[31]));
-          const float w10 = ptx::fmax3(u1[0], u1[1], u1[2]), w11 = ptx::fmax3(u1[3], u1[4], u1[5]);
-          const float w12 = ptx::fmax3(u1[6], u1[7], u1[8]), w13 = ptx::fmax3(u1[9], __uint_as_float(r1[30]), __uint_as_float(r1[31]));
-          cm0 = fmaxf(ptx::fmax3(w00, w01, w02), w03);
-          cm1 = fmaxf(ptx::fmax3(w10, w11, w12), w13);
-        }
-        float thr;
-        if (MODE == 0) {
-          M = fmaxf(M, fmaxf(cm0, cm1));
-          thr = fminf(M, cap) - margin;
-        } else if (MODE == 1) {
-          // two distinct columns reach min(two largest chunk maxima): a lower bound of the second best score
-          M2 = fmaxf(M2, fminf(M, cm0));
-          M = fmaxf(M, cm0);
-          M2 = fmaxf(M2, fminf(M, cm1));
-          M = fmaxf(M, cm1);
-          thr = fminf(M2, cap) - margin;
-        } else {
+          const float cm0 = fmaxf(fmaxf(fmaxf(t0[0], t0[1]), fmaxf(t0[2], t0[3])), fmaxf(fmaxf(t0[4], t0[5]), fmaxf(t0[6], t0[7])));
+          const float cm1 = fmaxf(fmaxf(fmaxf(t1[0], t1[1]), fmaxf(t1[2], t1[3])), fmaxf(fmaxf(t1[4], t1[5]), fmaxf(t1[6], t1[7])));
           // kk distinct columns reach the kk-th largest 4-column-group maximum (first level of the max tree): a
           // lower bound of the kk-th best score; finer than whole chunks because near neighbours sit close together
           // in the table.  M and the list live in g-space (score - goff).
@@ -1362,38 +1453,35 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
                 if (t1[i] - goff > M) M = knn_topk_insert(topk, p.kk, t1[i] - goff);
             }
           }
-          thr = (M - margin) + goff;
-        }
-        // candidate masks: d_j = v_j - thr as packed pairs (FADD2), then the sign bits are shifted into a mask with
-        // one funnel shift per column: 1.5 issue slots per accumulator element (round 1: 2.4 -- two FFMAs per
-        // element plus conversions).  NaN scores only occur in rows whose margin is not finite (flag 1).
-        uint32_t nc0, nc1;
-        {
-          const uint64_t nthr2 = ptx::pack2(-thr, -thr);
-          uint32_t c00 = 0, c01 = 0, c10 = 0, c11 = 0;   // two 16-column chains per chunk (shorter dependency chains)
+          const float thr = (M - margin) + goff;
+          // candidate masks: d_j = v_j - thr as packed pairs, then the sign bits are shifted into a mask with one funnel
+          // shift per column
+          uint32_t nc0, nc1;
+          {
+            const uint64_t nthr2 = ptx::pack2(-thr, -thr);
+            uint32_t c00 = 0, c01 = 0, c10 = 0, c11 = 0;   // two 16-column chains per chunk (shorter dependency chains)
 #pragma unroll
-          for (int jj = 0; jj < 32; jj += 2) {
-            float x0, y0, x1, y1;
-            ptx::unpack2(ptx::fadd2(ptx::pack2(__uint_as_float(r0[jj]), __uint_as_float(r0[jj + 1])), nthr2), x0, y0);
-            ptx::unpack2(ptx::fadd2(ptx::pack2(__uint_as_float(r1[jj]), __uint_as_float(r1[jj + 1])), nthr2), x1, y1);
-            if (jj < 16) {
-              c00 = __funnelshift_l(__float_as_uint(x0), c00, 1);
-              c00 = __funnelshift_l(__float_as_uint(y0), c00, 1);
-              c10 = __funnelshift_l(__float_as_uint(x1), c10, 1);
-              c10 = __funnelshift_l(__float_as_uint(y1), c10, 1);
-            } else {
-              c01 = __funnelshift_l(__float_as_uint(x0), c01, 1);
-              c01 = __funnelshift_l(__float_as_uint(y0), c01, 1);
-              c11 = __funnelshift_l(__float_as_uint(x1), c11, 1);
-              c11 = __funnelshift_l(__float_as_uint(y1), c11, 1);
+            for (int jj = 0; jj < 32; jj += 2) {
+              float x0, y0, x1, y1;
+              ptx::unpack2(ptx::fadd2(ptx::pack2(__uint_as_float(r0[jj]), __uint_as_float(r0[jj + 1])), nthr2), x0, y0);
+              ptx::unpack2(ptx::fadd2(ptx::pack2(__uint_as_float(r1[jj]), __uint_as_float(r1[jj + 1])), nthr2), x1, y1);
+              if (jj < 16) {
+                c00 = __funnelshift_l(__float_as_uint(x0), c00, 1);
+                c00 = __funnelshift_l(__float_as_uint(y0), c00, 1);
+                c10 = __funnelshift_l(__float_as_uint(x1), c10, 1);
+                c10 = __funnelshift_l(__float_as_uint(y1), c10, 1);
+              } else {
+                c01 = __funnelshift_l(__float_as_uint(x0), c01, 1);
+                c01 = __funnelshift_l(__float_as_uint(y0), c01, 1);
+                c11 = __funnelshift_l(__float_as_uint(x1), c11, 1);
+                c11 = __funnelshift_l(__float_as_uint(y1), c11, 1);
+              }
             }
+            // bit (31 - j) of (c?0 << 16 | c?1) = sign of d_j = "column j is below the threshold"
+            nc0 = (c00 << 16) | c01;
+            nc1 = (c10 << 16) | c11;
           }
-          // bit (31 - j) of (c?0 << 16 | c?1) = sign of d_j = "column j is below the threshold"
-          nc0 = (c00 << 16) | c01;
-          nc1 = (c10 << 16) | c11;
-        }
-        const uint32_t mask0 = __brev(~nc0), mask1 = __brev(~nc1);
-        if (MODE == 2) {
+          const uint32_t mask0 = __brev(~nc0), mask1 = __brev(~nc1);
           if (klive && !(p.knn_first_pass && seg == 0)) {
             if (mask0)
               cnt = knn_append(kent, cnt, M, cm0 - goff, mask0, static_cast<uint32_t>(n) * 4 + h * 2, margin, &flags);
@@ -1401,23 +1489,6 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
               cnt = knn_append(kent, cnt, M, cm1 - goff, mask1, static_cast<uint32_t>(n) * 4 + h * 2 + 1, margin, &flags);
           }
           if (it.seg_last()) { si++; seg++; }
-          continue;
-        }
-        if (it.seg_last()) si++;
-        // one entry per n-tile that holds a candidate in this thread's 64 columns (round 2 v7: one per 32-column chunk,
-        // two divergent append blocks per n-tile)
-        if (mask0 | mask1) {
-          constexpr uint32_t A = LIST_ARRAY / 4;
-          if (cnt >= LIST_LEN - 1) cnt = compact_list(lst, cnt, thr);   // rare: drop entries below the risen threshold
-          if (cnt < LIST_LEN) {
-            lst[cnt * 256] = __float_as_uint(fmaxf(cm0, cm1));
-            lst[A + cnt * 256] = mask0;
-            lst[2 * A + cnt * 256] = mask1;
-            lst[3 * A + cnt * 256] = static_cast<uint32_t>(n);
-            cnt++;
-          } else {
-            flags |= 2u;
-          }
         }
       }
       if (MODE == 2) {
@@ -1441,12 +1512,15 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
         ti++;
         continue;
       }
-      // publish this half-row's state; the emitter warps merge the halves and write the results
-      fin[slot] = M;
-      reinterpret_cast<uint32_t*>(fin)[256 + slot] = cnt;
-      reinterpret_cast<uint32_t*>(fin)[512 + slot] = flags;
-      fin[768 + slot] = margin;
-      if (MODE == 1) fin[1024 + slot] = M2;
+      // publish the per-row maxima (the same in the four lanes of a quad); the emitter warps merge the four lists of
+      // a row and write the results
+      if ((lane & 3) == 0) {
+#pragma unroll
+        for (int hh = 0; hh < 2; hh++) {
+          fin[FIN_M + qrow + 8 * hh] = Mr[hh];
+          if (MODE == 1) fin[FIN_M2 + qrow + 8 * hh] = M2r[hh];
+        }
+      }
       __syncwarp();
       if (lane == 0) ptx::mbar_arrive(&bars[BAR_EMIT_FULL + par]);
       ti++;
@@ -1460,7 +1534,8 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
     for (uint32_t tile = tile_begin; tile < tile_end; tile += gridDim.x, ti++) {
       const int par = ti & 1;
       const uint32_t* lst = reinterpret_cast<const uint32_t*>(smem + L.list) + par * LIST_LEN * 256;
-      const float* fin = reinterpret_cast<const float*>(smem + L.fin) + par * 5 * 256;
+      const uint16_t* lnt = reinterpret_cast<const uint16_t*>(smem + L.list + LIST_ARRAYS * LIST_ARRAY) + par * LIST_LEN * 256;
+      const float* fin = reinterpret_cast<const float*>(smem + L.fin) + par * FIN_WORDS;
       const uint32_t* finu = reinterpret_cast<const uint32_t*>(fin);
       TC_WAIT(BAR_EMIT_FULL + par, (ti >> 1) & 1, 12);
       uint64_t grow = static_cast<uint64_t>(tile) * TM + row;
@@ -1469,34 +1544,39 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
       const bool live = grow < n_eff;
       if (MODE == 1 && live) grow = p.rows[grow];
       if (live) {
-        float Mf = fmaxf(fin[row], fin[TM + row]);
-        if (MODE == 1)   // second largest of the two halves' (largest, second largest) pairs
-          Mf = fmaxf(fminf(fin[row], fin[TM + row]), fmaxf(fin[1024 + row], fin[1024 + TM + row]));
-        const float thr = fminf(Mf, cap) - fin[768 + row];
-        fl = finu[512 + row] | finu[512 + TM + row] | force;
+        // the row's four epilogue threads: lanes 4 (row % 8) + t of consumer warp row / 16; the row is their R0 or R1
+        const int hh = (row >> 3) & 1;
+        const int lid0 = (row >> 4) * 32 + (row & 7) * 4;
+        // MODE 1: the second largest of the row's chunk maxima (a lower bound of its second best score)
+        const float Mf = MODE == 1 ? fin[FIN_M2 + row] : fin[FIN_M + row];
+        const float mg = fin[FIN_MARGIN + row];
+        const float thr = fminf(Mf, cap) - mg;
+        fl = force;
         // cosine: if every dot may be <= -1 they all clamp to pi and the lowest index wins -> exact pass
-        if (p.metric == 1 && !(Mf >= fin[768 + row] - cap)) fl |= 8u;
+        if (p.metric == 1 && !(Mf >= mg - cap)) fl |= 8u;
         // padded table rows and dead (non-finite) centroids score exactly -65504 (zero row + sentinel bias): a
         // threshold that low cannot tell them from real candidates (an outlier far from every centroid) -> exact pass
         if (!(thr > SENTINEL_GUARD)) fl |= 8u;
-        for (int hh = 0; hh < 2; hh++) {
-          const int sl = hh * TM + row;
-          const uint32_t c2 = finu[256 + sl];
+        // Candidates reach cand[] ordered by (lane, entry, bit), not by column.  Nothing downstream depends on that
+        // order: the re-check reduction picks the smallest index among equal scores (sc == best && c < arg), and the
+        // Yinyang finish takes a warp minimum of the index.
+        for (int t = 0; t < 4; t++) {
+          const int sl = lid0 + t;
+          const uint32_t st = finu[FIN_STATE + sl];
+          fl |= (st >> (8 + 8 * hh)) & 0xffu;
+          const uint32_t c2 = st & 0xffu;
           for (uint32_t i = 0; i < c2; i++) {
             constexpr uint32_t A = LIST_ARRAY / 4;
-            if (!(__uint_as_float(lst[i * 256 + sl]) >= thr)) continue;
-            const uint32_t base = lst[3 * A + i * 256 + sl] * TN + hh * 64;
-#pragma unroll
-            for (int c = 0; c < 2; c++) {
-              uint32_t m = lst[(1 + c) * A + i * 256 + sl];
-              while (m) {
-                const int b = __ffs(m) - 1;
-                m &= m - 1;
-                const uint32_t col = base + c * 32 + b;
-                if (col < p.K) {
-                  if (total < MAX_CAND) cand[total] = col;
-                  total++;
-                }
+            if (!(__uint_as_float(lst[hh * A + i * 256 + sl]) >= thr)) continue;   // the row's chunk maximum
+            const uint32_t base = static_cast<uint32_t>(lnt[i * 256 + sl]) * TN + 2 * t;
+            uint32_t m = lst[(2 + hh) * A + i * 256 + sl];
+            while (m) {
+              const int b = __ffs(m) - 1;
+              m &= m - 1;
+              const uint32_t col = base + 8 * (b >> 1) + (b & 1);   // bit b = 2j + e: column 8j + 2t + e
+              if (col < p.K) {
+                if (total < MAX_CAND) cand[total] = col;
+                total++;
               }
             }
           }
