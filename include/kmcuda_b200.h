@@ -30,6 +30,23 @@ extern "C" {
 
 typedef struct kmcuda_b200_shard kmcuda_b200_shard;
 
+/* kmeans_cuda() with a weight per sample (scikit-learn's sample_weight).  The parameters are those of kmeans_cuda(),
+ * plus `weights`: [samples_size] fp32, a host pointer when device_ptrs < 0 and device memory on device `device_ptrs`
+ * otherwise (the rule for `samples`; fp32 in fp16x2 mode too).  weights == NULL is the unweighted run.
+ * Every weight must be finite and >= 0 and their sum > 0, otherwise kmcudaInvalidArguments; so is a weighted call
+ * with KMCUDA_B200_STRICT_UPDATE=1.  The assignment step is unchanged; the centroid update is sum(w x) / sum(w) (L2)
+ * or the angular recurrence with weight totals for counts; a cluster whose weight total is 0 is treated as the
+ * reference treats an empty cluster (L2: NaN centroid, never chosen again; angular: the same recurrence);
+ * k-means++ draws proportionally to w * d, AFK-MC2 uses q = w / 2W + w d^2 / (2 sum w d^2), random init skips rows
+ * of weight 0, and average_distance is sum(w d) / sum(w).  With every weight 1 the result is bit-identical to
+ * kmeans_cuda(). */
+KMCUDAResult kmcuda_b200_kmeans_weighted(KMCUDAInitMethod init, const void *init_params, float tolerance,
+                                         float yinyang_t, KMCUDADistanceMetric metric, uint32_t samples_size,
+                                         uint16_t features_size, uint32_t clusters_size, uint32_t seed,
+                                         uint32_t device, int32_t device_ptrs, int32_t fp16x2, int32_t verbosity,
+                                         const float *samples, const float *weights, float *centroids,
+                                         uint32_t *assignments, float *average_distance);
+
 /* Creates the per-shard workspace (fp16 centroid table, TMA descriptors, re-check queues, sort
  * buffers) for up to max_samples samples of features_size fp32 features and clusters_size clusters. */
 KMCUDAResult kmcuda_b200_shard_create(kmcuda_b200_shard **shard, KMCUDADistanceMetric metric,

@@ -41,6 +41,7 @@ struct UpdateWorkspace {
   uint32_t *keys_in = nullptr, *keys_out = nullptr, *vals_in = nullptr, *vals_out = nullptr;
   uint32_t* offsets = nullptr;   // [K+1]
   float* partial = nullptr;      // [update_partial_rows(max_n, K)][D]: one row per (chunk, cluster) run
+  float* partial_w = nullptr;    // [update_partial_rows(max_n, K)]: weight total per run (weighted update only)
   void* cub_tmp = nullptr;
   size_t cub_tmp_bytes = 0;
   uint32_t iota_n = 0;           // vals_in[0 .. iota_n) already holds the identity permutation
@@ -51,9 +52,11 @@ struct UpdateWorkspace {
 constexpr uint32_t kSumChunk = KMB_SUM_CHUNK;   // sorted positions per CTA of the member-sum kernel
 size_t update_partial_rows(uint32_t n, uint32_t K);
 size_t update_cub_bytes(uint32_t n);
-// sums[K][D] (fp32) and counts[K] (uint32) of this shard's samples
+// sums[K][D] (fp32) and counts[K] (uint32) of this shard's samples.  With sample weights w[n]: sums = sum of w_i x_i
+// and wsums[K] = sum of w_i over the members (ws.partial_w must be set); counts stay member counts.
 cudaError_t launch_partial_sums(const float* X, uint32_t n, int D, uint32_t K, const uint32_t* assign,
-                                UpdateWorkspace& ws, float* sums, uint32_t* counts, cudaStream_t st);
+                                UpdateWorkspace& ws, float* sums, uint32_t* counts, cudaStream_t st,
+                                const float* w = nullptr, float* wsums = nullptr);
 // strict parity mode: the reference's running-sum update replayed in sample order (simt_kernels.cu)
 size_t strict_update_cub_bytes(uint32_t n);
 cudaError_t launch_strict_update(int metric, const float* X, uint32_t n, int D, uint32_t K, const uint32_t* prev,
@@ -70,9 +73,19 @@ struct PeerBuffers {
 };
 cudaError_t launch_peer_reduce(const PeerBuffers& pb, uint32_t K, int D, float* out_sums, uint32_t* out_counts,
                                cudaStream_t st);
-// C = sums/count (L2, NaN for empty) or sums/||sums|| (cosine); ccounts = counts
+// weighted update: out = p[0] + p[1] + ... (device order) of `count` floats, the per-cluster weight totals
+struct PeerF32 {
+  int n;
+  const float* p[kMaxPeers];
+};
+cudaError_t launch_peer_sum_f32(const PeerF32& pb, size_t count, float* out, cudaStream_t st);
+// C = sums/count (L2, NaN for empty) or sums/||sums|| (cosine); ccounts = counts.  Weighted (wsums != nullptr): the
+// count is replaced by the weight total, cweights[K] holds it between updates (the cosine recurrence's old count)
 cudaError_t launch_normalize(int metric, const float* sums, const uint32_t* counts, uint32_t K, int D,
-                             float* C, uint32_t* ccounts, float* prev_sums, cudaStream_t st);
+                             float* C, uint32_t* ccounts, float* prev_sums, cudaStream_t st,
+                             const float* wsums = nullptr, float* cweights = nullptr);
+// sample weights: flags[0] |= 1 if some w is NaN, infinite or negative; *total += sum of w (both zeroed by the caller)
+cudaError_t launch_check_weights(const float* w, uint32_t n, uint32_t* flags, double* total, cudaStream_t st);
 
 // ---- Yinyang -------------------------------------------------------------------------------------
 // bounds layout [n][G+1] (one contiguous record per sample): [0] = upper bound, [1+g] = lower bound of group g
@@ -105,15 +118,19 @@ cudaError_t launch_yy_step(int metric, TcPlan* plan, const float* X, const float
                            const YyWorkspace& ws, uint32_t* d_changed, bool reference_order_scan, cudaStream_t st);
 
 // ---- misc ------------------------------------------------------------------------------------------
+// w (sample weights, optional): *d_sum accumulates w_i * d_i
 cudaError_t launch_average_distance(int metric, const float* X, const float* C, uint32_t n, int D,
-                                    const uint32_t* assign, double* d_sum, cudaStream_t st);
+                                    const uint32_t* assign, double* d_sum, cudaStream_t st, const float* w = nullptr);
 cudaError_t launch_afkmc2_min_dist(int metric, const float* X, const float* C, int D, uint32_t k,
                                    const uint32_t* rows, uint32_t m, float* min_dists, cudaStream_t st);
+// w (optional): dists[] stays the plain minimum distance, *d_sum accumulates w_i * d_i
 cudaError_t launch_plusplus_step(int metric, const float* X, uint32_t n, int D, const float* centroid,
-                                 int first, float* dists, double* d_sum, cudaStream_t st);
-// device-resident k-means++ round (simt_kernels.cu): bsum / bpre hold ceil(n / 256) + 1 doubles, chosen [K]
+                                 int first, float* dists, double* d_sum, cudaStream_t st, const float* w = nullptr);
+// device-resident k-means++ round (simt_kernels.cu): bsum / bpre hold ceil(n / 256) + 1 doubles, chosen [K];
+// w (optional): the draw is proportional to w_i * d_i and never picks a zero-weight row
 cudaError_t launch_plusplus_round(int metric, const float* X, uint32_t n, int D, float* C, uint32_t i, double choice,
-                                  float* dists, double* bsum, double* bpre, uint32_t* chosen, cudaStream_t st);
+                                  float* dists, double* bsum, double* bpre, uint32_t* chosen, cudaStream_t st,
+                                  const float* w = nullptr);
 cudaError_t launch_half_to_float(const void* src, float* dst, size_t n, cudaStream_t st);
 cudaError_t launch_float_to_half(const float* src, void* dst, size_t n, cudaStream_t st);
 cudaError_t launch_fill_u32(uint32_t* p, uint32_t v, size_t n, cudaStream_t st);

@@ -120,17 +120,54 @@ void* as_pointer(PyObject* o) {
   return reinterpret_cast<void*>(static_cast<uintptr_t>(PyLong_AsUnsignedLongLong(o)));
 }
 
+// sample_weight intake: with ndarray samples a 1-D numeric array-like of length n (converted to float32, kept alive in
+// `keep`); with device-pointer samples an int device pointer on the samples' device
+bool take_weights(PyObject* obj, bool device_samples, uint32_t n, Ref* keep, const float** data) {
+  if (device_samples) {
+    if (!PyLong_Check(obj) || PyBool_Check(obj)) {
+      PyErr_SetString(PyExc_TypeError, "\"sample_weight\" must be a device pointer (integer) when \"samples\" is a "
+                                       "pointer tuple");
+      return false;
+    }
+    *data = static_cast<const float*>(as_pointer(obj));
+    if (PyErr_Occurred()) return false;
+    if (!*data) {
+      PyErr_SetString(PyExc_ValueError, "\"sample_weight\" is null");
+      return false;
+    }
+    return true;
+  }
+  Ref probe(PyArray_FROM_O(obj));
+  if (!probe.p || !(PyArray_ISBOOL(probe.arr()) || PyArray_ISINTEGER(probe.arr()) || PyArray_ISFLOAT(probe.arr()))) {
+    PyErr_Clear();
+    PyErr_SetString(PyExc_TypeError, "\"sample_weight\" must be a 1D numeric array");
+    return false;
+  }
+  if (PyArray_NDIM(probe.arr()) != 1) {
+    PyErr_SetString(PyExc_ValueError, "\"sample_weight\" must be a 1D array");
+    return false;
+  }
+  if (static_cast<uint64_t>(PyArray_DIM(probe.arr(), 0)) != n) {
+    PyErr_SetString(PyExc_ValueError, "\"sample_weight\" must be of the same length as \"samples\"");
+    return false;
+  }
+  keep->reset(PyArray_FROM_OTF(probe.p, NPY_FLOAT32, NPY_ARRAY_IN_ARRAY | NPY_ARRAY_FORCECAST));
+  if (!keep->p) return false;
+  *data = static_cast<const float*>(PyArray_DATA(keep->arr()));
+  return true;
+}
+
 PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
   uint32_t clusters = 0, afkmc2_m = 0, seed = static_cast<uint32_t>(time(nullptr)), device = 0;
   int32_t verbosity = 0;
   int adflag = 0;
   float tolerance = .01f, yinyang_t = .1f;
-  PyObject *samples_obj, *init_obj = Py_None, *metric_obj = Py_None;
+  PyObject *samples_obj, *init_obj = Py_None, *metric_obj = Py_None, *weight_obj = Py_None;
   static const char* kwlist[] = {"samples", "clusters", "tolerance", "init", "yinyang_t", "metric",
-                                 "average_distance", "seed", "device", "verbosity", nullptr};
-  if (!PyArg_ParseTupleAndKeywords(args, kwargs, "OI|fOfOpIIi", const_cast<char**>(kwlist), &samples_obj,
+                                 "average_distance", "seed", "device", "verbosity", "sample_weight", nullptr};
+  if (!PyArg_ParseTupleAndKeywords(args, kwargs, "OI|fOfOpIIiO", const_cast<char**>(kwlist), &samples_obj,
                                    &clusters, &tolerance, &init_obj, &yinyang_t, &metric_obj, &adflag, &seed,
-                                   &device, &verbosity))
+                                   &device, &verbosity, &weight_obj))
     return nullptr;
   KMCUDAInitMethod init = kmcudaInitMethodPlusPlus;
   auto named_init = [&init](PyObject* o) {
@@ -205,6 +242,9 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
     return nullptr;
   }
   if (!check_features(d)) return nullptr;
+  const float* weights = nullptr;
+  Ref keep_weights;
+  if (weight_obj != Py_None && !take_weights(weight_obj, device_ptrs >= 0, n, &keep_weights, &weights)) return nullptr;
   Ref centroids_arr, assignments_arr;
   if (device_ptrs < 0) {
     npy_intp cdims[2] = {static_cast<npy_intp>(clusters), static_cast<npy_intp>(fp16x2 ? d * 2 : d)};
@@ -253,9 +293,14 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
   float average_distance = 0;
   int result;
   Py_BEGIN_ALLOW_THREADS
-  result = kmeans_cuda(init, &afkmc2_m, tolerance, yinyang_t, metric, n, static_cast<uint16_t>(d), clusters, seed,
-                       device, device_ptrs, fp16x2, verbosity, samples, centroids, assignments,
-                       adflag ? &average_distance : nullptr);
+  if (weights)
+    result = kmcuda_b200_kmeans_weighted(init, &afkmc2_m, tolerance, yinyang_t, metric, n, static_cast<uint16_t>(d),
+                                         clusters, seed, device, device_ptrs, fp16x2, verbosity, samples, weights,
+                                         centroids, assignments, adflag ? &average_distance : nullptr);
+  else
+    result = kmeans_cuda(init, &afkmc2_m, tolerance, yinyang_t, metric, n, static_cast<uint16_t>(d), clusters, seed,
+                         device, device_ptrs, fp16x2, verbosity, samples, centroids, assignments,
+                         adflag ? &average_distance : nullptr);
   Py_END_ALLOW_THREADS
   if (result != kmcudaSuccess) return raise_for(result, "kmeans_cuda");
   if (device_ptrs < 0) {
@@ -380,7 +425,8 @@ PyObject* py_knn_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
 
 char module_doc[] = "K-means and K-nn on NVIDIA H100 (drop-in for src-d/kmcuda's libKMCUDA).";
 char kmeans_doc[] = "kmeans_cuda(samples, clusters, tolerance=.01, init=\"k-means++\", yinyang_t=.1, metric=\"L2\", "
-                    "average_distance=False, seed=time(), device=0, verbosity=0) -> (centroids, assignments[, avg])";
+                    "average_distance=False, seed=time(), device=0, verbosity=0, sample_weight=None) -> "
+                    "(centroids, assignments[, avg])";
 char knn_doc[] = "knn_cuda(k, samples, centroids, assignments, metric=\"L2\", device=0, verbosity=0) -> neighbors";
 
 PyMethodDef module_functions[] = {

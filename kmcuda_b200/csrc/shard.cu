@@ -298,15 +298,23 @@ KMCUDAResult Shard::check_pipeline() {
 }
 
 KMCUDAResult Shard::partial_sums(uint32_t n, const float* X, const uint32_t* assignments, float* sums,
-                                 uint32_t* counts, cudaStream_t st) {
+                                 uint32_t* counts, cudaStream_t st, const float* weights, float* wsums) {
   if (n > max_n || ws.cub_tmp == nullptr) return kmcudaInvalidArguments;
-  KMB_CU(launch_partial_sums(X, n, D, K, assignments, ws, sums, counts, st), kmcudaRuntimeError);
+  if (weights) {
+    if (!wsums) return kmcudaInvalidArguments;
+    if (!ws_partial_w.get()) {
+      KMB_CU(ws_partial_w.alloc(update_partial_rows(max_n, K)), kmcudaMemoryAllocationFailure);
+      ws.partial_w = ws_partial_w;
+    }
+  }
+  KMB_CU(launch_partial_sums(X, n, D, K, assignments, ws, sums, counts, st, weights, wsums), kmcudaRuntimeError);
   return kmcudaSuccess;
 }
 
 KMCUDAResult Shard::finish_update(const float* sums, const uint32_t* counts, float* C,
-                                  uint32_t* ccounts, cudaStream_t st) {
-  KMB_CU(launch_normalize(metric, sums, counts, K, D, C, ccounts, prev_sums, st), kmcudaRuntimeError);
+                                  uint32_t* ccounts, cudaStream_t st, const float* wsums, float* cweights) {
+  if (wsums && !cweights) return kmcudaInvalidArguments;
+  KMB_CU(launch_normalize(metric, sums, counts, K, D, C, ccounts, prev_sums, st, wsums, cweights), kmcudaRuntimeError);
   return kmcudaSuccess;
 }
 

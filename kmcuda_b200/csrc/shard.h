@@ -110,10 +110,13 @@ class Shard {
   // hot path
   KMCUDAResult assign(uint32_t n, const float* X, const float* C, uint32_t* assignments,
                       uint32_t* prev, uint32_t* d_changed, cudaStream_t st);
+  // weights (optional, [n] on this device): weighted member sums, and wsums[K] = the members' weight totals
   KMCUDAResult partial_sums(uint32_t n, const float* X, const uint32_t* assignments, float* sums,
-                            uint32_t* counts, cudaStream_t st);
+                            uint32_t* counts, cudaStream_t st, const float* weights = nullptr,
+                            float* wsums = nullptr);
+  // wsums (optional): normalise by the weight totals; cweights[K] keeps them for the next cosine update
   KMCUDAResult finish_update(const float* sums, const uint32_t* counts, float* C, uint32_t* ccounts,
-                             cudaStream_t st);
+                             cudaStream_t st, const float* wsums = nullptr, float* cweights = nullptr);
   // strict parity mode (KMCUDA_B200_STRICT_UPDATE=1): the reference's running-sum update in sample order, in place
   KMCUDAResult update_reference_order(uint32_t n, const float* X, const uint32_t* assignments, const uint32_t* prev,
                                       float* C, uint32_t* ccounts, cudaStream_t st);
@@ -157,6 +160,7 @@ class Shard {
   UpdateWorkspace ws;
   DevBuf<uint32_t> ws_keys_out, ws_vals_in, ws_vals_out, ws_offsets;
   DevBuf<float> ws_partial;
+  DevBuf<float> ws_partial_w;   // weighted update only, allocated on first use
   DevBuf<float> prev_sums;   // cosine update: member sums of the previous iteration
   DevBuf<char> ws_cub;
   TcPlan* tc = nullptr;

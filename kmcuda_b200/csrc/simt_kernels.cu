@@ -421,11 +421,14 @@ __device__ __forceinline__ float sum_load(const float* p) {
 // 2.26 ms at 8M x 256 with 4-byte loads and 8 rows in flight, 1.89 ms with 16 rows in flight)
 // (the minimum-blocks bound is there for the register budget: without it ptxas aims at 32 registers = full occupancy
 // and sinks the row loads between the additions, one or two in flight instead of kUpdateUnroll)
-template <int VEC>
+// WEIGHTED: member row i enters the compensated sum as w[i] * x_i, and the run's weight total (compensated, same order)
+// goes to partial_w[b + c], so combine_partials_kernel folds it like a one-feature row.  The 4-byte weight gathers are
+// issued with the group's row loads.  With every weight 1.0 the products are exact and the sums are the unweighted ones.
+template <int VEC, bool WEIGHTED>
 __global__ void __launch_bounds__(256, VEC == 4 ? 3 : 5)
 cluster_sums_kernel(const float* __restrict__ X, int D, const uint32_t* __restrict__ keys,
                     const uint32_t* __restrict__ idx, const uint32_t* __restrict__ offsets, uint32_t K,
-                    float* __restrict__ partial) {
+                    float* __restrict__ partial, const float* __restrict__ w, float* __restrict__ partial_w) {
   const uint32_t b = blockIdx.x;
   const uint32_t total = offsets[K];                     // positions past it carry the "unassigned" key
   uint32_t lo = b * kSumChunk;
@@ -436,6 +439,7 @@ cluster_sums_kernel(const float* __restrict__ X, int D, const uint32_t* __restri
     const uint32_t e = min(hi, offsets[c + 1]);
     for (int f = threadIdx.x; f < nf; f += blockDim.x) {
       float sum[VEC], comp[VEC];
+      float wsum = 0.f, wcomp = 0.f;
 #pragma unroll
       for (int q = 0; q < VEC; q++) sum[q] = comp[q] = 0.f;
       uint32_t j = lo;
@@ -444,9 +448,11 @@ cluster_sums_kernel(const float* __restrict__ X, int D, const uint32_t* __restri
       for (int u = 0; u < kUpdateUnroll; u++) id[u] = idx[min(j + u, e - 1)];
       for (; j + kUpdateUnroll <= e; j += kUpdateUnroll) {
         float v[kUpdateUnroll][VEC];
+        float wt[kUpdateUnroll];
 #pragma unroll
         for (int u = 0; u < kUpdateUnroll; u++) {
           const float* src = X + static_cast<size_t>(id[u]) * D + f * VEC;
+          if (WEIGHTED) wt[u] = __ldg(w + id[u]);
           if (VEC == 4) {
 #if KMB_SUM_STREAMING
             const float4 t4 = __ldcs(reinterpret_cast<const float4*>(src));
@@ -461,25 +467,38 @@ cluster_sums_kernel(const float* __restrict__ X, int D, const uint32_t* __restri
 #pragma unroll
         for (int u = 0; u < kUpdateUnroll; u++) id[u] = idx[min(j + kUpdateUnroll + u, e - 1)];
 #pragma unroll
-        for (int u = 0; u < kUpdateUnroll; u++)
+        for (int u = 0; u < kUpdateUnroll; u++) {
 #pragma unroll
           for (int q = 0; q < VEC; q++) {
-            const float y = v[u][q] - comp[q], t = sum[q] + y;
+            const float y = (WEIGHTED ? v[u][q] * wt[u] : v[u][q]) - comp[q], t = sum[q] + y;
             comp[q] = (t - sum[q]) - y;
             sum[q] = t;
           }
+          if (WEIGHTED) {
+            const float y = wt[u] - wcomp, t = wsum + y;
+            wcomp = (t - wsum) - y;
+            wsum = t;
+          }
+        }
       }
       for (; j < e; j++) {
         const float* src = X + static_cast<size_t>(idx[j]) * D + f * VEC;
+        const float wj = WEIGHTED ? __ldg(w + idx[j]) : 1.f;
 #pragma unroll
         for (int q = 0; q < VEC; q++) {
-          const float y = sum_load(src + q) - comp[q], t = sum[q] + y;
+          const float y = (WEIGHTED ? sum_load(src + q) * wj : sum_load(src + q)) - comp[q], t = sum[q] + y;
           comp[q] = (t - sum[q]) - y;
           sum[q] = t;
+        }
+        if (WEIGHTED) {
+          const float y = wj - wcomp, t = wsum + y;
+          wcomp = (t - wsum) - y;
+          wsum = t;
         }
       }
 #pragma unroll
       for (int q = 0; q < VEC; q++) partial[(static_cast<size_t>(b) + c) * D + f * VEC + q] = sum[q];
+      if (WEIGHTED && f == 0) partial_w[static_cast<size_t>(b) + c] = wsum;
     }
     lo = e;
   }
@@ -516,10 +535,13 @@ size_t update_cub_bytes(uint32_t n) {
 }
 
 cudaError_t launch_partial_sums(const float* X, uint32_t n, int D, uint32_t K, const uint32_t* assign,
-                                UpdateWorkspace& ws, float* sums, uint32_t* counts, cudaStream_t st) {
+                                UpdateWorkspace& ws, float* sums, uint32_t* counts, cudaStream_t st,
+                                const float* w, float* wsums) {
+  if (w && (!wsums || !ws.partial_w)) return cudaErrorInvalidValue;
   if (n == 0) {
     cudaMemsetAsync(sums, 0, sizeof(float) * static_cast<size_t>(K) * D, st);
     cudaMemsetAsync(counts, 0, sizeof(uint32_t) * K, st);
+    if (w) cudaMemsetAsync(wsums, 0, sizeof(float) * K, st);
     return cudaGetLastError();
   }
   if (ws.iota_n < n) {   // the identity permutation is an input the sort never modifies: written once per workspace
@@ -533,13 +555,26 @@ cudaError_t launch_partial_sums(const float* X, uint32_t n, int D, uint32_t K, c
                                                   ws.vals_out, (int)n, 0, bits, st);
   if (e != cudaSuccess) return e;
   launch_segment_offsets(ws.keys_out, n, K, ws.offsets, counts, st);
+  const unsigned grid = cdiv(n, kSumChunk);
   if (D % 4 == 0 && (reinterpret_cast<uintptr_t>(X) & 15) == 0) {
     const int threads = std::min(256, (D / 4 + 31) / 32 * 32);
-    cluster_sums_kernel<4><<<cdiv(n, kSumChunk), threads, 0, st>>>(X, D, ws.keys_out, ws.vals_out, ws.offsets, K, ws.partial);
+    if (w)
+      cluster_sums_kernel<4, true><<<grid, threads, 0, st>>>(X, D, ws.keys_out, ws.vals_out, ws.offsets, K, ws.partial,
+                                                            w, ws.partial_w);
+    else
+      cluster_sums_kernel<4, false><<<grid, threads, 0, st>>>(X, D, ws.keys_out, ws.vals_out, ws.offsets, K, ws.partial,
+                                                             nullptr, nullptr);
   } else {
-    cluster_sums_kernel<1><<<cdiv(n, kSumChunk), 256, 0, st>>>(X, D, ws.keys_out, ws.vals_out, ws.offsets, K, ws.partial);
+    if (w)
+      cluster_sums_kernel<1, true><<<grid, 256, 0, st>>>(X, D, ws.keys_out, ws.vals_out, ws.offsets, K, ws.partial, w,
+                                                        ws.partial_w);
+    else
+      cluster_sums_kernel<1, false><<<grid, 256, 0, st>>>(X, D, ws.keys_out, ws.vals_out, ws.offsets, K, ws.partial,
+                                                         nullptr, nullptr);
   }
   combine_partials_kernel<<<cdiv(static_cast<size_t>(K) * D, 256), 256, 0, st>>>(ws.partial, ws.offsets, K, D, sums);
+  // the weight totals are one-feature rows of the same (chunk, cluster) runs: the same fold gives them
+  if (w) combine_partials_kernel<<<cdiv(K, 256), 256, 0, st>>>(ws.partial_w, ws.offsets, K, 1, wsums);
   return cudaGetLastError();
 }
 
@@ -734,6 +769,21 @@ cudaError_t launch_peer_min_u32(const PeerU32& pb, size_t count, uint32_t* out, 
   return cudaGetLastError();
 }
 
+// weighted update: the per-cluster weight totals of every shard, added in device order like the sums
+__global__ void peer_sum_f32_kernel(const PeerF32 pb, size_t count, float* __restrict__ out) {
+  const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
+  for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < count; i += stride) {
+    float acc = pb.p[0][i];
+    for (int d = 1; d < pb.n; d++) acc += pb.p[d][i];
+    out[i] = acc;
+  }
+}
+cudaError_t launch_peer_sum_f32(const PeerF32& pb, size_t count, float* out, cudaStream_t st) {
+  const unsigned grid = static_cast<unsigned>(std::min<size_t>(device_sms() * 4, (count + 255) / 256 + 1));
+  peer_sum_f32_kernel<<<grid, 256, 0, st>>>(pb, count, out);
+  return cudaGetLastError();
+}
+
 cudaError_t launch_peer_reduce(const PeerBuffers& pb, uint32_t K, int D, float* out_sums, uint32_t* out_counts,
                                cudaStream_t st) {
   const size_t nsums = static_cast<size_t>(K) * D;
@@ -755,8 +805,63 @@ __global__ void normalize_l2_kernel(const float* __restrict__ sums, const uint32
   if (i - static_cast<size_t>(c) * D == 0) ccounts[c] = cnt;
 }
 
+// Weighted L2: C = S_w * rcp(W_c).  W_c = 0 (no members, or only zero-weight ones) gives rcp = inf and a NaN centroid,
+// the reference's empty-cluster rule.
+__global__ void normalize_l2_weighted_kernel(const float* __restrict__ sums, const uint32_t* __restrict__ counts,
+                                             const float* __restrict__ wsums, uint32_t K, int D, float* __restrict__ C,
+                                             uint32_t* __restrict__ ccounts, float* __restrict__ cweights) {
+  const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= static_cast<size_t>(K) * D) return;
+  const uint32_t c = i / D;
+  const float wc = wsums[c];
+  C[i] = sums[i] * __frcp_rn(wc);
+  if (i - static_cast<size_t>(c) * D == 0) {
+    ccounts[c] = counts[c];
+    cweights[c] = wc;
+  }
+}
+
+// Weighted angular recurrence: raw = W_old * c_old + (S_w,cur - S_w,prev), then normalise; W_old (cweights) is the
+// previous update's weight total, as normalize_kernel<1> uses the previous count.  A cluster of weight 0 goes through
+// the same recurrence, as the reference's angular update treats an empty cluster (so all-ones weights reproduce the
+// unweighted run even when a cluster empties).
+__global__ void normalize_cos_weighted_kernel(const float* __restrict__ sums, const uint32_t* __restrict__ counts,
+                                              const float* __restrict__ wsums, uint32_t K, int D, float* __restrict__ C,
+                                              uint32_t* __restrict__ ccounts, float* __restrict__ cweights,
+                                              float* __restrict__ prev_sums) {
+  uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= K) return;
+  const float* s = sums + static_cast<size_t>(c) * D;
+  float* o = C + static_cast<size_t>(c) * D;
+  float* ps = prev_sums + static_cast<size_t>(c) * D;
+  const float old_w = cweights[c], wc = wsums[c];
+  Kahan k;
+  for (int f = 0; f < D; f++) {
+    const float cur = s[f];
+    const float raw = o[f] * old_w + (cur - ps[f]);
+    ps[f] = cur;
+    o[f] = raw;
+    k.mac(raw, raw);
+  }
+  const float scale = __frcp_rn(__fsqrt_rn(k.sum));
+  for (int f = 0; f < D; f++) o[f] = o[f] * scale;
+  ccounts[c] = counts[c];
+  cweights[c] = wc;
+}
+
 cudaError_t launch_normalize(int metric, const float* sums, const uint32_t* counts, uint32_t K, int D,
-                             float* C, uint32_t* ccounts, float* prev_sums, cudaStream_t st) {
+                             float* C, uint32_t* ccounts, float* prev_sums, cudaStream_t st,
+                             const float* wsums, float* cweights) {
+  if (wsums) {
+    if (!cweights) return cudaErrorInvalidValue;
+    if (metric == 1)
+      normalize_cos_weighted_kernel<<<cdiv(K, 64), 64, 0, st>>>(sums, counts, wsums, K, D, C, ccounts, cweights,
+                                                                prev_sums);
+    else
+      normalize_l2_weighted_kernel<<<cdiv(static_cast<size_t>(K) * D, 256), 256, 0, st>>>(sums, counts, wsums, K, D, C,
+                                                                                          ccounts, cweights);
+    return cudaGetLastError();
+  }
   if (metric == 1) normalize_kernel<1><<<cdiv(K, 64), 64, 0, st>>>(sums, counts, K, D, C, ccounts, prev_sums);
   else normalize_l2_kernel<<<cdiv(static_cast<size_t>(K) * D, 256), 256, 0, st>>>(sums, counts, K, D, C, ccounts);
   return cudaGetLastError();
@@ -810,18 +915,37 @@ __global__ void average_distance_kernel(const float* __restrict__ X, const float
   if ((threadIdx.x & 31) == 0) atomicAdd(d_sum, static_cast<double>(dist));
 }
 
+// weighted: sum of w_i * d_i (the caller divides by the weight total)
+template <int METRIC>
+__global__ void average_distance_weighted_kernel(const float* __restrict__ X, const float* __restrict__ C,
+                                                 uint32_t n, int D, const uint32_t* __restrict__ assign,
+                                                 const float* __restrict__ w, double* __restrict__ d_sum) {
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  float dist = 0.f;
+  if (i < n)
+    dist = distance_exact<METRIC>(X + static_cast<size_t>(i) * D, C + static_cast<size_t>(assign[i]) * D, D) * w[i];
+  for (int o = 16; o > 0; o >>= 1) dist += __shfl_down_sync(0xffffffffu, dist, o);
+  if ((threadIdx.x & 31) == 0) atomicAdd(d_sum, static_cast<double>(dist));
+}
+
 cudaError_t launch_average_distance(int metric, const float* X, const float* C, uint32_t n, int D,
-                                    const uint32_t* assign, double* d_sum, cudaStream_t st) {
+                                    const uint32_t* assign, double* d_sum, cudaStream_t st, const float* w) {
   if (n == 0) return cudaSuccess;
+  if (w) {
+    if (metric == 1) average_distance_weighted_kernel<1><<<cdiv(n, 256), 256, 0, st>>>(X, C, n, D, assign, w, d_sum);
+    else average_distance_weighted_kernel<0><<<cdiv(n, 256), 256, 0, st>>>(X, C, n, D, assign, w, d_sum);
+    return cudaGetLastError();
+  }
   if (metric == 1) average_distance_kernel<1><<<cdiv(n, 256), 256, 0, st>>>(X, C, n, D, assign, d_sum);
   else average_distance_kernel<0><<<cdiv(n, 256), 256, 0, st>>>(X, C, n, D, assign, d_sum);
   return cudaGetLastError();
 }
 
-template <int METRIC>
+// WEIGHTED: dists[] keeps the plain minimum distance d_i (the next round compares against it); d_sum adds w_i * d_i
+template <int METRIC, bool WEIGHTED>
 __global__ void plusplus_kernel(const float* __restrict__ X, uint32_t n, int D,
                                 const float* __restrict__ centroid, int first,
-                                float* __restrict__ dists, double* __restrict__ d_sum) {
+                                float* __restrict__ dists, double* __restrict__ d_sum, const float* __restrict__ w) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   float dist = 0.f;
   if (i < n) {
@@ -830,16 +954,57 @@ __global__ void plusplus_kernel(const float* __restrict__ X, uint32_t n, int D,
     float prev;
     if (first || dist < (prev = dists[i])) dists[i] = dist;
     else dist = prev;
+    if (WEIGHTED) dist *= w[i];
   }
   for (int o = 16; o > 0; o >>= 1) dist += __shfl_down_sync(0xffffffffu, dist, o);
   if ((threadIdx.x & 31) == 0) atomicAdd(d_sum, static_cast<double>(dist));
 }
 
 cudaError_t launch_plusplus_step(int metric, const float* X, uint32_t n, int D, const float* centroid,
-                                 int first, float* dists, double* d_sum, cudaStream_t st) {
+                                 int first, float* dists, double* d_sum, cudaStream_t st, const float* w) {
   if (n == 0) return cudaSuccess;
-  if (metric == 1) plusplus_kernel<1><<<cdiv(n, 256), 256, 0, st>>>(X, n, D, centroid, first, dists, d_sum);
-  else plusplus_kernel<0><<<cdiv(n, 256), 256, 0, st>>>(X, n, D, centroid, first, dists, d_sum);
+  const unsigned grid = cdiv(n, 256);
+  if (w) {
+    if (metric == 1) plusplus_kernel<1, true><<<grid, 256, 0, st>>>(X, n, D, centroid, first, dists, d_sum, w);
+    else plusplus_kernel<0, true><<<grid, 256, 0, st>>>(X, n, D, centroid, first, dists, d_sum, w);
+    return cudaGetLastError();
+  }
+  if (metric == 1) plusplus_kernel<1, false><<<grid, 256, 0, st>>>(X, n, D, centroid, first, dists, d_sum, nullptr);
+  else plusplus_kernel<0, false><<<grid, 256, 0, st>>>(X, n, D, centroid, first, dists, d_sum, nullptr);
+  return cudaGetLastError();
+}
+
+// Weight check of kmcuda_b200_kmeans_weighted: flags[0] |= 1 for a weight that is NaN, infinite or negative; *total +=
+// the shard's weights (double).  One pass over the shard, block-reduced, one atomic per block.
+__global__ void __launch_bounds__(256)
+check_weights_kernel(const float* __restrict__ w, uint32_t n, uint32_t* __restrict__ flags, double* __restrict__ total) {
+  __shared__ double s_part[8];
+  __shared__ int s_bad;
+  if (threadIdx.x == 0) s_bad = 0;
+  __syncthreads();
+  double acc = 0.0;
+  int bad = 0;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float v = w[i];
+    if (!(v >= 0.f && v <= FLT_MAX)) bad = 1;   // NaN fails both comparisons
+    else acc += static_cast<double>(v);
+  }
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_down_sync(0xffffffffu, acc, o);
+  if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = acc;
+  if (bad) s_bad = 1;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+    for (int k = 0; k < 8; k++) t += s_part[k];
+    atomicAdd(total, t);
+    if (s_bad) atomicOr(flags, 1u);
+  }
+}
+
+cudaError_t launch_check_weights(const float* w, uint32_t n, uint32_t* flags, double* total, cudaStream_t st) {
+  if (n == 0) return cudaSuccess;
+  const unsigned grid = std::min(cdiv(n, 256), device_sms() * 8u);
+  check_weights_kernel<<<grid, 256, 0, st>>>(w, n, flags, total);
   return cudaGetLastError();
 }
 
@@ -853,10 +1018,31 @@ cudaError_t launch_plusplus_step(int metric, const float* X, uint32_t n, int D, 
 // ------------------------------------------------------------------------------------------------
 constexpr int kPpBlock = 256;
 
-template <int METRIC>
+// WEIGHTED (sample weights): the draw is proportional to w_i * d_i -- dists[] keeps d_i, the block sums and the walks of
+// pp_pick_kernel / pp_prefix use w_i * d_i (the same number as d_i when w_i = 1)
+template <bool WEIGHTED>
+__device__ __forceinline__ double pp_mass(const float* __restrict__ dists, const float* __restrict__ w, uint32_t u) {
+  const float d = dists[u];
+  if (!(d == d)) return 0.0;
+  return WEIGHTED ? static_cast<double>(d * w[u]) : static_cast<double>(d);
+}
+
+// The reference's walk can land on a sample of zero mass (its backward branch picks t - 1, and a draw of exactly 0
+// stops before the first sample).  A weighted seeding never picks a zero-weight row: such a pick moves to the next
+// positive-weight row, or the previous one at the end (a positive weight exists: the call validated the weights).
+__device__ __forceinline__ uint32_t skip_zero_weight(const float* __restrict__ w, uint32_t n, uint32_t s) {
+  if (w[s] > 0.f) return s;
+  for (uint32_t u = s + 1; u < n; u++)
+    if (w[u] > 0.f) return u;
+  for (uint32_t u = s; u-- > 0;)
+    if (w[u] > 0.f) return u;
+  return s;
+}
+
+template <int METRIC, bool WEIGHTED>
 __global__ void __launch_bounds__(kPpBlock)
 pp_update_kernel(const float* __restrict__ X, uint32_t n, int D, const float* __restrict__ centroid, int first,
-                 float* __restrict__ dists, double* __restrict__ bsum) {
+                 float* __restrict__ dists, double* __restrict__ bsum, const float* __restrict__ w) {
   __shared__ double s_part[kPpBlock / 32];
   const uint32_t i = blockIdx.x * kPpBlock + threadIdx.x;
   float dist = 0.f;
@@ -866,6 +1052,7 @@ pp_update_kernel(const float* __restrict__ X, uint32_t n, int D, const float* __
     float prev;
     if (first || dist < (prev = dists[i])) dists[i] = dist;
     else dist = prev;
+    if (WEIGHTED) dist *= w[i];
   }
   double v = (dist == dist) ? static_cast<double>(dist) : 0.0;
   for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
@@ -873,26 +1060,26 @@ pp_update_kernel(const float* __restrict__ X, uint32_t n, int D, const float* __
   __syncthreads();
   if (threadIdx.x == 0) {
     double t = 0.0;
-    for (int w = 0; w < kPpBlock / 32; w++) t += s_part[w];
+    for (int k = 0; k < kPpBlock / 32; k++) t += s_part[k];
     bsum[blockIdx.x] = t;            // deterministic (fixed order), unlike an atomic total
   }
 }
 
 // prefix P(t) = sum of the first t distances, from the scanned block sums + the tail of one block
-__device__ double pp_prefix(const float* __restrict__ dists, const double* __restrict__ bpre, uint32_t t) {
+template <bool WEIGHTED>
+__device__ double pp_prefix(const float* __restrict__ dists, const float* __restrict__ w,
+                            const double* __restrict__ bpre, uint32_t t) {
   const uint32_t b = t / kPpBlock;
   double p = bpre[b];
-  for (uint32_t u = b * kPpBlock; u < t; u++) {
-    const float d = dists[u];
-    if (d == d) p += static_cast<double>(d);
-  }
+  for (uint32_t u = b * kPpBlock; u < t; u++) p += pp_mass<WEIGHTED>(dists, w, u);
   return p;
 }
 
+template <bool WEIGHTED>
 __global__ void __launch_bounds__(1024)
 pp_pick_kernel(const float* __restrict__ X, uint32_t n, int D, const float* __restrict__ dists,
                const double* __restrict__ bsum, double* __restrict__ bpre, uint32_t nb, double choice,
-               float* __restrict__ next_centroid, uint32_t* __restrict__ chosen_out) {
+               float* __restrict__ next_centroid, uint32_t* __restrict__ chosen_out, const float* __restrict__ w) {
   __shared__ double s_chunk[1024];
   __shared__ double s_total;
   __shared__ uint32_t s_j;
@@ -927,7 +1114,7 @@ pp_pick_kernel(const float* __restrict__ X, uint32_t n, int D, const float* __re
     uint32_t j;
     // smallest j >= from with P(j) >= cs (n if none): binary search over the block prefixes, then inside the block
     auto first_reaching = [&](uint32_t from) -> uint32_t {
-      if (pp_prefix(dists, bpre, from) >= cs) return from;
+      if (pp_prefix<WEIGHTED>(dists, w, bpre, from) >= cs) return from;
       uint32_t blo = from / kPpBlock, bhi = nb;          // invariant: prefix at block start blo < cs <= ... search block
       while (blo + 1 < bhi) {
         const uint32_t mid = blo + (bhi - blo) / 2;
@@ -935,17 +1122,15 @@ pp_pick_kernel(const float* __restrict__ X, uint32_t n, int D, const float* __re
       }
       double p = bpre[blo];
       uint32_t u = blo * kPpBlock;
-      if (u < from) { p = pp_prefix(dists, bpre, from); u = from; }
+      if (u < from) { p = pp_prefix<WEIGHTED>(dists, w, bpre, from); u = from; }
       const uint32_t end = min(n, (blo + 1) * kPpBlock);
       for (; u < end; u++) {
-        const float d = dists[u];
-        if (d == d) p += static_cast<double>(d);
+        p += pp_mass<WEIGHTED>(dists, w, u);
         if (p >= cs) return u + 1;
       }
       // rounding left the crossing in the next block (or nowhere): continue linearly
       for (; u < n; u++) {
-        const float d = dists[u];
-        if (d == d) p += static_cast<double>(d);
+        p += pp_mass<WEIGHTED>(dists, w, u);
         if (p >= cs) return u + 1;
       }
       return n;
@@ -954,14 +1139,13 @@ pp_pick_kernel(const float* __restrict__ X, uint32_t n, int D, const float* __re
       j = first_reaching(0);                                              // kmcuda.cc:298-302
     } else {
       ca = min(ca, n - 1);
-      const double s2 = pp_prefix(dists, bpre, ca);
+      const double s2 = pp_prefix<WEIGHTED>(dists, w, bpre, ca);
       if (s2 < cs) {
         j = first_reaching(ca);                                           // kmcuda.cc:309-313
       } else {
         // backward walk (kmcuda.cc:314-320): it subtracts d[ca], d[ca-1], ... from P(ca) until the sum drops below the
         // draw or j reaches 1, i.e. it stops at the largest t <= ca with P(t) - d[ca] < cs, and picks sample t - 1
-        const float dca = dists[ca];
-        const double lim = cs + ((dca == dca) ? static_cast<double>(dca) : 0.0);
+        const double lim = cs + pp_mass<WEIGHTED>(dists, w, ca);
         // largest t <= ca with P(t) < lim: the block by binary search over the block prefixes (P at block starts),
         // then a scan inside that block
         uint32_t tlo = 0;
@@ -974,8 +1158,7 @@ pp_pick_kernel(const float* __restrict__ X, uint32_t n, int D, const float* __re
           double pcur = bpre[blo];
           tlo = blo * kPpBlock;
           while (tlo < ca) {
-            const float d = dists[tlo];
-            const double pn = pcur + ((d == d) ? static_cast<double>(d) : 0.0);
+            const double pn = pcur + pp_mass<WEIGHTED>(dists, w, tlo);
             if (!(pn < lim)) break;
             pcur = pn;
             tlo++;
@@ -986,6 +1169,7 @@ pp_pick_kernel(const float* __restrict__ X, uint32_t n, int D, const float* __re
       }
     }
     if (j == 0 || j > n) j = min(max(j, 1u), n);                          // kmcuda.cc:322-327
+    if (WEIGHTED) j = 1 + skip_zero_weight(w, n, j - 1);
     s_j = j - 1;
     *chosen_out = j - 1;
   }
@@ -996,12 +1180,20 @@ pp_pick_kernel(const float* __restrict__ X, uint32_t n, int D, const float* __re
 
 // one k-means++ round on the device: distances to C[i-1], pick sample for C[i]
 cudaError_t launch_plusplus_round(int metric, const float* X, uint32_t n, int D, float* C, uint32_t i, double choice,
-                                  float* dists, double* bsum, double* bpre, uint32_t* chosen, cudaStream_t st) {
+                                  float* dists, double* bsum, double* bpre, uint32_t* chosen, cudaStream_t st,
+                                  const float* w) {
   const uint32_t nb = cdiv(n, kPpBlock);
   const float* cprev = C + static_cast<size_t>(i - 1) * D;
-  if (metric == 1) pp_update_kernel<1><<<nb, kPpBlock, 0, st>>>(X, n, D, cprev, i == 1, dists, bsum);
-  else pp_update_kernel<0><<<nb, kPpBlock, 0, st>>>(X, n, D, cprev, i == 1, dists, bsum);
-  pp_pick_kernel<<<1, 1024, 0, st>>>(X, n, D, dists, bsum, bpre, nb, choice, C + static_cast<size_t>(i) * D, chosen + i);
+  float* cnext = C + static_cast<size_t>(i) * D;
+  if (w) {
+    if (metric == 1) pp_update_kernel<1, true><<<nb, kPpBlock, 0, st>>>(X, n, D, cprev, i == 1, dists, bsum, w);
+    else pp_update_kernel<0, true><<<nb, kPpBlock, 0, st>>>(X, n, D, cprev, i == 1, dists, bsum, w);
+    pp_pick_kernel<true><<<1, 1024, 0, st>>>(X, n, D, dists, bsum, bpre, nb, choice, cnext, chosen + i, w);
+    return cudaGetLastError();
+  }
+  if (metric == 1) pp_update_kernel<1, false><<<nb, kPpBlock, 0, st>>>(X, n, D, cprev, i == 1, dists, bsum, nullptr);
+  else pp_update_kernel<0, false><<<nb, kPpBlock, 0, st>>>(X, n, D, cprev, i == 1, dists, bsum, nullptr);
+  pp_pick_kernel<false><<<1, 1024, 0, st>>>(X, n, D, dists, bsum, bpre, nb, choice, cnext, chosen + i, nullptr);
   return cudaGetLastError();
 }
 
