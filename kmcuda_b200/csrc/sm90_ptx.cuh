@@ -53,14 +53,15 @@ __device__ __forceinline__ bool mbar_try_wait_nohint(uint32_t addr, uint32_t par
       : "memory");
   return done != 0;
 }
-// Out-of-line remainder of every wait: a tight polling loop (a hinted try_wait returns on every update of the
-// barrier, not only when the phase flips, so the error word and the clock are checked only every 1024 probes).
+// Remainder of every wait: a tight polling loop (a hinted try_wait returns on every update of the barrier, not only
+// when the phase flips, so the error word and the clock are checked only every 1024 probes).  Inlined: under setmaxnreg,
+// ptxas cannot allocate a call made while wgmma accumulators are in flight.
 // `site` names the waiting role; after ~2 s (or as soon as another thread has reported an error) the wait gives up
 // and reports 0x1000 + site in *err: a stuck pipeline must not hang the GPU.
 #ifndef KMB_SLOW_HINT_NS
 #define KMB_SLOW_HINT_NS 20000
 #endif
-__device__ __noinline__ void mbar_wait_slow(uint32_t addr, uint32_t parity, uint32_t* err, uint32_t site, uint32_t flag_u32) {
+__device__ __forceinline__ void mbar_wait_slow(uint32_t addr, uint32_t parity, uint32_t* err, uint32_t site, uint32_t flag_u32) {
   // flag_u32: a word of this CTA's shared memory that is set once any wait of the CTA has given up; from then on every
   // wait returns at once, so a broken pipeline drains in milliseconds instead of timing out wait by wait
   uint32_t dead;
@@ -208,6 +209,13 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc,
       : "l"(adesc), "l"(bdesc), "r"(accumulate)
       : "memory");
 }
+
+// per-warpgroup register budget (every warp of the warpgroup executes it): .dec hands registers back to the CTA's pool,
+// .inc waits until the pool can grant the new count
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 __device__ __forceinline__ float4 ldg_nc_f4(const float* p) {
   float4 v;
