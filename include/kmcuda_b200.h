@@ -30,6 +30,17 @@ extern "C" {
 
 typedef struct kmcuda_b200_shard kmcuda_b200_shard;
 
+/* Extra KMCUDAInitMethod value accepted by kmeans_cuda() and kmcuda_b200_kmeans_weighted(): k-means|| seeding
+ * (Bahmani et al., "Scalable K-Means++", VLDB 2012).  init_params -> uint32_t rounds (NULL or 0 = 5; above 32 is
+ * kmcudaInvalidArguments).  c0 is k-means++'s first centroid (srand(seed), rand() % N, redrawn on NaN / zero-weight
+ * rows).  Each round draws every row independently with probability 2K w d^2 / sum(w d^2), d = true distance to the
+ * nearest candidate so far, through a counter hash of (seed, round, row), so the draws are the same on any number of
+ * GPUs; it then runs one assignment pass against that round's candidates.  The candidates, each weighted by the total
+ * sample weight nearest to it, are clustered to K by kmcuda_b200_kmeans_weighted(k-means++, tolerance 0.01,
+ * yinyang_t 0, same metric and seed) on the first device; with at most K candidates they are the first centroids and
+ * random init's walk from srand(seed) fills the rest.  Verbosity >= 1 logs one "k-means|| round" line per round. */
+#define kmcudaInitMethodKMeansParallel ((KMCUDAInitMethod)4)
+
 /* kmeans_cuda() with a weight per sample (scikit-learn's sample_weight).  The parameters are those of kmeans_cuda(),
  * plus `weights`: [samples_size] fp32, a host pointer when device_ptrs < 0 and device memory on device `device_ptrs`
  * otherwise (the rule for `samples`; fp32 in fp16x2 mode too).  weights == NULL is the unweighted run.

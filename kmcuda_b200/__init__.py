@@ -5,6 +5,7 @@ Python surface = the reference's `libKMCUDA` module (reference src/python.cc:33-
     kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1, metric="L2",
                 average_distance=False, seed=time(), device=0, verbosity=0,   # python.cc:159-410
                 sample_weight=None)                                           # extension: per-sample weights
+                init="k-means||" / ("k-means||", rounds)                      # extension: k-means|| seeding
     knn_cuda(k, samples, centroids, assignments, metric="L2", device=0, verbosity=0)  # python.cc:412-632
     supports_fp16                                                             # python.cc:52
 
@@ -49,10 +50,13 @@ supports_fp16 = True
 # enums of include/kmcuda.h
 SUCCESS, INVALID_ARGUMENTS, NO_SUCH_DEVICE, MEMORY_ALLOCATION_FAILURE, RUNTIME_ERROR, MEMORY_COPY_ERROR = range(6)
 INIT_RANDOM, INIT_PLUSPLUS, INIT_AFKMC2, INIT_IMPORT = range(4)
+INIT_KMEANS_PARALLEL = 4   # include/kmcuda_b200.h: kmcudaInitMethodKMeansParallel
+KMEANS_PARALLEL_MAX_ROUNDS = 32
 METRIC_L2, METRIC_COSINE = range(2)
 
 _INIT_METHODS = {"kmeans++": INIT_PLUSPLUS, "k-means++": INIT_PLUSPLUS, "afkmc2": INIT_AFKMC2,
-                 "afk-mc2": INIT_AFKMC2, "random": INIT_RANDOM}
+                 "afk-mc2": INIT_AFKMC2, "random": INIT_RANDOM, "k-means||": INIT_KMEANS_PARALLEL,
+                 "kmeans||": INIT_KMEANS_PARALLEL}
 _METRICS = {"euclidean": METRIC_L2, "L2": METRIC_L2, "l2": METRIC_L2, "cos": METRIC_COSINE,
             "cosine": METRIC_COSINE, "angular": METRIC_COSINE}
 
@@ -114,6 +118,15 @@ def _get_sample_weight(sample_weight, n, device_ptrs):
     return arr, arr.ctypes.data
 
 
+def _kmeans_parallel_rounds(rounds):
+    """the rounds of init=("k-means||", rounds): an integer in [0, 32], 0 = the default (5)"""
+    if isinstance(rounds, bool) or not isinstance(rounds, (int, np.integer)):
+        raise ValueError("k-means|| rounds must be an integer, got %r" % (rounds,))
+    if not 0 <= rounds <= KMEANS_PARALLEL_MAX_ROUNDS:
+        raise ValueError("k-means|| rounds must be in [0, %d], got %d" % (KMEANS_PARALLEL_MAX_ROUNDS, rounds))
+    return int(rounds)
+
+
 def _raise_for(result, fn):
     if result == SUCCESS:
         return
@@ -156,6 +169,8 @@ def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1
         init_method = _INIT_METHODS[init[0]]
         if len(init) > 1 and init_method == INIT_AFKMC2:
             afkmc2_m = ctypes.c_uint32(int(init[1]))
+        if len(init) > 1 and init_method == INIT_KMEANS_PARALLEL:
+            afkmc2_m = ctypes.c_uint32(_kmeans_parallel_rounds(init[1]))
     else:
         init_method = INIT_IMPORT
     metric_id = _get_metric(metric)

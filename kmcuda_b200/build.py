@@ -20,7 +20,8 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libKMCUDA.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
-CU_SOURCES = ["simt_kernels.cu", "knn_kernels.cu", "assign_tc.cu", "yinyang.cu", "shard.cu", "exchange.cu", "api.cu"]
+CU_SOURCES = ["simt_kernels.cu", "knn_kernels.cu", "assign_tc.cu", "yinyang.cu", "shard.cu", "exchange.cu",
+              "kmeans_parallel.cu", "api.cu"]
 CC_SOURCES = ["py_module.cc"]
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

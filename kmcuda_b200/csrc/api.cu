@@ -35,6 +35,8 @@ namespace kmb {
 static const float kYinyangGroupTolerance = 0.02f;      // reference kmeans.cu:27
 static const float kYinyangDraftReassignments = 0.11f;  // reference kmeans.cu:28
 static const float kYinyangRefreshEpsilon = 1e-4f;      // reference kmeans.cu:29
+static const uint32_t kKMeansParallelRounds = 5;        // k-means|| rounds when init_params gives none
+static const uint32_t kKMeansParallelMaxRounds = 32;    // the round number is 8 bits of the draw hash's key
 
 // NCCL is resolved lazily with dlopen the first time a job spans more than one GPU.  Linking it
 // would either pin a second libnccl.so.2 into processes that also import torch (which ships its own,
@@ -326,6 +328,7 @@ class Job {
   KMCUDAResult init_random();
   KMCUDAResult init_plusplus();
   KMCUDAResult init_afkmc2(uint32_t m, uint32_t seed);
+  KMCUDAResult init_kmeans_parallel(uint32_t rounds, uint32_t seed);
   KMCUDAResult assign_pass(uint32_t* changed);
   KMCUDAResult update();
   KMCUDAResult lloyd(float tolerance, int* iter_out, uint32_t* changed_out);
@@ -548,18 +551,23 @@ KMCUDAResult Job::fetch_row(uint32_t idx, float* host_row) {
   return kmcudaRuntimeError;
 }
 
-// K distinct random samples; same host RNG walk as the reference (kmcuda.cc:245-260):
-// identity permutation shuffled with rand() the way libstdc++'s std::random_shuffle does.
-// Weighted: the walk over the shuffled order skips rows of weight 0.
-KMCUDAResult Job::init_random() {
-  KMB_INFO("randomly picking initial centroids...\n");
-  KMB_RET(load_host_weights());
+// identity permutation of N rows shuffled with rand() the way libstdc++'s std::random_shuffle does (kmcuda.cc:245-260)
+static std::vector<uint32_t> random_order(uint32_t N) {
   std::vector<uint32_t> chosen(N);
   for (uint32_t s = 0; s < N; s++) chosen[s] = s;
   for (uint32_t i = 1; i < N; i++) {
     uint32_t j = static_cast<uint32_t>(rand() % (static_cast<int64_t>(i) + 1));
     if (i != j) std::swap(chosen[i], chosen[j]);
   }
+  return chosen;
+}
+
+// K distinct random samples; same host RNG walk as the reference (kmcuda.cc:245-260).
+// Weighted: the walk over the shuffled order skips rows of weight 0.
+KMCUDAResult Job::init_random() {
+  KMB_INFO("randomly picking initial centroids...\n");
+  KMB_RET(load_host_weights());
+  const std::vector<uint32_t> chosen = random_order(N);
   std::vector<float> hostC(static_cast<size_t>(K) * D);
   uint32_t c = 0;
   for (uint32_t s = 0; s < N && c < K; s++) {
@@ -803,6 +811,230 @@ KMCUDAResult Job::init_afkmc2(uint32_t m, uint32_t seed) {
   return set_centroids_from_host(hostC.data());
 }
 
+// k-means|| (Bahmani et al., "Scalable K-Means++", VLDB 2012; DESIGN.md §4g).  c0 is k-means++'s first centroid; each
+// of `rounds` rounds draws every row independently with probability l w_i d_i^2 / phi (l = 2K, d_i the true distance
+// to the nearest candidate so far, phi = sum w_i d_i^2), runs one assignment pass against the round's new candidates
+// only and lowers d_i where the winner is closer.  The candidates, weighted by the sample weight they are nearest to,
+// are then clustered down to K by the library's own weighted k-means++ / Lloyd run; with at most K candidates they are
+// the centroids and init_random's walk fills the rest.  Every shard draws its own rows with a counter hash of the
+// global row index, so the draws do not depend on the device split.
+KMCUDAResult Job::init_kmeans_parallel(uint32_t rounds, uint32_t seed) {
+  std::vector<float> cand(D);          // the candidate rows in list order (round, row index), host copy
+  std::vector<uint32_t> cand_rows(1);  // their global row indices
+  KMB_RET(draw_first_centroid(cand.data(), &cand_rows[0]));
+  struct Work {
+    DevBuf<float> table, gathered;     // this round's candidates (all shards'), this shard's drawn rows
+    DevBuf<uint32_t> nearest, idx, count;
+    DevBuf<double> bsum, phi;
+    DevBuf<uint8_t> flags;
+    DevBuf<char> tmp;
+    size_t tmp_bytes = 0;
+    uint32_t nb = 0, drawn = 0;
+  };
+  std::vector<Work> wk(devs.size());
+  for (size_t s = 0; s < devs.size(); s++) {
+    Dev& d = devs[s];
+    Work& w = wk[s];
+    KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+    w.nb = kmp_blocks(d.len);
+    w.tmp_bytes = kmp_select_bytes(d.len);
+    KMB_CU(d.dists.alloc(d.len), kmcudaMemoryAllocationFailure);
+    KMB_CU(w.nearest.alloc(d.len), kmcudaMemoryAllocationFailure);
+    KMB_CU(w.idx.alloc(d.len), kmcudaMemoryAllocationFailure);
+    KMB_CU(w.count.alloc(1), kmcudaMemoryAllocationFailure);
+    KMB_CU(w.bsum.alloc(w.nb), kmcudaMemoryAllocationFailure);
+    KMB_CU(w.phi.alloc(1), kmcudaMemoryAllocationFailure);
+    KMB_CU(w.flags.alloc(d.len), kmcudaMemoryAllocationFailure);
+    KMB_CU(w.tmp.alloc(w.tmp_bytes), kmcudaMemoryAllocationFailure);
+    KMB_CU(w.table.alloc(D), kmcudaMemoryAllocationFailure);
+    KMB_CU(cudaMemcpyAsync(w.table.get(), cand.data(), sizeof(float) * D, cudaMemcpyHostToDevice, d.st),
+           kmcudaMemoryCopyError);
+    KMB_CU(launch_kmp_update(metric, d.X, d.len, D, w.table, 1, nullptr, 0, d.dists, w.nearest, d.w.get(), w.bsum, d.st),
+           kmcudaRuntimeError);
+    KMB_CU(launch_kmp_sum(w.bsum, w.nb, w.phi, d.st), kmcudaRuntimeError);
+  }
+  const double ell = 2.0 * K;
+  for (uint32_t r = 1; r <= rounds; r++) {
+    double phi = 0;
+    for (auto& w : wk) w.drawn = 0;
+    for (size_t s = 0; s < devs.size(); s++) {   // device order: the same total on every run
+      double part = 0;
+      KMB_CU(cudaSetDevice(devs[s].dev), kmcudaRuntimeError);
+      KMB_CU(cudaMemcpyAsync(&part, wk[s].phi.get(), sizeof(double), cudaMemcpyDeviceToHost, devs[s].st),
+             kmcudaMemoryCopyError);
+      KMB_CU(cudaStreamSynchronize(devs[s].st), kmcudaRuntimeError);
+      phi += part;
+    }
+    if (!(phi > 0)) break;   // every row sits on a candidate
+    for (size_t s = 0; s < devs.size(); s++) {
+      Dev& d = devs[s];
+      Work& w = wk[s];
+      KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+      KMB_CU(launch_kmp_draw(d.dists, d.w.get(), d.len, d.off, seed, r, ell, phi, w.flags, w.idx, w.count, w.tmp,
+                             w.tmp_bytes, d.st), kmcudaRuntimeError);
+      KMB_CU(cudaMemcpyAsync(&w.drawn, w.count.get(), sizeof(uint32_t), cudaMemcpyDeviceToHost, d.st),
+             kmcudaMemoryCopyError);
+    }
+    KMB_RET(sync_all());
+    const uint32_t base = static_cast<uint32_t>(cand_rows.size());
+    uint32_t fresh = 0;
+    for (auto& w : wk) fresh += w.drawn;
+    KMB_INFO("k-means|| round %" PRIu32 ": %" PRIu32 " candidates, cost %.17g\n", r, fresh, phi);
+    if (fresh == 0) continue;   // nothing changes: the next round draws again from the same d
+    // gather each shard's drawn rows, then every device gets the whole round's table in device (= row) order
+    cand_rows.resize(base + fresh);
+    for (size_t s = 0, at = base; s < devs.size(); s++) {
+      Dev& d = devs[s];
+      Work& w = wk[s];
+      if (w.drawn == 0) continue;
+      KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+      KMB_CU(w.gathered.alloc(static_cast<size_t>(w.drawn) * D), kmcudaMemoryAllocationFailure);
+      KMB_CU(launch_kmp_gather(d.X, D, w.idx, w.drawn, w.gathered, d.st), kmcudaRuntimeError);
+      KMB_CU(cudaMemcpyAsync(cand_rows.data() + at, w.idx.get(), sizeof(uint32_t) * w.drawn, cudaMemcpyDeviceToHost,
+                             d.st), kmcudaMemoryCopyError);
+      at += w.drawn;
+    }
+    KMB_RET(sync_all());
+    for (size_t s = 0, at = base; s < devs.size(); s++) {
+      for (uint32_t j = 0; j < wk[s].drawn; j++) cand_rows[at + j] += devs[s].off;
+      at += wk[s].drawn;
+    }
+    for (size_t t = 0; t < devs.size(); t++) {
+      Dev& d = devs[t];
+      KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+      KMB_CU(wk[t].table.alloc(static_cast<size_t>(fresh) * D), kmcudaMemoryAllocationFailure);
+      size_t at = 0;
+      for (size_t s = 0; s < devs.size(); s++) {
+        if (wk[s].drawn == 0) continue;
+        KMB_CU(cudaMemcpyPeerAsync(wk[t].table.get() + at * D, d.dev, wk[s].gathered.get(), devs[s].dev,
+                                   sizeof(float) * wk[s].drawn * D, d.st), kmcudaMemoryCopyError);
+        at += wk[s].drawn;
+      }
+    }
+    cand.resize(static_cast<size_t>(base + fresh) * D);
+    KMB_CU(cudaSetDevice(devs[0].dev), kmcudaRuntimeError);
+    KMB_CU(cudaMemcpyAsync(cand.data() + static_cast<size_t>(base) * D, wk[0].table.get(),
+                           sizeof(float) * static_cast<size_t>(fresh) * D, cudaMemcpyDeviceToHost, devs[0].st),
+           kmcudaMemoryCopyError);
+    KMB_RET(sync_all());   // (the peer copies have read every `gathered` buffer)
+    // one assignment pass of every shard against the round's candidates, then the running-minimum update
+    std::vector<std::unique_ptr<Shard>> pass(devs.size());
+    for (size_t s = 0; s < devs.size(); s++) {
+      Dev& d = devs[s];
+      Work& w = wk[s];
+      pass[s].reset(new Shard(metric, d.dev, d.len, D, fresh, verbosity));
+      KMB_RET(pass[s]->create(false));
+      KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+      KMB_CU(cudaMemsetAsync(d.assign.get(), 0xff, sizeof(uint32_t) * d.len, d.st), kmcudaRuntimeError);
+      KMB_RET(pass[s]->assign(d.len, d.X, w.table, d.assign, d.prev, d.d_changed, d.st));
+      KMB_CU(launch_kmp_update(metric, d.X, d.len, D, w.table, fresh, d.assign, base, d.dists, w.nearest, d.w.get(),
+                               w.bsum, d.st), kmcudaRuntimeError);
+      KMB_CU(launch_kmp_sum(w.bsum, w.nb, w.phi, d.st), kmcudaRuntimeError);
+    }
+    KMB_RET(sync_all());
+    for (auto& p : pass) KMB_RET(p->check_pipeline());
+  }
+  const uint32_t Cn = static_cast<uint32_t>(cand_rows.size());
+  KMB_INFO("k-means||: %" PRIu32 " candidates -> %" PRIu32 " centroids\n", Cn, K);
+  g_prof.mark("init: k-means|| rounds");
+  std::vector<float> hostC(static_cast<size_t>(K) * D);
+  if (Cn <= K) {
+    // the candidates, then init_random's walk from srand(seed) over the rows not chosen yet (and of positive weight)
+    memcpy(hostC.data(), cand.data(), sizeof(float) * static_cast<size_t>(Cn) * D);
+    std::vector<char> taken(N, 0);
+    for (uint32_t i : cand_rows) taken[i] = 1;
+    srand(seed);
+    const std::vector<uint32_t> order = random_order(N);
+    uint32_t c = Cn;
+    for (uint32_t s = 0; s < N && c < K; s++) {
+      const uint32_t i = order[s];
+      if (taken[i] || (weighted && !(host_w[i] > 0.f))) continue;
+      KMB_RET(fetch_row(i, hostC.data() + static_cast<size_t>(c) * D));
+      c++;
+    }
+    if (c < K) {
+      KMB_INFO("k-means||: only %" PRIu32 " samples have a positive weight, %" PRIu32 " clusters\n", c, K);
+      return kmcudaInvalidArguments;
+    }
+    for (auto& d : devs) d.dists.release();
+    KMB_RET(set_centroids_from_host(hostC.data()));
+    g_prof.mark("init: k-means|| recluster");
+    return kmcudaSuccess;
+  }
+  // candidate weights W_j = sum of w_i over the rows nearest to candidate j: exact counts, or compensated fp32 sums per
+  // device added in device order (the weighted update's rule)
+  std::vector<float> W(Cn, 0.f);
+  {
+    std::vector<uint32_t> total(Cn, 0), part_u(Cn);
+    std::vector<float> part_f(Cn);
+    for (size_t s = 0; s < devs.size(); s++) {
+      Dev& d = devs[s];
+      Work& w = wk[s];
+      KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+      if (weighted) {
+        DevBuf<uint32_t> keys, start;
+        DevBuf<float> wsorted, Wd;
+        const size_t bytes = kmp_weights_bytes(d.len);
+        KMB_CU(keys.alloc(d.len), kmcudaMemoryAllocationFailure);
+        KMB_CU(start.alloc(2 * static_cast<size_t>(Cn)), kmcudaMemoryAllocationFailure);
+        KMB_CU(wsorted.alloc(d.len), kmcudaMemoryAllocationFailure);
+        KMB_CU(Wd.alloc(Cn), kmcudaMemoryAllocationFailure);
+        KMB_CU(w.tmp.alloc(bytes), kmcudaMemoryAllocationFailure);
+        KMB_CU(launch_kmp_weights(w.nearest, d.w, d.len, Cn, keys, wsorted, start, w.tmp, bytes, Wd, d.st),
+               kmcudaRuntimeError);
+        KMB_CU(cudaMemcpyAsync(part_f.data(), Wd.get(), sizeof(float) * Cn, cudaMemcpyDeviceToHost, d.st),
+               kmcudaMemoryCopyError);
+        KMB_CU(cudaStreamSynchronize(d.st), kmcudaRuntimeError);
+        for (uint32_t j = 0; j < Cn; j++) W[j] += part_f[j];
+      } else {
+        DevBuf<uint32_t> counts;
+        KMB_CU(counts.alloc(Cn), kmcudaMemoryAllocationFailure);
+        KMB_CU(cudaMemsetAsync(counts.get(), 0, sizeof(uint32_t) * Cn, d.st), kmcudaRuntimeError);
+        KMB_CU(launch_kmp_counts(w.nearest, d.len, counts, d.st), kmcudaRuntimeError);
+        KMB_CU(cudaMemcpyAsync(part_u.data(), counts.get(), sizeof(uint32_t) * Cn, cudaMemcpyDeviceToHost, d.st),
+               kmcudaMemoryCopyError);
+        KMB_CU(cudaStreamSynchronize(d.st), kmcudaRuntimeError);
+        for (uint32_t j = 0; j < Cn; j++) total[j] += part_u[j];
+      }
+    }
+    if (!weighted)
+      for (uint32_t j = 0; j < Cn; j++) W[j] = static_cast<float>(total[j]);
+  }
+  for (auto& d : devs) d.dists.release();
+  wk.clear();
+  // recluster: the steps of kmcuda_b200_kmeans_weighted(k-means++, tolerance 0.01, yinyang_t 0, metric, seed,
+  // verbosity 0) on the candidate rows on the first device, with the same result.  Its phases stay out of the caller's
+  // profile and log.  Two checks of the public call do not apply to the nested run:
+  // - the unit-length probe of angular samples: the call's own samples passed it or were fp16x2, whose widened rows
+  //   are unit length only to fp16 precision;
+  // - KMCUDA_B200_STRICT_UPDATE=1, which replays the reference's unweighted update and would drop the weights W.
+  {
+    const bool prof = g_prof.on;
+    g_prof.on = false;
+    Job sub(metric, Cn, D, K, 0);
+    sub.weighted = true;
+    KMCUDAResult res = sub.setup({devs[0].dev}, true);
+    if (res == kmcudaSuccess) {
+      sub.devs[0].shard->strict_update = false;
+      res = sub.ingest(cand.data(), W.data(), -1, false);
+    }
+    if (res == kmcudaSuccess) res = sub.check_weights();
+    if (res == kmcudaSuccess) {
+      srand(seed);
+      res = sub.init_plusplus();
+    }
+    if (res == kmcudaSuccess) res = sub.yinyang(0.01f, 0);
+    g_prof.on = prof;
+    KMB_RET(res);
+    KMB_CU(cudaSetDevice(devs[0].dev), kmcudaRuntimeError);
+    KMB_CU(cudaMemcpy(hostC.data(), sub.devs[0].C.get(), sizeof(float) * hostC.size(), cudaMemcpyDeviceToHost),
+           kmcudaMemoryCopyError);
+  }
+  KMB_RET(set_centroids_from_host(hostC.data()));
+  g_prof.mark("init: k-means|| recluster");
+  return kmcudaSuccess;
+}
+
 KMCUDAResult Job::init_centroids(KMCUDAInitMethod method, const void* init_params, uint32_t seed,
                                  int device_ptrs, bool fp16x2, const float* user_centroids) {
   if (metric == 1 && !fp16x2) {  // three probe samples must be unit length (kmcuda.cc:195-219)
@@ -859,6 +1091,11 @@ KMCUDAResult Job::init_centroids(KMCUDAInitMethod method, const void* init_param
         return kmcudaInvalidArguments;
       }
       KMB_RET(init_afkmc2(m, seed));
+      break;
+    }
+    case kmcudaInitMethodKMeansParallel: {
+      const uint32_t r = init_params ? *reinterpret_cast<const uint32_t*>(init_params) : 0;
+      KMB_RET(init_kmeans_parallel(r ? r : kKMeansParallelRounds, seed));   // (r <= 32: kmeans_impl)
       break;
     }
     default:
@@ -1199,6 +1436,9 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
   if (!(tolerance >= 0 && tolerance <= 1)) return kmcudaInvalidArguments;
   if (!(yinyang_t >= 0 && yinyang_t <= 0.5)) return kmcudaInvalidArguments;
   if (static_cast<uint64_t>(features_size) * (fp16x2 ? 2 : 1) > 65535u) return kmcudaInvalidArguments;
+  if (init == kmcudaInitMethodKMeansParallel && init_params &&
+      *static_cast<const uint32_t*>(init_params) > kKMeansParallelMaxRounds)
+    return kmcudaInvalidArguments;
   if (weights) {
     // strict mode replays the reference's unweighted running sums; there is no weighted reference to replay
     const char* su = getenv("KMCUDA_B200_STRICT_UPDATE");

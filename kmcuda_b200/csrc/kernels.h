@@ -131,6 +131,31 @@ cudaError_t launch_plusplus_step(int metric, const float* X, uint32_t n, int D, 
 cudaError_t launch_plusplus_round(int metric, const float* X, uint32_t n, int D, float* C, uint32_t i, double choice,
                                   float* dists, double* bsum, double* bpre, uint32_t* chosen, cudaStream_t st,
                                   const float* w = nullptr);
+// ---- k-means|| seeding (kmeans_parallel.cu) -------------------------------------------------------------------------
+// running-minimum update of a round: assign == nullptr is the start (every row against cand[0] = c0, nearest = 0),
+// otherwise row i compares its true distance to cand[assign[i]] (assign[i] < ncand) with dists[i] and on e < d takes
+// nearest[i] = base + assign[i].  bsum[kmp_blocks(n)] receives the per-block partials of sum w_i d_i^2 (w optional).
+uint32_t kmp_blocks(uint32_t n);
+cudaError_t launch_kmp_update(int metric, const float* X, uint32_t n, int D, const float* cand, uint32_t ncand,
+                              const uint32_t* assign, uint32_t base, float* dists, uint32_t* nearest, const float* w,
+                              double* bsum, cudaStream_t st);
+// *out = the block partials added in a fixed order
+cudaError_t launch_kmp_sum(const double* bsum, uint32_t nb, double* out, cudaStream_t st);
+// the draw of round `round`: flags[i] = u(seed, round, off + i) < ell * w_i d_i^2 / phi; idx[0 .. *d_count) = the
+// drawn local row ids, ascending.  tmp: kmp_select_bytes(n) bytes
+size_t kmp_select_bytes(uint32_t n);
+cudaError_t launch_kmp_draw(const float* dists, const float* w, uint32_t n, uint32_t off, uint32_t seed, uint32_t round,
+                            double ell, double phi, uint8_t* flags, uint32_t* idx, uint32_t* d_count, void* tmp,
+                            size_t tmp_bytes, cudaStream_t st);
+// out[j][:] = X[idx[j]][:]
+cudaError_t launch_kmp_gather(const float* X, int D, const uint32_t* idx, uint32_t cnt, float* out, cudaStream_t st);
+// candidate weights: counts[nearest[i]] += 1 (counts zeroed by the caller), or with sample weights W[C] = compensated
+// fp32 sums of w per candidate in a fixed order (keys_out / w_out [n], start [2C], tmp: kmp_weights_bytes(n) bytes)
+cudaError_t launch_kmp_counts(const uint32_t* nearest, uint32_t n, uint32_t* counts, cudaStream_t st);
+size_t kmp_weights_bytes(uint32_t n);
+cudaError_t launch_kmp_weights(const uint32_t* nearest, const float* w, uint32_t n, uint32_t C, uint32_t* keys_out,
+                               float* w_out, uint32_t* start, void* tmp, size_t tmp_bytes, float* W, cudaStream_t st);
+
 cudaError_t launch_half_to_float(const void* src, float* dst, size_t n, cudaStream_t st);
 cudaError_t launch_float_to_half(const float* src, void* dst, size_t n, cudaStream_t st);
 cudaError_t launch_fill_u32(uint32_t* p, uint32_t v, size_t n, cudaStream_t st);

@@ -172,6 +172,10 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
   KMCUDAInitMethod init = kmcudaInitMethodPlusPlus;
   auto named_init = [&init](PyObject* o) {
     const char* s = PyUnicode_Check(o) ? PyUnicode_AsUTF8(o) : nullptr;
+    if (s && (strcmp(s, "k-means||") == 0 || strcmp(s, "kmeans||") == 0)) {   // kmcuda_b200.h, not in kmcuda.h's table
+      init = kmcudaInitMethodKMeansParallel;
+      return true;
+    }
     auto it = s ? kmcuda::init_methods.find(s) : kmcuda::init_methods.end();
     if (it == kmcuda::init_methods.end()) {
       PyErr_SetString(PyExc_ValueError, "Unknown centroids initialization method. Supported values are "
@@ -194,6 +198,23 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
     if (!named_init(first)) return nullptr;
     if (PyTuple_Size(init_obj) > 1 && init == kmcudaInitMethodAFKMC2)
       afkmc2_m = static_cast<uint32_t>(PyLong_AsUnsignedLong(PyTuple_GetItem(init_obj, 1)));
+    if (PyTuple_Size(init_obj) > 1 && init == kmcudaInitMethodKMeansParallel) {   // rounds: an integer in [0, 32]
+      PyObject* r = PyTuple_GetItem(init_obj, 1);
+      long v = -1;
+      if (PyLong_Check(r) && !PyBool_Check(r)) {
+        int overflow = 0;
+        v = PyLong_AsLongAndOverflow(r, &overflow);
+        if (overflow) v = -1;
+      } else if (PyArray_IsScalar(r, Integer)) {
+        v = PyLong_AsLong(r);
+      }
+      if (v < 0 || v > 32) {
+        PyErr_Clear();
+        PyErr_SetString(PyExc_ValueError, "k-means|| rounds must be an integer in [0, 32]");
+        return nullptr;
+      }
+      afkmc2_m = static_cast<uint32_t>(v);
+    }
   } else {
     init = kmcudaInitMethodImport;
   }
