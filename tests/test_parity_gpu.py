@@ -121,9 +121,9 @@ def _unit(a):
                                           (9000, 324, 700, "L2"), (20000, 240, 2000, "L2"),
                                           (20000, 240, 2000, "cos"), (9000, 196, 700, "L2")])
 def test_tensor_core_wide_shapes_match_reference(ref, n, d, k, metric):
-    """cosine, D up to 512 (single A buffer in shared memory; above 256 the shallow pipeline with quad-shuffle
-    regrouping), ragged last K-blocks and K >> 1024 (chunk-list compaction) through the wgmma filter: bit-identical
-    to the reference kernel"""
+    """cosine, D up to 512 (the A operand in a ring of K-block slots; above 256 the shallow pipeline with 8 slots and
+    2 B stages), ragged last K-blocks and K >> 1024 (list compaction) through the wgmma filter, whose MODE 0 epilogue
+    builds the candidate masks on the accumulator fragment as it lands: bit-identical to the reference kernel"""
     rng = np.random.default_rng(n + d + k)
     X = rng.standard_normal((n, d)).astype(np.float32)
     if metric == "cos":
