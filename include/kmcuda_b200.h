@@ -58,6 +58,27 @@ KMCUDAResult kmcuda_b200_kmeans_weighted(KMCUDAInitMethod init, const void *init
                                          const float *samples, const float *weights, float *centroids,
                                          uint32_t *assignments, float *average_distance);
 
+/* Mini-batch k-means (Sculley, "Web-scale k-means clustering", WWW 2010), scikit-learn's MiniBatchKMeans with this
+ * library's draws.  init, init_params, tolerance, metric ... weights and the outputs are those of
+ * kmcuda_b200_kmeans_weighted(); `init` runs on the full data exactly as there.  Then step s = 1, 2, ... draws
+ * b = min(batch_size, samples_size) rows with replacement, row_j = floor(u(seed, s, j) * samples_size) with u a counter
+ * hash, assigns them exactly (the reference's argmin), and for every centroid with batch weight W_b > 0 sets
+ * c = (c W + S_b) / (W + W_b), W += W_b (W starts at 0; S_b, W_b are the batch's weighted member sums).  Centroids with
+ * W < 0.01 max W (at most floor(b / 2) of the smallest) become batch rows drawn proportionally to the weight without
+ * replacement, whenever some W is 0 or 10 * clusters_size rows have been drawn since the last time; their W becomes the
+ * smallest remaining one.  The run stops after max_steps steps (0 = floor(100 * samples_size / b)), when tolerance > 0
+ * and the squared centroid move of a step is <= tolerance * the mean per-feature variance of the samples, or after 10
+ * steps without a new minimum of the smoothed batch inertia (step 1 excluded).  One full assignment pass then gives
+ * `assignments`.  Verbosity >= 1 logs one "mini-batch step" line per step and the reason it stopped.
+ * kmcudaInvalidArguments: batch_size == 0, the cosine metric, a device mask with more than one bit (0 = the first GPU),
+ * KMCUDA_B200_STRICT_UPDATE=1.  With every weight 1 the result is bit-identical to weights == NULL. */
+KMCUDAResult kmcuda_b200_kmeans_minibatch(KMCUDAInitMethod init, const void *init_params, float tolerance,
+                                          KMCUDADistanceMetric metric, uint32_t samples_size, uint16_t features_size,
+                                          uint32_t clusters_size, uint32_t seed, uint32_t device, int32_t device_ptrs,
+                                          int32_t fp16x2, int32_t verbosity, const float *samples,
+                                          const float *weights, uint32_t batch_size, uint32_t max_steps,
+                                          float *centroids, uint32_t *assignments, float *average_distance);
+
 /* Creates the per-shard workspace (fp16 centroid table, TMA descriptors, re-check queues, sort
  * buffers) for up to max_samples samples of features_size fp32 features and clusters_size clusters. */
 KMCUDAResult kmcuda_b200_shard_create(kmcuda_b200_shard **shard, KMCUDADistanceMetric metric,

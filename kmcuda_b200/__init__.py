@@ -4,7 +4,8 @@ Python surface = the reference's `libKMCUDA` module (reference src/python.cc:33-
 
     kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1, metric="L2",
                 average_distance=False, seed=time(), device=0, verbosity=0,   # python.cc:159-410
-                sample_weight=None)                                           # extension: per-sample weights
+                sample_weight=None,                                           # extension: per-sample weights
+                batch_size=None, max_steps=0)                                 # extension: mini-batch k-means
                 init="k-means||" / ("k-means||", rounds)                      # extension: k-means|| seeding
     knn_cuda(k, samples, centroids, assignments, metric="L2", device=0, verbosity=0)  # python.cc:412-632
     supports_fp16                                                             # python.cc:52
@@ -39,6 +40,9 @@ _lib.kmeans_cuda.argtypes = [
 _lib.kmcuda_b200_kmeans_weighted.restype = ctypes.c_int
 _lib.kmcuda_b200_kmeans_weighted.argtypes = _lib.kmeans_cuda.argtypes[:14] + [ctypes.c_void_p] + \
     _lib.kmeans_cuda.argtypes[14:]
+_lib.kmcuda_b200_kmeans_minibatch.restype = ctypes.c_int
+_lib.kmcuda_b200_kmeans_minibatch.argtypes = _lib.kmeans_cuda.argtypes[:3] + _lib.kmeans_cuda.argtypes[4:14] + \
+    [ctypes.c_void_p, ctypes.c_uint32, ctypes.c_uint32] + _lib.kmeans_cuda.argtypes[14:]
 _lib.knn_cuda.restype = ctypes.c_int
 _lib.knn_cuda.argtypes = [
     ctypes.c_uint16, ctypes.c_int, ctypes.c_uint32, ctypes.c_uint16, ctypes.c_uint32, ctypes.c_uint32,
@@ -127,6 +131,15 @@ def _kmeans_parallel_rounds(rounds):
     return int(rounds)
 
 
+def _count(value, name, lowest):
+    """batch_size / max_steps: an integer >= lowest that fits in 32 bits"""
+    if isinstance(value, bool) or not isinstance(value, (int, np.integer)):
+        raise TypeError("\"%s\" must be an integer, got %r" % (name, value))
+    if not lowest <= value <= 0xFFFFFFFF:
+        raise ValueError("\"%s\" must be an integer in [%d, 2^32), got %d" % (name, lowest, value))
+    return int(value)
+
+
 def _raise_for(result, fn):
     if result == SUCCESS:
         return
@@ -144,12 +157,22 @@ def _raise_for(result, fn):
 
 
 def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1, metric="L2",
-                average_distance=False, seed=None, device=0, verbosity=0, sample_weight=None):
+                average_distance=False, seed=None, device=0, verbosity=0, sample_weight=None, batch_size=None,
+                max_steps=0):
     """K-means on the GPU(s); see the module docstring.  Returns (centroids, assignments[, avg_distance]).
 
     sample_weight: one non-negative weight per sample (include/kmcuda_b200.h, kmcuda_b200_kmeans_weighted), a 1-D
-    array-like of length N, or an int device pointer when `samples` is the device-pointer tuple; None = unweighted."""
+    array-like of length N, or an int device pointer when `samples` is the device-pointer tuple; None = unweighted.
+
+    batch_size: an int >= 1 runs mini-batch k-means (kmcuda_b200_kmeans_minibatch, scikit-learn's MiniBatchKMeans)
+    with batches of min(batch_size, N) rows for at most max_steps steps (0 = 100 * N // batch size) on one GPU, L2
+    only; yinyang_t is ignored.  None = the Lloyd / Yinyang run."""
     clusters = int(clusters)
+    if batch_size is not None:
+        batch_size = _count(batch_size, "batch_size", 1)
+    max_steps = _count(max_steps, "max_steps", 0)
+    if max_steps and batch_size is None:
+        raise ValueError("\"max_steps\" applies to mini-batch runs only: pass \"batch_size\" too")
     if seed is None:
         seed = int(time.time()) & 0xFFFFFFFF
     afkmc2_m = ctypes.c_uint32(0)
@@ -230,7 +253,12 @@ def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1
     common = (init_method, ctypes.byref(afkmc2_m), tolerance, yinyang_t, metric_id, n, d, clusters,
               int(seed) & 0xFFFFFFFF, int(device), device_ptrs, int(fp16x2), int(verbosity), samples_ptr)
     outputs = (centroids_ptr, assignments_ptr, ctypes.byref(avg) if average_distance else None)
-    if weights_ptr is None:
+    if batch_size is not None:
+        if yinyang_t and verbosity > 0:
+            print("mini-batch k-means: yinyang_t is ignored", flush=True)
+        result = _lib.kmcuda_b200_kmeans_minibatch(*common[:3], *common[4:], weights_ptr, batch_size, max_steps,
+                                                   *outputs)
+    elif weights_ptr is None:
         result = _lib.kmeans_cuda(*common, *outputs)
     else:
         result = _lib.kmcuda_b200_kmeans_weighted(*common, weights_ptr, *outputs)

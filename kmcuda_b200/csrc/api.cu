@@ -334,6 +334,7 @@ class Job {
   KMCUDAResult lloyd(float tolerance, int* iter_out, uint32_t* changed_out);
   KMCUDAResult lloyd_continue(float tolerance, int iter);
   KMCUDAResult yinyang(float tolerance, uint32_t G);
+  KMCUDAResult minibatch(uint32_t batch_size, uint64_t max_steps, float tolerance, uint32_t seed);
   double lloyd_iter_ms = 0;   // wall time of the fastest complete Lloyd iteration of this run (assign pass + update), 0 = none yet
   KMCUDAResult group_centroids(uint32_t G, std::vector<uint32_t>* groups);
   KMCUDAResult average_distance(float* out);
@@ -1378,6 +1379,157 @@ KMCUDAResult Job::yinyang(float tolerance, uint32_t G) {
   }
 }
 
+// Mini-batch k-means (DESIGN.md §4h): scikit-learn's MiniBatchKMeans steps with this library's draws, on one GPU.  Each
+// step draws b rows with replacement, assigns them exactly, blends the batch's weighted member sums into the centroids
+// with the running weight totals W, and on the steps scikit-learn's rule picks turns the centroids of low W into batch
+// rows.  The only host round trip of a step is the stop decision (batch inertia, sum of squared centroid moves, count of
+// W == 0).  After the last step one ordinary assignment pass gives the assignments.
+KMCUDAResult Job::minibatch(uint32_t batch_size, uint64_t max_steps, float tolerance, uint32_t seed) {
+  static const double kReassignmentRatio = 0.01;
+  static const int kMaxNoImprovement = 10;
+  Dev& d = devs[0];
+  KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+  const uint32_t b = std::min(batch_size, N);
+  const uint64_t steps = max_steps ? max_steps : 100ull * N / b;
+  Shard bs(metric, d.dev, b, D, K, verbosity);
+  KMB_RET(bs.create(true));
+  const size_t kd = static_cast<size_t>(K) * D;
+  DevBuf<float> Cn, S, Wb;
+  DevBuf<uint32_t> rows, result, row_result, keys, counts, cidx_in, cidx, pos_in, picked, small;
+  DevBuf<double> W, Wn, bsum, stats, dsq, wsorted, ekey_in, ekey, minkept;
+  DevBuf<char> tmp;
+  const uint32_t nb = mb_blocks(b);
+  const size_t tmp_bytes = mb_reassign_bytes(b, K);
+  KMB_CU(Cn.alloc(kd), kmcudaMemoryAllocationFailure);
+  KMB_CU(S.alloc(kd), kmcudaMemoryAllocationFailure);
+  KMB_CU(Wb.alloc(K), kmcudaMemoryAllocationFailure);
+  KMB_CU(rows.alloc(b), kmcudaMemoryAllocationFailure);
+  KMB_CU(result.alloc(b), kmcudaMemoryAllocationFailure);
+  KMB_CU(row_result.alloc(N), kmcudaMemoryAllocationFailure);
+  KMB_CU(keys.alloc(b), kmcudaMemoryAllocationFailure);
+  KMB_CU(counts.alloc(K), kmcudaMemoryAllocationFailure);
+  KMB_CU(cidx_in.alloc(K), kmcudaMemoryAllocationFailure);
+  KMB_CU(cidx.alloc(K), kmcudaMemoryAllocationFailure);
+  KMB_CU(pos_in.alloc(b), kmcudaMemoryAllocationFailure);
+  KMB_CU(picked.alloc(b), kmcudaMemoryAllocationFailure);
+  KMB_CU(small.alloc(2), kmcudaMemoryAllocationFailure);
+  KMB_CU(W.alloc(K), kmcudaMemoryAllocationFailure);
+  KMB_CU(Wn.alloc(K), kmcudaMemoryAllocationFailure);
+  KMB_CU(bsum.alloc(nb), kmcudaMemoryAllocationFailure);
+  KMB_CU(stats.alloc(3), kmcudaMemoryAllocationFailure);
+  KMB_CU(dsq.alloc(K), kmcudaMemoryAllocationFailure);
+  KMB_CU(wsorted.alloc(K), kmcudaMemoryAllocationFailure);
+  KMB_CU(ekey_in.alloc(b), kmcudaMemoryAllocationFailure);
+  KMB_CU(ekey.alloc(b), kmcudaMemoryAllocationFailure);
+  KMB_CU(minkept.alloc(1), kmcudaMemoryAllocationFailure);
+  KMB_CU(tmp.alloc(tmp_bytes), kmcudaMemoryAllocationFailure);
+  KMB_CU(cudaMemsetAsync(W.get(), 0, sizeof(double) * K, d.st), kmcudaRuntimeError);
+  // scikit-learn's _tolerance: tolerance times the mean of the unweighted per-feature variances
+  double tol_abs = 0;
+  if (tolerance > 0) {
+    DevBuf<double> work, var;
+    KMB_CU(work.alloc(mb_variance_doubles(D)), kmcudaMemoryAllocationFailure);
+    KMB_CU(var.alloc(D), kmcudaMemoryAllocationFailure);
+    KMB_CU(launch_mb_variance(d.X, N, D, work, var, d.st), kmcudaRuntimeError);
+    std::vector<double> hv(D);
+    KMB_CU(cudaMemcpyAsync(hv.data(), var.get(), sizeof(double) * D, cudaMemcpyDeviceToHost, d.st),
+           kmcudaMemoryCopyError);
+    KMB_CU(cudaStreamSynchronize(d.st), kmcudaRuntimeError);
+    double m = 0;
+    for (int f = 0; f < D; f++) m += hv[f];
+    tol_abs = m / D * static_cast<double>(tolerance);
+  }
+  g_prof.mark("mini-batch: setup");
+  MbReassign ra;
+  ra.K = K;
+  ra.b = b;
+  ra.D = D;
+  ra.ratio = kReassignmentRatio;
+  ra.w = d.w.get();
+  ra.X = d.X;
+  ra.rows = rows;
+  ra.cidx_in = cidx_in;
+  ra.cidx = cidx;
+  ra.pos_in = pos_in;
+  ra.picked = picked;
+  ra.npos = small.get();
+  ra.m = small.get() + 1;
+  ra.wsorted = wsorted;
+  ra.ekey_in = ekey_in;
+  ra.ekey = ekey;
+  ra.minkept = minkept;
+  ra.tmp = tmp.get();
+  ra.tmp_bytes = tmp_bytes;
+  float *cur = d.C.get(), *nxt = Cn.get();
+  double *wcur = W.get(), *wnxt = Wn.get();
+  const double alpha = std::min(1.0, 2.0 * b / (static_cast<double>(N) + 1));
+  double ewa = 0, ewa_min = 0, h[3] = {0, 0, static_cast<double>(K)};
+  bool have_ewa = false, have_min = false;
+  int no_improvement = 0;
+  uint64_t since_reassign = 0, s = 1;
+  for (; s <= steps; s++) {
+    // scikit-learn's _random_reassign, on the weight totals before this step
+    since_reassign += b;
+    const bool reassign = h[2] > 0 || since_reassign >= 10ull * K;
+    if (reassign) since_reassign = 0;
+    KMB_CU(launch_mb_draw(N, b, mb_step_key(seed, s, kMbTagBatch), rows, d.st), kmcudaRuntimeError);
+    KMB_RET(bs.assign_rows(b, d.X, N, rows, cur, row_result, result, d.st));
+    KMB_CU(launch_mb_inertia(d.X, rows, b, D, cur, K, result, d.w.get(), keys, bsum, d.st), kmcudaRuntimeError);
+    KMB_CU(launch_kmp_sum(bsum, nb, stats.get(), d.st), kmcudaRuntimeError);
+    // unweighted: the member counts are the weight totals (a weight of 1 per entry; all-ones weights give the same bits)
+    KMB_RET(bs.partial_sums_rows(b, d.X, rows, keys, S, counts, d.st, d.w.get(), weighted ? Wb.get() : nullptr));
+    KMB_CU(launch_mb_blend(cur, wcur, S, weighted ? Wb.get() : nullptr, counts, K, D, nxt, wnxt, d.st),
+           kmcudaRuntimeError);
+    if (reassign) {
+      ra.key = mb_step_key(seed, s, kMbTagReassign);
+      ra.C = nxt;
+      ra.W = wnxt;
+      KMB_CU(launch_mb_reassign(ra, d.st), kmcudaRuntimeError);
+    }
+    KMB_CU(launch_mb_stats(cur, nxt, wnxt, K, D, dsq, stats.get() + 1, d.st), kmcudaRuntimeError);
+    KMB_CU(cudaMemcpyAsync(h, stats.get(), sizeof(h), cudaMemcpyDeviceToHost, d.st), kmcudaMemoryCopyError);
+    KMB_CU(cudaStreamSynchronize(d.st), kmcudaRuntimeError);
+    KMB_RET(bs.check_pipeline());
+    std::swap(cur, nxt);
+    std::swap(wcur, wnxt);
+    // scikit-learn's _mini_batch_convergence
+    const double mean = h[0] / b;
+    if (s == 1) {
+      KMB_INFO("mini-batch step %" PRIu64 "/%" PRIu64 ": mean batch inertia %.17g\n", s, steps, mean);
+      continue;
+    }
+    ewa = have_ewa ? ewa * (1 - alpha) + mean * alpha : mean;
+    have_ewa = true;
+    KMB_INFO("mini-batch step %" PRIu64 "/%" PRIu64 ": mean batch inertia %.17g, ewa inertia %.17g\n", s, steps, mean,
+             ewa);
+    if (tol_abs > 0 && h[1] <= tol_abs) {
+      KMB_INFO("mini-batch: converged (small centers change) at step %" PRIu64 "/%" PRIu64 "\n", s, steps);
+      break;
+    }
+    if (!have_min || ewa < ewa_min) {
+      no_improvement = 0;
+      ewa_min = ewa;
+      have_min = true;
+    } else {
+      no_improvement++;
+    }
+    if (no_improvement >= kMaxNoImprovement) {
+      KMB_INFO("mini-batch: converged (lack of improvement in inertia) at step %" PRIu64 "/%" PRIu64 "\n", s, steps);
+      break;
+    }
+  }
+  if (s > steps) KMB_INFO("mini-batch: %" PRIu64 " steps\n", steps);
+  if (cur != d.C.get())
+    KMB_CU(cudaMemcpyAsync(d.C.get(), cur, sizeof(float) * kd, cudaMemcpyDeviceToDevice, d.st), kmcudaMemoryCopyError);
+  g_prof.mark("mini-batch: steps");
+  KMB_CU(cudaMemsetAsync(d.assign.get(), 0xff, sizeof(uint32_t) * d.len, d.st), kmcudaRuntimeError);
+  KMB_CU(cudaMemsetAsync(d.prev.get(), 0xff, sizeof(uint32_t) * d.len, d.st), kmcudaRuntimeError);
+  uint32_t changed = 0;
+  KMB_RET(assign_pass(&changed));
+  g_prof.mark("assign pass");
+  return kmcudaSuccess;
+}
+
 KMCUDAResult Job::average_distance(float* out) {
   KMB_INFO("calculating the average distance...\n");
   double sum = 0;
@@ -1418,7 +1570,8 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
                                 uint16_t features_size, uint32_t clusters_size, uint32_t seed,
                                 uint32_t device, int32_t device_ptrs, int32_t fp16x2, int32_t verbosity,
                                 const float* samples, const float* weights, float* centroids,
-                                uint32_t* assignments, float* average_distance) {
+                                uint32_t* assignments, float* average_distance, bool minibatch = false,
+                                uint32_t batch_size = 0, uint32_t max_steps = 0) {
   KMB_DEBUG("arguments: %d %p %.3f %.2f %d %" PRIu32 " %" PRIu16 " %" PRIu32 " %" PRIu32 " %" PRIu32
             " %d %" PRIi32 " %p %p %p %p\n", init, init_params, tolerance, yinyang_t, metric, samples_size,
             features_size, clusters_size, seed, device, fp16x2, verbosity, samples, centroids, assignments,
@@ -1439,6 +1592,16 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
   if (init == kmcudaInitMethodKMeansParallel && init_params &&
       *static_cast<const uint32_t*>(init_params) > kKMeansParallelMaxRounds)
     return kmcudaInvalidArguments;
+  if (minibatch) {
+    // one GPU, L2, a real batch; strict mode replays a Lloyd update that mini-batch steps do not have
+    const char* su = getenv("KMCUDA_B200_STRICT_UPDATE");
+    if (batch_size == 0 || metric == kmcudaDistanceMetricCosine || (device & (device - 1)) != 0 ||
+        (su && su[0] == '1')) {
+      KMB_INFO("mini-batch k-means takes batch_size >= 1, the L2 metric, one device and no strict update mode\n");
+      return kmcudaInvalidArguments;
+    }
+    if (device == 0) device = 1;
+  }
   if (weights) {
     // strict mode replays the reference's unweighted running sums; there is no weighted reference to replay
     const char* su = getenv("KMCUDA_B200_STRICT_UPDATE");
@@ -1469,7 +1632,8 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
   if (verbosity > 1) KMB_RET(print_memory_stats(dev_ids));
   KMB_RET(job.init_centroids(init, init_params, seed, device_ptrs, fp16x2 != 0, centroids));
   g_prof.mark("init centroids");
-  KMB_RET(job.yinyang(tolerance, yy_groups_size));
+  if (minibatch) KMB_RET(job.minibatch(batch_size, max_steps, tolerance, seed));
+  else KMB_RET(job.yinyang(tolerance, yy_groups_size));
   if (average_distance) KMB_RET(job.average_distance(average_distance));
   g_prof.mark("average distance");
   // copy-out: centroids from the first device (identical everywhere), assignment slices from each shard
@@ -1529,6 +1693,18 @@ KMCUDAResult kmcuda_b200_kmeans_weighted(KMCUDAInitMethod init, const void* init
   return kmeans_impl(init, init_params, tolerance, yinyang_t, metric, samples_size, features_size, clusters_size, seed,
                      device, device_ptrs, fp16x2, verbosity, samples, weights, centroids, assignments,
                      average_distance);
+}
+
+KMCUDAResult kmcuda_b200_kmeans_minibatch(KMCUDAInitMethod init, const void* init_params, float tolerance,
+                                          KMCUDADistanceMetric metric, uint32_t samples_size,
+                                          uint16_t features_size, uint32_t clusters_size, uint32_t seed,
+                                          uint32_t device, int32_t device_ptrs, int32_t fp16x2, int32_t verbosity,
+                                          const float* samples, const float* weights, uint32_t batch_size,
+                                          uint32_t max_steps, float* centroids, uint32_t* assignments,
+                                          float* average_distance) {
+  return kmeans_impl(init, init_params, tolerance, 0.f, metric, samples_size, features_size, clusters_size, seed,
+                     device, device_ptrs, fp16x2, verbosity, samples, weights, centroids, assignments,
+                     average_distance, true, batch_size, max_steps);
 }
 
 KMCUDAResult knn_cuda(uint16_t k, KMCUDADistanceMetric metric, uint32_t samples_size,

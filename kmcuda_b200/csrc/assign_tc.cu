@@ -820,10 +820,14 @@ __device__ __forceinline__ void regroup_quad(const float (&acc)[64], int lane, u
 }
 
 // NKB: K-blocks of 64 features (compile-time: the MMA issue loop must be branch- and address-arithmetic-free); MODE 0 =
-// Lloyd assignment, 1 = Yinyang local step, 2 = k-NN, 3 = Yinyang bounds refresh (see Params).
-template <int NKB, int MODE>
-__global__ void __launch_bounds__(N_THREADS, 1)
-tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
+// Lloyd assignment, 1 = Yinyang local step, 2 = k-NN, 3 = Yinyang bounds refresh (see Params); the kernels below wrap
+// it as tc_assign_kernel<NKB, MODE> and tc_assign_rows_kernel<NKB>.  ROWS (MODE 0 only): the
+// mini-batch pass over a row list -- position i of the pass is sample p.rows[i]: the converters load X[rows[i]], results
+// and the re-check queue are by position (pair_row keeps the sample row for the re-check's loads), and a row the filter
+// cannot bound goes to the overflow list as its sample row with result[i] = kOverflowRow (tc_assign_rows resolves it).
+template <int NKB, int MODE, bool ROWS>
+__device__ __forceinline__ void
+tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
   static_assert(NKB <= MAX_NKB, "the A operand of a tile must fit its shared-memory region");
   constexpr int BST = b_stages(NKB), AUGB = aug_bufs(NKB), NDEPTH = norm_depth(NKB), ASLOTS = a_slots(NKB);
   // 1024-byte alignment (128B-swizzle atoms) by an OFFSET into the shared array: the pointer keeps its shared address
@@ -1013,7 +1017,8 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
           rqbase = __shfl_sync(0xffffffffu, rqbase, 0) + __popc(mmask & ((1u << lane) - 1));
           if (live) {
             if (overflow) {
-              p.ovf_rows[atomicAdd(&p.counters[CNT_OVF], 1u)] = static_cast<uint32_t>(grow);
+              p.ovf_rows[atomicAdd(&p.counters[CNT_OVF], 1u)] = ROWS ? p.rows[grow] : static_cast<uint32_t>(grow);
+              if (ROWS) p.result[grow] = kOverflowRow;
             } else if (MODE == 0 && total == 1) {
               if (p.assign) nchanged += commit_assignment(p.assign, p.prev, grow, cand[0]);
               else p.result[grow] = cand[0];
@@ -1022,7 +1027,7 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
               if (!p.assign) p.result[grow] = kUntouched;
             } else if (base + total <= p.max_pairs) {
               for (uint32_t i = 0; i < total; i++) {
-                p.pair_row[base + i] = static_cast<uint32_t>(grow);
+                p.pair_row[base + i] = ROWS ? p.rows[grow] : static_cast<uint32_t>(grow);
                 p.pair_cand[base + i] = cand[i];
               }
               p.rowq[3 * rqbase] = static_cast<uint32_t>(grow);
@@ -1033,7 +1038,8 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
               p.rowq[3 * rqbase] = static_cast<uint32_t>(grow);
               p.rowq[3 * rqbase + 1] = 0;
               p.rowq[3 * rqbase + 2] = 0;
-              p.ovf_rows[atomicAdd(&p.counters[CNT_OVF], 1u)] = static_cast<uint32_t>(grow);
+              p.ovf_rows[atomicAdd(&p.counters[CNT_OVF], 1u)] = ROWS ? p.rows[grow] : static_cast<uint32_t>(grow);
+              if (ROWS) p.result[grow] = kOverflowRow;
             }
           }
         }
@@ -1057,7 +1063,7 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
       if (MODE == 0 || MODE == 3) {
         const uint64_t grow = static_cast<uint64_t>(tile) * TM + row;
         xlive = grow < p.n;
-        xrow = p.X + (xlive ? grow : 0ull) * p.D;
+        xrow = p.X + (xlive ? (ROWS ? static_cast<uint64_t>(p.rows[grow]) : grow) : 0ull) * p.D;
       }
       if (MODE == 1) {
         const uint32_t li = min(tile * TM + row, n_eff - 1);   // ragged tail: repeat the last listed row
@@ -1662,6 +1668,19 @@ tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
   __syncthreads();
 }
 
+template <int NKB, int MODE>
+__global__ void __launch_bounds__(N_THREADS, 1)
+tc_assign_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
+  tc_assign_body<NKB, MODE, false>(tmap_b, p);
+}
+
+// the mini-batch pass over a row list (ROWS above): MODE 0 with the samples read through p.rows
+template <int NKB>
+__global__ void __launch_bounds__(N_THREADS, 1)
+tc_assign_rows_kernel(const __grid_constant__ CUtensorMap tmap_b, const Params p) {
+  tc_assign_body<NKB, 0, true>(tmap_b, p);
+}
+
 }  // namespace tc
 
 // ---------------------------------------------------------------------------------------------------
@@ -1858,6 +1877,20 @@ static void tc_launch_mode(int nkb, unsigned grid, size_t smem, cudaStream_t st,
     default: tc_assign_kernel<8, MODE><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
   }
 }
+static void tc_launch_rows(int nkb, unsigned grid, size_t smem, cudaStream_t st, const CUtensorMap& tb,
+                           const tc::Params& prm) {
+  using namespace tc;
+  switch (nkb) {
+    case 1: tc_assign_rows_kernel<1><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
+    case 2: tc_assign_rows_kernel<2><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
+    case 3: tc_assign_rows_kernel<3><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
+    case 4: tc_assign_rows_kernel<4><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
+    case 5: tc_assign_rows_kernel<5><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
+    case 6: tc_assign_rows_kernel<6><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
+    case 7: tc_assign_rows_kernel<7><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
+    default: tc_assign_rows_kernel<8><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
+  }
+}
 static void tc_launch_main(int mode, int nkb, unsigned grid, size_t smem, cudaStream_t st, const CUtensorMap& tb,
                            const tc::Params& prm) {
   if (mode == 3) tc_launch_mode<3>(nkb, grid, smem, st, tb, prm);
@@ -1898,6 +1931,8 @@ static cudaError_t tc_set_smem_attr_one(int bytes) {
   e = cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
   if (e != cudaSuccess) return e;
   e = cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) return e;
+  e = cudaFuncSetAttribute(tc::tc_assign_rows_kernel<NKB>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
   if (e != cudaSuccess) return e;
   return cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
 }
@@ -2171,6 +2206,50 @@ cudaError_t tc_assign(TcPlan* p, const float* X, const float* C, const float* cs
     return e;
   if (assign)
     finalize_rows_kernel<<<p->num_sms, 256, 0, st>>>(p->ovf_rows, p->counters + CNT_OVF, result, assign, prev, d_changed);
+  if ((e = cudaGetLastError()) != cudaSuccess) return e;
+  if (p->inject_error) cudaMemsetAsync(p->counters + CNT_ERR, 0x11, sizeof(uint32_t), st);
+  return cudaMemcpyAsync(p->h_counters, p->counters, sizeof(uint32_t) * CNT_N, cudaMemcpyDeviceToHost, st);
+}
+
+// resolves the positions of a row-list pass that took the exact list pass: result[i] = row_result[rows[i]]
+__global__ void resolve_overflow_rows_kernel(const uint32_t* __restrict__ rows, uint32_t n,
+                                             const uint32_t* __restrict__ row_result, uint32_t* __restrict__ result) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    if (result[i] == kOverflowRow) result[i] = row_result[rows[i]];
+}
+
+cudaError_t tc_assign_rows(TcPlan* p, const float* X, uint32_t nX, const uint32_t* rows, uint32_t n, const float* C,
+                           const float* csq, uint32_t* result, uint32_t* row_result, cudaStream_t st) {
+  using namespace tc;
+  if (n > p->max_n) return cudaErrorInvalidValue;
+  if ((reinterpret_cast<uintptr_t>(X) & 15) || (reinterpret_cast<uintptr_t>(C) & 15)) return cudaErrorMisalignedAddress;
+  cudaError_t e;
+  Params prm;
+  if ((e = tc_prepare(p, C, csq, n, &prm, st, false, true)) != cudaSuccess) return e;
+  prm.X = X;
+  prm.rows = rows;
+  prm.result = result;
+  const unsigned grid = min(static_cast<uint32_t>(p->num_sms), prm.ntiles);
+  const int slot = static_cast<int>(p->passes % TcPlan::kEvRing);
+  p->graph_slot = -1;
+  cudaEventRecord(p->ev0[slot], st);
+  tc_launch_rows(p->nkb, grid, p->smem_bytes, st, p->tmap, prm);
+  cudaEventRecord(p->ev1[slot], st);
+  p->passes++;
+  if ((e = cudaGetLastError()) != cudaSuccess) return e;
+  const unsigned rgrid = p->num_sms * 4;
+  if (p->metric == 1)
+    recheck_pairs_kernel<1, 0><<<rgrid, 128, 0, st>>>(X, C, csq, p->D, p->pair_row, p->pair_cand,
+                                                      p->counters + CNT_PAIRS, p->max_pairs, nX, p->K, p->pair_score);
+  else
+    recheck_pairs_kernel<0, 0><<<rgrid, 128, 0, st>>>(X, C, csq, p->D, p->pair_row, p->pair_cand,
+                                                      p->counters + CNT_PAIRS, p->max_pairs, nX, p->K, p->pair_score);
+  recheck_reduce_kernel<<<p->num_sms * 2, 256, 0, st>>>(p->rowq, p->counters + CNT_ROWQ, p->pair_cand,
+                                                        p->pair_score, result, nullptr, nullptr, nullptr);
+  if ((e = launch_assign_exact(p->metric, X, C, csq, n, p->D, p->K, p->ovf_rows, p->counters + CNT_OVF, row_result,
+                               st)) != cudaSuccess)
+    return e;
+  resolve_overflow_rows_kernel<<<p->num_sms * 2, 256, 0, st>>>(rows, n, row_result, result);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
   if (p->inject_error) cudaMemsetAsync(p->counters + CNT_ERR, 0x11, sizeof(uint32_t), st);
   return cudaMemcpyAsync(p->h_counters, p->counters, sizeof(uint32_t) * CNT_N, cudaMemcpyDeviceToHost, st);

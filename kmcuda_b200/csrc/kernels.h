@@ -22,6 +22,7 @@ void pool_free(void* p);
 void pool_trim();
 
 constexpr uint32_t kUntouched = 0xFFFFFFFEu;  // "no centroid won": leave the assignment alone
+constexpr uint32_t kOverflowRow = 0xFFFFFFFDu;  // row-list pass: this position waits for the exact list pass
 
 // ---- exact Lloyd assignment (all K centroids), optional row list -------------------------------
 // result[i] = argmin (strict <, ascending index), K for "insane" rows, kUntouched if nothing wins.
@@ -54,9 +55,11 @@ size_t update_partial_rows(uint32_t n, uint32_t K);
 size_t update_cub_bytes(uint32_t n);
 // sums[K][D] (fp32) and counts[K] (uint32) of this shard's samples.  With sample weights w[n]: sums = sum of w_i x_i
 // and wsums[K] = sum of w_i over the members (ws.partial_w must be set); counts stay member counts.
+// vals (optional, [n]): the sample row of each entry (mini-batch: entries are sampled rows, w is indexed by row);
+// nullptr = entry i is row i
 cudaError_t launch_partial_sums(const float* X, uint32_t n, int D, uint32_t K, const uint32_t* assign,
                                 UpdateWorkspace& ws, float* sums, uint32_t* counts, cudaStream_t st,
-                                const float* w = nullptr, float* wsums = nullptr);
+                                const float* w = nullptr, float* wsums = nullptr, const uint32_t* vals = nullptr);
 // strict parity mode: the reference's running-sum update replayed in sample order (simt_kernels.cu)
 size_t strict_update_cub_bytes(uint32_t n);
 cudaError_t launch_strict_update(int metric, const float* X, uint32_t n, int D, uint32_t K, const uint32_t* prev,
@@ -156,6 +159,51 @@ size_t kmp_weights_bytes(uint32_t n);
 cudaError_t launch_kmp_weights(const uint32_t* nearest, const float* w, uint32_t n, uint32_t C, uint32_t* keys_out,
                                float* w_out, uint32_t* start, void* tmp, size_t tmp_bytes, float* W, cudaStream_t st);
 
+// ---- mini-batch k-means (minibatch.cu) --------------------------------------------------------------------------------
+// the key of one step's draws: mix(mix(tag ^ seed) + step); the tags keep the batch draw and the reassignment draw apart
+// from each other and from the k-means|| draws (whose first-level inputs stay below 2^40)
+constexpr uint64_t kMbTagBatch = 0x6D696E6962617463ull;      // "minibatc"
+constexpr uint64_t kMbTagReassign = 0x7265617373696721ull;   // "reassig!"
+uint64_t mb_step_key(uint32_t seed, uint64_t step, uint64_t tag);
+// rows[j] = floor(u(key, j) * N), j < b
+cudaError_t launch_mb_draw(uint32_t N, uint32_t b, uint64_t key, uint32_t* rows, cudaStream_t st);
+// bsum[mb_blocks(n)] = block partials of sum w_j * (Kahan sum of (X[rows[j]] - C[a_j])^2), a_j = result[j],
+// w_j = w[rows[j]] (1 without weights); keys[j] = a_j, or K when result[j] is not a centroid (such an entry has no
+// inertia and no member sum)
+uint32_t mb_blocks(uint32_t n);
+cudaError_t launch_mb_inertia(const float* X, const uint32_t* rows, uint32_t n, int D, const float* C, uint32_t K,
+                              const uint32_t* result, const float* w, uint32_t* keys, double* bsum, cudaStream_t st);
+// Cnew = (C W + S) / (W + Wb) per centroid with Wb > 0 (else C), Wnew = W + Wb; Wb = wsums, or the member counts
+// when wsums is nullptr (unweighted: a weight of 1 per entry)
+cudaError_t launch_mb_blend(const float* C, const double* W, const float* S, const float* wsums,
+                            const uint32_t* counts, uint32_t K, int D, float* Cnew, double* Wnew, cudaStream_t st);
+// random reassignment of the centroids of low weight (minibatch.cu), entries drawn from X[rows[j]] with weight
+// w[rows[j]]; buffers: cidx_in / cidx [K], wsorted [K], ekey_in /
+// ekey [b] (double), pos_in / picked [b], npos / m [1], minkept [1], tmp of mb_reassign_bytes(b, K)
+struct MbReassign {
+  uint32_t K, b;
+  int D;
+  uint64_t key;
+  double ratio;
+  const float* w;          // [N] sample weights, nullptr = 1
+  const float* X;          // [N][D]
+  const uint32_t* rows;    // [b] the step's entries
+  float* C;     // [K][D], updated in place
+  double* W;    // [K], updated in place
+  uint32_t *cidx_in, *cidx, *pos_in, *picked, *npos, *m;
+  double *wsorted, *ekey_in, *ekey, *minkept;
+  void* tmp;
+  size_t tmp_bytes;
+};
+size_t mb_reassign_bytes(uint32_t b, uint32_t K);
+cudaError_t launch_mb_reassign(const MbReassign& r, cudaStream_t st);
+// out[0] = sum_c ||Cnew_c - Cold_c||^2 (double, fixed order), out[1] = #{W_c == 0}; dsq: [K] scratch
+cudaError_t launch_mb_stats(const float* Cold, const float* Cnew, const double* W, uint32_t K, int D, double* dsq,
+                            double* out, cudaStream_t st);
+// var[D] = per-feature variance of X[n][D] (population, two passes in double); work: mb_variance_doubles(D) doubles
+size_t mb_variance_doubles(int D);
+cudaError_t launch_mb_variance(const float* X, uint32_t n, int D, double* work, double* var, cudaStream_t st);
+
 cudaError_t launch_half_to_float(const void* src, float* dst, size_t n, cudaStream_t st);
 cudaError_t launch_float_to_half(const float* src, void* dst, size_t n, cudaStream_t st);
 cudaError_t launch_fill_u32(uint32_t* p, uint32_t v, size_t n, cudaStream_t st);
@@ -194,6 +242,10 @@ void tc_plan_destroy(TcPlan* plan);
 cudaError_t tc_assign(TcPlan* plan, const float* X, const float* C, const float* csq, uint32_t n,
                       uint32_t* result, uint32_t* assign, uint32_t* prev, uint32_t* d_changed, cudaStream_t st,
                       bool compute_csq = false);
+// mini-batch pass over a row list (tc_assign_kernel<NKB, 0, true>): result[i] = the winner of sample rows[i], i < n, as
+// launch_assign_exact defines it; X has nX rows; row_result [nX] is scratch of the exact list pass (indexed by row)
+cudaError_t tc_assign_rows(TcPlan* plan, const float* X, uint32_t nX, const uint32_t* rows, uint32_t n, const float* C,
+                           const float* csq, uint32_t* result, uint32_t* row_result, cudaStream_t st);
 // statistics of the last pass (for logging / bench): queue length and overflow rows
 void tc_last_stats(TcPlan* plan, uint32_t* n_recheck, uint32_t* n_overflow);
 // Yinyang local step (assign_tc.cu): candidate pairs with exact true distances for the listed rows

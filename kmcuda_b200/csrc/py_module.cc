@@ -10,6 +10,7 @@
 #include <numpy/arrayobject.h>
 
 #include <cinttypes>
+#include <cstdio>
 #include <cstring>
 #include <ctime>
 #include <string>
@@ -162,13 +163,38 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
   int32_t verbosity = 0;
   int adflag = 0;
   float tolerance = .01f, yinyang_t = .1f;
-  PyObject *samples_obj, *init_obj = Py_None, *metric_obj = Py_None, *weight_obj = Py_None;
+  PyObject *samples_obj, *init_obj = Py_None, *metric_obj = Py_None, *weight_obj = Py_None, *batch_obj = Py_None;
+  PyObject* steps_obj = nullptr;
   static const char* kwlist[] = {"samples", "clusters", "tolerance", "init", "yinyang_t", "metric",
-                                 "average_distance", "seed", "device", "verbosity", "sample_weight", nullptr};
-  if (!PyArg_ParseTupleAndKeywords(args, kwargs, "OI|fOfOpIIiO", const_cast<char**>(kwlist), &samples_obj,
+                                 "average_distance", "seed", "device", "verbosity", "sample_weight", "batch_size",
+                                 "max_steps", nullptr};
+  if (!PyArg_ParseTupleAndKeywords(args, kwargs, "OI|fOfOpIIiOOO", const_cast<char**>(kwlist), &samples_obj,
                                    &clusters, &tolerance, &init_obj, &yinyang_t, &metric_obj, &adflag, &seed,
-                                   &device, &verbosity, &weight_obj))
+                                   &device, &verbosity, &weight_obj, &batch_obj, &steps_obj))
     return nullptr;
+  // mini-batch k-means (kmcuda_b200.h): batch_size an integer >= 1, max_steps an integer >= 0
+  uint32_t batch_size = 0, max_steps = 0;
+  auto take_count = [](PyObject* o, const char* name, unsigned long lo, uint32_t* out) {
+    if (PyBool_Check(o) || !(PyLong_Check(o) || PyArray_IsScalar(o, Integer))) {
+      PyErr_Format(PyExc_TypeError, "\"%s\" must be an integer", name);
+      return false;
+    }
+    int overflow = 0;
+    const long long v = PyLong_AsLongLongAndOverflow(o, &overflow);
+    if (overflow || v < static_cast<long long>(lo) || v > 0xFFFFFFFFll) {
+      PyErr_Clear();
+      PyErr_Format(PyExc_ValueError, "\"%s\" must be an integer in [%lu, 2^32)", name, lo);
+      return false;
+    }
+    *out = static_cast<uint32_t>(v);
+    return true;
+  };
+  if (batch_obj != Py_None && !take_count(batch_obj, "batch_size", 1, &batch_size)) return nullptr;
+  if (steps_obj && !take_count(steps_obj, "max_steps", 0, &max_steps)) return nullptr;
+  if (max_steps && !batch_size) {
+    PyErr_SetString(PyExc_ValueError, "\"max_steps\" applies to mini-batch runs only: pass \"batch_size\" too");
+    return nullptr;
+  }
   KMCUDAInitMethod init = kmcudaInitMethodPlusPlus;
   auto named_init = [&init](PyObject* o) {
     const char* s = PyUnicode_Check(o) ? PyUnicode_AsUTF8(o) : nullptr;
@@ -313,8 +339,16 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
   }
   float average_distance = 0;
   int result;
+  if (batch_size && yinyang_t > 0 && verbosity > 0) {
+    printf("mini-batch k-means: yinyang_t is ignored\n");
+    fflush(stdout);
+  }
   Py_BEGIN_ALLOW_THREADS
-  if (weights)
+  if (batch_size)
+    result = kmcuda_b200_kmeans_minibatch(init, &afkmc2_m, tolerance, metric, n, static_cast<uint16_t>(d), clusters,
+                                          seed, device, device_ptrs, fp16x2, verbosity, samples, weights, batch_size,
+                                          max_steps, centroids, assignments, adflag ? &average_distance : nullptr);
+  else if (weights)
     result = kmcuda_b200_kmeans_weighted(init, &afkmc2_m, tolerance, yinyang_t, metric, n, static_cast<uint16_t>(d),
                                          clusters, seed, device, device_ptrs, fp16x2, verbosity, samples, weights,
                                          centroids, assignments, adflag ? &average_distance : nullptr);
@@ -446,7 +480,8 @@ PyObject* py_knn_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
 
 char module_doc[] = "K-means and K-nn on NVIDIA H100 (drop-in for src-d/kmcuda's libKMCUDA).";
 char kmeans_doc[] = "kmeans_cuda(samples, clusters, tolerance=.01, init=\"k-means++\", yinyang_t=.1, metric=\"L2\", "
-                    "average_distance=False, seed=time(), device=0, verbosity=0, sample_weight=None) -> "
+                    "average_distance=False, seed=time(), device=0, verbosity=0, sample_weight=None, batch_size=None, "
+                    "max_steps=0) -> "
                     "(centroids, assignments[, avg])";
 char knn_doc[] = "knn_cuda(k, samples, centroids, assignments, metric=\"L2\", device=0, verbosity=0) -> neighbors";
 

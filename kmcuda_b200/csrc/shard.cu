@@ -270,6 +270,46 @@ KMCUDAResult Shard::assign(uint32_t n, const float* X, const float* C, uint32_t*
   return kmcudaSuccess;
 }
 
+// Mini-batch assignment of a row list: result[j] = the winner of sample rows[j] as launch_assign_exact defines it, by
+// list position (duplicates get the same winner in every position).  Tensor-core route: the row-list variant of the
+// pass (tc_assign_rows); other shapes: the exact kernel's list mode into the row-indexed scratch, then by position.
+__global__ void rows_to_positions_kernel(const uint32_t* __restrict__ rows, uint32_t n,
+                                         const uint32_t* __restrict__ row_result, uint32_t* __restrict__ result) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) result[i] = row_result[rows[i]];
+}
+
+KMCUDAResult Shard::assign_rows(uint32_t n, const float* X, uint32_t nX, const uint32_t* rows, const float* C,
+                                uint32_t* row_result, uint32_t* result, cudaStream_t st) {
+  if (n > max_n) return kmcudaInvalidArguments;
+  last_tc = false;
+  if (n == 0) return kmcudaSuccess;
+  if (tc) {
+    KMB_CU(tc_assign_rows(tc, X, nX, rows, n, C, csq, result, row_result, st), kmcudaRuntimeError);
+    last_tc = true;
+    return kmcudaSuccess;
+  }
+  if (!d_count.get()) KMB_CU(d_count.alloc(1), kmcudaMemoryAllocationFailure);
+  KMB_CU(launch_fill_u32(d_count, n, 1, st), kmcudaRuntimeError);
+  KMB_CU(launch_csqr(metric, C, K, D, csq, st), kmcudaRuntimeError);
+  KMB_CU(launch_assign_exact(metric, X, C, csq, n, D, K, rows, d_count, row_result, st), kmcudaRuntimeError);
+  rows_to_positions_kernel<<<(n + 255) / 256, 256, 0, st>>>(rows, n, row_result, result);
+  KMB_CU(cudaGetLastError(), kmcudaRuntimeError);
+  return kmcudaSuccess;
+}
+
+KMCUDAResult Shard::partial_sums_rows(uint32_t n, const float* X, const uint32_t* rows, const uint32_t* keys,
+                                      float* sums, uint32_t* counts, cudaStream_t st, const float* weights,
+                                      float* wsums) {
+  if (n > max_n || ws.cub_tmp == nullptr) return kmcudaInvalidArguments;
+  if (weights && !ws_partial_w.get()) {
+    KMB_CU(ws_partial_w.alloc(update_partial_rows(max_n, K)), kmcudaMemoryAllocationFailure);
+    ws.partial_w = ws_partial_w;
+  }
+  KMB_CU(launch_partial_sums(X, n, D, K, keys, ws, sums, counts, st, weights, wsums, rows), kmcudaRuntimeError);
+  return kmcudaSuccess;
+}
+
 KMCUDAResult Shard::update_reference_order(uint32_t n, const float* X, const uint32_t* assignments,
                                            const uint32_t* prev, float* C, uint32_t* ccounts, cudaStream_t st) {
   if (n > max_n) return kmcudaInvalidArguments;
@@ -444,6 +484,15 @@ int32_t kmcuda_b200_debug_yy_bounds(kmcuda_b200_shard* shard, uint32_t n, const 
     return -9;
   if (cudaStreamSynchronize(st) != cudaSuccess) return -10;
   return (use_tc && kmb::tc_last_error(s->tc)) ? -11 : 0;
+}
+// the mini-batch assignment (Shard::assign_rows) of the n listed rows of samples [samples_size][D]: result [n] by list
+// position, row_scratch [samples_size]; device pointers, enqueued on `stream`.  0, or a negative code
+int32_t kmcuda_b200_debug_assign_rows(kmcuda_b200_shard* shard, uint32_t n, const float* samples,
+                                      uint32_t samples_size, const uint32_t* rows, const float* centroids,
+                                      uint32_t* row_scratch, uint32_t* result, void* stream) {
+  if (!shard || !samples || !rows || !centroids || !row_scratch || !result) return -1;
+  return shard->impl->assign_rows(n, samples, samples_size, rows, centroids, row_scratch, result,
+                                  static_cast<cudaStream_t>(stream)) == kmcudaSuccess ? 0 : -2;
 }
 int32_t kmcuda_b200_debug_stats(kmcuda_b200_shard* shard, float* out4) {
   if (!shard || !shard->impl->tc) return -1;

@@ -110,6 +110,12 @@ class Shard {
   // hot path
   KMCUDAResult assign(uint32_t n, const float* X, const float* C, uint32_t* assignments,
                       uint32_t* prev, uint32_t* d_changed, cudaStream_t st);
+  // mini-batch: result[j] = the winner of sample rows[j] (n <= max_n entries, X has nX rows); row_result [nX] scratch
+  KMCUDAResult assign_rows(uint32_t n, const float* X, uint32_t nX, const uint32_t* rows, const float* C,
+                           uint32_t* row_result, uint32_t* result, cudaStream_t st);
+  // weights (optional, [nX], indexed by row): member sums of the entries rows[0 .. n) with winners keys[0 .. n)
+  KMCUDAResult partial_sums_rows(uint32_t n, const float* X, const uint32_t* rows, const uint32_t* keys, float* sums,
+                                 uint32_t* counts, cudaStream_t st, const float* weights, float* wsums);
   // weights (optional, [n] on this device): weighted member sums, and wsums[K] = the members' weight totals
   KMCUDAResult partial_sums(uint32_t n, const float* X, const uint32_t* assignments, float* sums,
                             uint32_t* counts, cudaStream_t st, const float* weights = nullptr,
@@ -159,6 +165,7 @@ class Shard {
   DevBuf<uint32_t> result;
   UpdateWorkspace ws;
   DevBuf<uint32_t> ws_keys_out, ws_vals_in, ws_vals_out, ws_offsets;
+  DevBuf<uint32_t> d_count;   // assign_rows on the exact route: the list length
   DevBuf<float> ws_partial;
   DevBuf<float> ws_partial_w;   // weighted update only, allocated on first use
   DevBuf<float> prev_sums;   // cosine update: member sums of the previous iteration

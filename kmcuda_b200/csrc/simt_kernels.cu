@@ -536,7 +536,7 @@ size_t update_cub_bytes(uint32_t n) {
 
 cudaError_t launch_partial_sums(const float* X, uint32_t n, int D, uint32_t K, const uint32_t* assign,
                                 UpdateWorkspace& ws, float* sums, uint32_t* counts, cudaStream_t st,
-                                const float* w, float* wsums) {
+                                const float* w, float* wsums, const uint32_t* vals) {
   if (w && (!wsums || !ws.partial_w)) return cudaErrorInvalidValue;
   if (n == 0) {
     cudaMemsetAsync(sums, 0, sizeof(float) * static_cast<size_t>(K) * D, st);
@@ -544,14 +544,14 @@ cudaError_t launch_partial_sums(const float* X, uint32_t n, int D, uint32_t K, c
     if (w) cudaMemsetAsync(wsums, 0, sizeof(float) * K, st);
     return cudaGetLastError();
   }
-  if (ws.iota_n < n) {   // the identity permutation is an input the sort never modifies: written once per workspace
+  if (!vals && ws.iota_n < n) {   // the identity permutation is an input the sort never modifies: written once per workspace
     iota_kernel<<<cdiv(n, 256), 256, 0, st>>>(ws.vals_in, n);
     ws.iota_n = n;
   }
   int bits = 1;
   while ((1ull << bits) <= K) bits++;  // keys are in [0, K] (K = "insane")
   size_t bytes = ws.cub_tmp_bytes;
-  cudaError_t e = cub::DeviceRadixSort::SortPairs(ws.cub_tmp, bytes, assign, ws.keys_out, ws.vals_in,
+  cudaError_t e = cub::DeviceRadixSort::SortPairs(ws.cub_tmp, bytes, assign, ws.keys_out, vals ? vals : ws.vals_in,
                                                   ws.vals_out, (int)n, 0, bits, st);
   if (e != cudaSuccess) return e;
   launch_segment_offsets(ws.keys_out, n, K, ws.offsets, counts, st);

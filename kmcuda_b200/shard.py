@@ -38,6 +38,9 @@ _lib.kmcuda_b200_debug_yy_bounds.restype = ctypes.c_int32
 _lib.kmcuda_b200_debug_yy_bounds.argtypes = [ctypes.c_void_p, ctypes.c_uint32, ctypes.c_void_p, ctypes.c_void_p,
                                              ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32, ctypes.c_int32,
                                              ctypes.c_void_p]
+_lib.kmcuda_b200_debug_assign_rows.restype = ctypes.c_int32
+_lib.kmcuda_b200_debug_assign_rows.argtypes = [ctypes.c_void_p, ctypes.c_uint32, ctypes.c_void_p, ctypes.c_uint32] + \
+    [ctypes.c_void_p] * 5
 _lib.kmcuda_b200_debug_stats.restype = ctypes.c_int32
 _lib.kmcuda_b200_debug_stats.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
 
@@ -152,6 +155,27 @@ class Shard:
                                               1 if use_tc else 0, _ptr(out, torch.float32))
         if rc != 0:
             raise RuntimeError("kmcuda_b200_debug_yy_bounds failed (%d)" % rc)
+        return out
+
+    def debug_assign_rows(self, X, C, rows, out=None, scratch=None, sync=True):
+        """the mini-batch assignment of the samples X[rows] (Shard::assign_rows, the row-list tensor-core pass): winners
+        by list position, uint32 as int32 [n], enqueued on the current torch stream.  sync: wait, and raise
+        RuntimeError when the pass reports a pipeline error.  The handle's max_samples bounds len(rows)."""
+        rows = rows.to(device=X.device, dtype=torch.int32).contiguous()
+        n = rows.shape[0]
+        if out is None:
+            out = torch.empty(n, dtype=torch.int32, device=X.device)
+        if scratch is None:
+            scratch = torch.empty(X.shape[0], dtype=torch.int32, device=X.device)
+        rc = _lib.kmcuda_b200_debug_assign_rows(self._h, n, _ptr(X, torch.float32), X.shape[0], _ptr(rows, torch.int32),
+                                                _ptr(C, torch.float32), _ptr(scratch, torch.int32),
+                                                _ptr(out, torch.int32), _stream_ptr())
+        if rc != 0:
+            raise RuntimeError("kmcuda_b200_debug_assign_rows failed (%d)" % rc)
+        if sync:
+            torch.cuda.synchronize()
+            if self.last_error():
+                raise RuntimeError("tensor-core pipeline error 0x%x" % self.last_error())
         return out
 
     def debug_stats(self):
