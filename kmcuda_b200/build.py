@@ -21,7 +21,8 @@ LIB = os.path.join(HERE, "libKMCUDA.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
 CU_SOURCES = ["simt_kernels.cu", "knn_kernels.cu", "assign_tc.cu", "yinyang.cu", "shard.cu", "exchange.cu",
-              "kmeans_parallel.cu", "minibatch.cu", "api.cu"]
+              "kmeans_parallel.cu", "minibatch.cu", "transfer.cu", "job.cu", "seeding.cu",
+              "knn_driver.cu", "api.cu"]
 CC_SOURCES = ["py_module.cc"]
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -85,7 +86,7 @@ def build(force=False, verbose=False, variant=None, defines=()):
                 if verbose and out.strip():
                     print(out)
     if force or jobs or _newer(LIB, objs):
-        _run([NVCC, "-shared", "-o", LIB] + objs + ["-ldl"])  # NCCL is bound at run time (api.cu)
+        _run([NVCC, "-shared", "-o", LIB] + objs + ["-ldl"])  # NCCL is bound at run time (job.cu)
     return LIB
 
 

@@ -1,0 +1,672 @@
+// job.cu -- the k-means Job (job.h): device setup and the NCCL binding, ingest, the weights check, the centroid update
+// and its exchange, the Lloyd / Yinyang / mini-batch loops, the Yinyang grouping and the average distance.
+//
+// Role of the host halves of the reference's kmeans.cu (Lloyd loop :934-1026, Yinyang loop :1028-1263) and of
+// kmcuda.cc's allocation + ingest (:139-170).  Differences by design (DESIGN.md): samples are range-partitioned across
+// the GPUs in the mask instead of replicated; no transpose; the per-iteration exchange is ONE NCCL all-reduce of the
+// [K][D] partial sums + [K] counts instead of 5-6 rounds of peer copies; centroid update is a deterministic sort +
+// segmented compensated sum instead of one thread per centroid.
+#include <dlfcn.h>
+
+#include <map>
+
+#include "job.h"
+
+namespace kmb {
+
+// NCCL is resolved lazily with dlopen the first time a job spans more than one GPU.  Linking it
+// would either pin a second libnccl.so.2 into processes that also import torch (which ships its own,
+// newer NCCL under the same soname) or, linked statically, add ~400 MB to the library.
+struct NcclApi {
+  ncclResult_t (*CommInitAll)(ncclComm_t*, int, const int*) = nullptr;
+  ncclResult_t (*CommDestroy)(ncclComm_t) = nullptr;
+  ncclResult_t (*AllReduce)(const void*, void*, size_t, ncclDataType_t, ncclRedOp_t, ncclComm_t, cudaStream_t) = nullptr;
+  ncclResult_t (*GroupStart)() = nullptr;
+  ncclResult_t (*GroupEnd)() = nullptr;
+  const char* (*GetErrorString)(ncclResult_t) = nullptr;
+  bool ok = false;
+};
+
+static const NcclApi& nccl_api() {
+  static NcclApi api;
+  static bool tried = false;
+  if (!tried) {
+    tried = true;
+    void* h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_NOLOAD | RTLD_LOCAL);  // already in the process?
+    if (!h) h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_LOCAL);
+    if (!h) h = dlopen("libnccl.so", RTLD_NOW | RTLD_LOCAL);
+    if (h) {
+      api.CommInitAll = reinterpret_cast<decltype(api.CommInitAll)>(dlsym(h, "ncclCommInitAll"));
+      api.CommDestroy = reinterpret_cast<decltype(api.CommDestroy)>(dlsym(h, "ncclCommDestroy"));
+      api.AllReduce = reinterpret_cast<decltype(api.AllReduce)>(dlsym(h, "ncclAllReduce"));
+      api.GroupStart = reinterpret_cast<decltype(api.GroupStart)>(dlsym(h, "ncclGroupStart"));
+      api.GroupEnd = reinterpret_cast<decltype(api.GroupEnd)>(dlsym(h, "ncclGroupEnd"));
+      api.GetErrorString = reinterpret_cast<decltype(api.GetErrorString)>(dlsym(h, "ncclGetErrorString"));
+      api.ok = api.CommInitAll && api.CommDestroy && api.AllReduce && api.GroupStart && api.GroupEnd &&
+               api.GetErrorString;
+    }
+  }
+  return api;
+}
+
+// NCCL communicators (fallback exchange, see Job::update) are cached per device list for the life of the process:
+// ncclCommInitAll costs seconds to minutes and the library is not re-entrant anyway (kmcuda.h:25-26)
+static std::map<std::vector<int>, std::vector<ncclComm_t>>& comm_cache() {
+  static std::map<std::vector<int>, std::vector<ncclComm_t>> cache;
+  return cache;
+}
+static void drop_cached_comms() {
+  for (auto& kv : comm_cache())
+    for (ncclComm_t c : kv.second)
+      if (c) nccl_api().CommDestroy(c);
+  comm_cache().clear();
+}
+
+// equal split of `amount` rows over the devices, chunk starts aligned to 512 bytes without
+// breaking rows (same rule as the reference's distribute(), private.h:240-273)
+std::vector<std::pair<uint32_t, uint32_t>> split_rows(uint32_t amount, uint32_t row_bytes, size_t ndev) {
+  std::vector<std::pair<uint32_t, uint32_t>> res;
+  if (ndev == 0) return res;
+  if (ndev == 1) {
+    res.emplace_back(0, amount);
+    return res;
+  }
+  uint32_t a = row_bytes, b = 512, gcd = 0;
+  for (;;) {
+    if (a == 0) { gcd = b; break; }
+    b %= a;
+    if (b == 0) { gcd = a; break; }
+    a %= b;
+  }
+  uint32_t stride = 512 / gcd, offset = 0;
+  for (size_t i = 0; i + 1 < ndev; i++) {
+    float step = (amount - offset + .0f) / (ndev - i);
+    uint32_t len = static_cast<uint32_t>(roundf(step / stride)) * stride;
+    len = std::min(len, amount - offset);
+    res.emplace_back(offset, len);
+    offset += len;
+  }
+  res.emplace_back(offset, amount - offset);
+  return res;
+}
+
+PhaseProfile g_prof;
+
+KMCUDAResult Job::setup(const std::vector<int>& dev_ids) {
+  auto plan = split_rows(N, static_cast<uint32_t>(D) * sizeof(float), dev_ids.size());
+  devs = std::vector<Dev>(dev_ids.size());
+  for (size_t i = 0; i < dev_ids.size(); i++) {
+    Dev& d = devs[i];
+    d.dev = dev_ids[i];
+    d.off = plan[i].first;
+    d.len = plan[i].second;
+    KMB_CU(cudaSetDevice(d.dev), kmcudaNoSuchDevice);
+    KMB_CU(cudaStreamCreateWithFlags(&d.st, cudaStreamNonBlocking), kmcudaRuntimeError);
+    KMB_CU(d.C.alloc(static_cast<size_t>(K) * D), kmcudaMemoryAllocationFailure);
+    KMB_CU(d.sums.alloc(static_cast<size_t>(K) * D), kmcudaMemoryAllocationFailure);
+    KMB_CU(d.assign.alloc(d.len), kmcudaMemoryAllocationFailure);
+    KMB_CU(d.prev.alloc(d.len), kmcudaMemoryAllocationFailure);
+    KMB_CU(d.ccounts.alloc(K), kmcudaMemoryAllocationFailure);
+    KMB_CU(d.counts.alloc(K), kmcudaMemoryAllocationFailure);
+    KMB_CU(d.d_changed.alloc(1), kmcudaMemoryAllocationFailure);
+    KMB_CU(d.d_dsum.alloc(1), kmcudaMemoryAllocationFailure);
+    if (weighted) {
+      KMB_CU(d.wsums.alloc(K), kmcudaMemoryAllocationFailure);
+      KMB_CU(d.cweights.alloc(K), kmcudaMemoryAllocationFailure);
+    }
+    g_prof.mark("setup: stream + job buffers");
+    d.shard.reset(new Shard(metric, d.dev, d.len, D, K, verbosity));
+    KMB_RET(d.shard->create(true));
+    g_prof.mark("setup: shard workspace + tensor-core plan");
+  }
+  if (devs.size() > 1) {
+    // Exchange step of the centroid update.  Preferred: every GPU reads its peers' partial sums straight from
+    // peer memory (NVLink 5 / NVSwitch: K*D*4 bytes per peer, 1 MB at 1024 x 256) and adds them in device order,
+    // so all GPUs hold bit-identical centroids and no communicator has to be bootstrapped (ncclCommInitAll took
+    // ~100 s on the first multi-GPU call in round 1).  Fallback when some pair has no peer access, or
+    // KMCUDA_B200_EXCHANGE=nccl: one grouped ncclAllReduce of sums + counts per iteration.
+    const char* ex = getenv("KMCUDA_B200_EXCHANGE");
+    peer_exchange = !(ex && strcmp(ex, "nccl") == 0);
+    for (size_t i = 0; i < devs.size() && peer_exchange; i++)
+      for (size_t j = 0; j < devs.size() && peer_exchange; j++) {
+        if (i == j) continue;
+        int access = 0;
+        if (cudaDeviceCanAccessPeer(&access, devs[i].dev, devs[j].dev) != cudaSuccess || !access) peer_exchange = false;
+      }
+    if (peer_exchange) {
+      for (auto& d : devs) {
+        KMB_CU(cudaSetDevice(d.dev), kmcudaNoSuchDevice);
+        KMB_CU(d.rsums.alloc(static_cast<size_t>(K) * D), kmcudaMemoryAllocationFailure);
+        KMB_CU(d.rcounts.alloc(K), kmcudaMemoryAllocationFailure);
+        if (weighted) KMB_CU(d.rweights.alloc(K), kmcudaMemoryAllocationFailure);
+        KMB_CU(cudaEventCreateWithFlags(&d.ev_partial, cudaEventDisableTiming), kmcudaRuntimeError);
+        KMB_CU(cudaEventCreateWithFlags(&d.ev_reduced, cudaEventDisableTiming), kmcudaRuntimeError);
+      }
+      KMB_DEBUG("centroid update exchange: peer memory, %zu devices\n", devs.size());
+    } else {
+      if (!nccl_api().ok) {
+        KMB_INFO("multi-GPU jobs without full peer access need NCCL (libnccl.so.2), which could not be loaded\n");
+        return kmcudaRuntimeError;
+      }
+      auto it = comm_cache().find(dev_ids);
+      if (it == comm_cache().end()) {
+        std::vector<ncclComm_t> comms(devs.size());
+        ncclResult_t r = nccl_api().CommInitAll(comms.data(), static_cast<int>(devs.size()), dev_ids.data());
+        if (r != ncclSuccess) {
+          KMB_INFO("ncclCommInitAll failed: %s\n", nccl_api().GetErrorString(r));
+          return kmcudaRuntimeError;
+        }
+        it = comm_cache().emplace(dev_ids, comms).first;
+      }
+      for (size_t i = 0; i < devs.size(); i++) devs[i].comm = it->second[i];
+      KMB_DEBUG("centroid update exchange: NCCL all-reduce, %zu ranks\n", devs.size());
+    }
+  }
+  if (verbosity > 1) {
+    printf("plans: [");
+    for (size_t i = 0; i < devs.size(); i++) printf("%s(%" PRIu32 ", %" PRIu32 ")", i ? ", " : "", devs[i].off, devs[i].len);
+    printf("]\n");
+  }
+  return kmcudaSuccess;
+}
+
+KMCUDAResult Job::sync_all() {
+  for (auto& d : devs) {
+    KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+    KMB_CU(cudaStreamSynchronize(d.st), kmcudaRuntimeError);
+  }
+  return kmcudaSuccess;
+}
+
+// samples: [N][D] fp32, or [N][D/2] half2 when fp16x2 (D is already the real dimension here); weights: [N] fp32 or
+// nullptr, on the host or on device `device_ptrs` like the samples (always fp32)
+KMCUDAResult Job::ingest(const float* samples, const float* weights, int device_ptrs, bool fp16x2) {
+  for (auto& d : devs) {
+    KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+    if (weights) KMB_RET(copy_in(d.w, weights + d.off, d.len, d.dev, device_ptrs, false, d.st, verbosity));
+    const float* src = samples + static_cast<size_t>(d.off) * (fp16x2 ? D / 2 : D);
+    KMB_RET(copy_in(d.X, src, static_cast<size_t>(d.len) * D, d.dev, device_ptrs, fp16x2, d.st, verbosity));
+  }
+  return sync_all();
+}
+
+// every weight finite and >= 0, their sum > 0: one pass over each shard's slice on its device, then one flag and one
+// partial total per device come back (the same check for host and device weights)
+KMCUDAResult Job::check_weights() {
+  for (auto& d : devs) {
+    KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+    KMB_CU(cudaMemsetAsync(d.d_changed.get(), 0, sizeof(uint32_t), d.st), kmcudaRuntimeError);
+    KMB_CU(cudaMemsetAsync(d.d_dsum.get(), 0, sizeof(double), d.st), kmcudaRuntimeError);
+    KMB_CU(launch_check_weights(d.w, d.len, d.d_changed, d.d_dsum, d.st), kmcudaRuntimeError);
+  }
+  std::vector<uint32_t> flags;
+  std::vector<double> parts;
+  KMB_RET(gather([&](size_t i) { return devs[i].d_changed.get(); }, &flags,
+                 [&](size_t i) { return devs[i].d_dsum.get(); }, &parts));
+  uint32_t bad = 0;
+  double total = 0;
+  for (size_t i = 0; i < devs.size(); i++) {
+    bad |= flags[i];
+    total += parts[i];
+  }
+  if (bad) {
+    KMB_INFO("sample weights must be finite and >= 0\n");
+    return kmcudaInvalidArguments;
+  }
+  if (!(total > 0)) {
+    KMB_INFO("the sample weights sum to 0\n");
+    return kmcudaInvalidArguments;
+  }
+  wtotal = total;
+  return kmcudaSuccess;
+}
+
+// host copy of the weights, for the seeding steps that run on the host (first centroid, random init, AFK-MC2, the
+// multi-GPU k-means++ walk); fetched once from the shards, so host and device inputs are served alike
+KMCUDAResult Job::load_host_weights() {
+  if (!weighted || !host_w.empty()) return kmcudaSuccess;
+  host_w.resize(N);
+  for (auto& d : devs) {
+    KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+    KMB_CU(cudaMemcpyAsync(host_w.data() + d.off, d.w.get(), sizeof(float) * d.len, cudaMemcpyDeviceToHost, d.st),
+           kmcudaMemoryCopyError);
+  }
+  return sync_all();
+}
+
+// one assignment pass over every shard; *changed = total reassignments
+KMCUDAResult Job::assign_pass(uint32_t* changed) {
+  for (auto& d : devs) {
+    KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+    KMB_CU(cudaMemsetAsync(d.d_changed.get(), 0, sizeof(uint32_t), d.st), kmcudaRuntimeError);
+    KMB_RET(d.shard->assign(d.len, d.X, d.C, d.assign, d.prev, d.d_changed, d.st));
+  }
+  std::vector<uint32_t> mine;
+  KMB_RET(gather([&](size_t i) { return devs[i].d_changed.get(); }, &mine));
+  uint32_t total = 0;
+  for (size_t i = 0; i < devs.size(); i++) {
+    total += mine[i];
+    KMB_RET(devs[i].shard->check_pipeline());
+  }
+  *changed = total;
+  return kmcudaSuccess;
+}
+
+// centroid update: shard partial sums -> exchange (peer-memory reduce, or NCCL all-reduce) -> normalise on every GPU
+KMCUDAResult Job::update() {
+  if (devs.size() == 1 && devs[0].shard->strict_update) {
+    // strict parity mode: the reference's running sums in sample order (bit-identical centroids, one GPU)
+    Dev& d = devs[0];
+    KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+    return d.shard->update_reference_order(d.len, d.X, d.assign, d.prev, d.C, d.ccounts, d.st);
+  }
+  if (devs.size() > 1 && peer_exchange) {
+    // nobody may overwrite its partial sums while a peer of the previous iteration is still reading them
+    for (auto& d : devs) {
+      KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+      for (auto& e : devs)
+        if (&e != &d) KMB_CU(cudaStreamWaitEvent(d.st, e.ev_reduced, 0), kmcudaRuntimeError);
+    }
+  }
+  for (auto& d : devs) {
+    KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+    KMB_RET(d.shard->partial_sums(d.len, d.X, d.assign, d.sums, d.counts, d.st, d.w.get(), d.wsums.get()));
+    if (devs.size() > 1 && peer_exchange) KMB_CU(cudaEventRecord(d.ev_partial, d.st), kmcudaRuntimeError);
+  }
+  if (devs.size() > 1 && peer_exchange) {
+    PeerBuffers pb;
+    PeerF32 pw;   // weighted: the per-cluster weight totals travel with the sums
+    pb.n = pw.n = static_cast<int>(devs.size());
+    for (size_t i = 0; i < devs.size(); i++) {
+      pb.sums[i] = devs[i].sums.get();
+      pb.counts[i] = devs[i].counts.get();
+      pw.p[i] = devs[i].wsums.get();
+    }
+    for (auto& d : devs) {
+      KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+      for (auto& e : devs)
+        if (&e != &d) KMB_CU(cudaStreamWaitEvent(d.st, e.ev_partial, 0), kmcudaRuntimeError);
+      KMB_CU(launch_peer_reduce(pb, K, D, d.rsums, d.rcounts, d.st), kmcudaRuntimeError);
+      if (weighted) KMB_CU(launch_peer_sum_f32(pw, K, d.rweights, d.st), kmcudaRuntimeError);
+      KMB_CU(cudaEventRecord(d.ev_reduced, d.st), kmcudaRuntimeError);
+      KMB_RET(d.shard->finish_update(d.rsums, d.rcounts, d.C, d.ccounts, d.st, d.rweights.get(), d.cweights.get()));
+    }
+    return kmcudaSuccess;
+  }
+  if (devs.size() > 1) {
+    const NcclApi& nc = nccl_api();
+    ncclResult_t r = nc.GroupStart();
+    for (auto& d : devs) {
+      if (r != ncclSuccess) break;
+      r = nc.AllReduce(d.sums.get(), d.sums.get(), static_cast<size_t>(K) * D, ncclFloat32, ncclSum, d.comm, d.st);
+      if (r == ncclSuccess)
+        r = nc.AllReduce(d.counts.get(), d.counts.get(), K, ncclUint32, ncclSum, d.comm, d.st);
+      if (r == ncclSuccess && weighted)
+        r = nc.AllReduce(d.wsums.get(), d.wsums.get(), K, ncclFloat32, ncclSum, d.comm, d.st);
+    }
+    ncclResult_t rend = nc.GroupEnd();
+    if (r == ncclSuccess) r = rend;
+    if (r != ncclSuccess) {
+      KMB_INFO("ncclAllReduce failed: %s\n", nc.GetErrorString(r));
+      drop_cached_comms();   // a communicator that reported an error is not reused by later calls
+      return kmcudaRuntimeError;
+    }
+  }
+  for (auto& d : devs) {
+    KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+    KMB_RET(d.shard->finish_update(d.sums, d.counts, d.C, d.ccounts, d.st, d.wsums.get(), d.cweights.get()));
+  }
+  return kmcudaSuccess;
+}
+
+// reference kmeans_cuda_lloyd, kmeans.cu:934-1026 (resume == false)
+KMCUDAResult Job::lloyd(float tolerance, int* iter_out, uint32_t* changed_out) {
+  for (auto& d : devs) {
+    KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+    KMB_CU(cudaMemsetAsync(d.ccounts.get(), 0, sizeof(uint32_t) * K, d.st), kmcudaRuntimeError);
+    if (d.cweights.get()) KMB_CU(cudaMemsetAsync(d.cweights.get(), 0, sizeof(float) * K, d.st), kmcudaRuntimeError);
+    KMB_RET(d.shard->reset_update_state(d.st));
+    KMB_CU(cudaMemsetAsync(d.assign.get(), 0xff, sizeof(uint32_t) * d.len, d.st), kmcudaRuntimeError);
+    KMB_CU(cudaMemsetAsync(d.prev.get(), 0xff, sizeof(uint32_t) * d.len, d.st), kmcudaRuntimeError);
+  }
+  auto t_prev = std::chrono::steady_clock::now();
+  for (int iter = 1;; iter++) {
+    uint32_t changed = 0;
+    KMB_RET(assign_pass(&changed));
+    g_prof.mark("assign pass");
+    // iteration period (update of the previous iteration + this pass; assign_pass synchronises): what a Yinyang
+    // iteration has to beat (Job::yinyang)
+    const auto t_now = std::chrono::steady_clock::now();
+    if (iter >= 2) {
+      const double ms = std::chrono::duration<double, std::milli>(t_now - t_prev).count();
+      if (lloyd_iter_ms == 0 || ms < lloyd_iter_ms) lloyd_iter_ms = ms;
+    }
+    t_prev = t_now;
+    KMB_INFO("iteration %d: %" PRIu32 " reassignments\n", iter, changed);
+    if (iter_out) *iter_out = iter;
+    if (changed_out) *changed_out = changed;
+    if (changed <= tolerance * N) return kmcudaSuccess;  // float compare, kmeans.cu:707
+    KMB_RET(update());
+    g_prof.mark("centroid update");
+  }
+}
+
+// Lloyd iterations from the current state (assignments belong to the current centroids, the update is due): used when
+// the Yinyang iterations of a run turn out slower than its Lloyd passes (Job::yinyang)
+KMCUDAResult Job::lloyd_continue(float tolerance, int iter) {
+  for (;;) {
+    KMB_RET(update());
+    g_prof.mark("centroid update");
+    iter++;
+    uint32_t changed = 0;
+    KMB_RET(assign_pass(&changed));
+    g_prof.mark("assign pass");
+    KMB_INFO("iteration %d: %" PRIu32 " reassignments\n", iter, changed);
+    if (changed <= tolerance * N) return kmcudaSuccess;
+  }
+}
+
+// Yinyang groups = k-means (k-means++ with srand(0), Lloyd to 2 %) over the K centroids,
+// reference kmeans.cu:1061-1094.  Runs on the first device, result broadcast by the caller.
+KMCUDAResult Job::group_centroids(uint32_t G, std::vector<uint32_t>* groups) {
+  Job sub(metric, K, D, G, verbosity);
+  std::vector<int> one{devs[0].dev};
+  KMB_RET(sub.setup(one));
+  sub.devs[0].X.borrow(devs[0].C.get());
+  srand(0);
+  KMB_RET(sub.init_plusplus());
+  KMB_INFO("\rdone            \n");
+  KMB_RET(sub.lloyd(kYinyangGroupTolerance, nullptr, nullptr));
+  groups->resize(K);
+  KMB_CU(cudaSetDevice(devs[0].dev), kmcudaRuntimeError);
+  KMB_CU(cudaMemcpy(groups->data(), sub.devs[0].assign.get(), sizeof(uint32_t) * K, cudaMemcpyDeviceToHost),
+         kmcudaMemoryCopyError);
+  // The grouping only steers how tight the bounds are, never the result.  The exact part of a bounds refresh costs
+  // |group(a_i)| distances per sample, so a degenerate grouping (near-equidistant centroids: one group swallows most
+  // of them) is evened out: centroids in (group, index) order are cut into G runs of equal length.
+  {
+    std::vector<uint32_t> gsz(G, 0);
+    uint32_t live = 0;
+    for (uint32_t c = 0; c < K; c++)
+      if ((*groups)[c] < G) { gsz[(*groups)[c]]++; live++; }
+    const uint32_t avg = (live + G - 1) / G, biggest = *std::max_element(gsz.begin(), gsz.end());
+    if (avg && biggest > 4 * avg) {
+      KMB_INFO("Yinyang groups are unbalanced (largest %" PRIu32 ", average %" PRIu32 "): evened out\n", biggest, avg);
+      std::vector<uint32_t> order;
+      order.reserve(live);
+      for (uint32_t c = 0; c < K; c++)
+        if ((*groups)[c] < G) order.push_back(c);
+      std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) { return (*groups)[x] < (*groups)[y]; });
+      for (uint32_t i = 0; i < live; i++) (*groups)[order[i]] = static_cast<uint32_t>(static_cast<uint64_t>(i) * G / live);
+    }
+  }
+  return kmcudaSuccess;
+}
+
+// reference kmeans_cuda_yy, kmeans.cu:1028-1263
+KMCUDAResult Job::yinyang(float tolerance, uint32_t G) {
+  if (G == 0 || kYinyangDraftReassignments <= tolerance) {
+    if (verbosity > 0) {
+      if (G == 0) printf("too few clusters for this yinyang_t => Lloyd\n");
+      else printf("tolerance is too high (>= %.2f) => Lloyd\n", kYinyangDraftReassignments);
+    }
+    return lloyd(tolerance, nullptr, nullptr);
+  }
+  KMB_INFO("running Lloyd until reassignments drop below %" PRIu32 "\n",
+           static_cast<uint32_t>(kYinyangDraftReassignments * N));
+  int iter = 0;
+  uint32_t changed = 0;
+  KMB_RET(lloyd(kYinyangDraftReassignments, &iter, &changed));
+  if (changed <= tolerance * N) return kmcudaSuccess;
+  std::vector<uint32_t> groups;
+  KMB_RET(group_centroids(G, &groups));
+  g_prof.mark("yinyang: group centroids");
+  for (auto& d : devs) {
+    KMB_RET(d.shard->enable_yinyang(G));
+    KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+    KMB_CU(cudaMemcpyAsync(d.shard->groups.get(), groups.data(), sizeof(uint32_t) * K, cudaMemcpyHostToDevice, d.st),
+           kmcudaMemoryCopyError);
+    KMB_CU(cudaMemsetAsync(d.d_changed.get(), 0, sizeof(uint32_t), d.st), kmcudaRuntimeError);
+    KMB_RET(d.shard->yy_prepare(groups.data(), d.st));
+  }
+  KMB_RET(sync_all());
+  bool refresh = true;
+  // A Yinyang iteration only pays when it beats a Lloyd pass of the same run, and with the tensor-core pass that takes a
+  // large K (the bounds stream is 8 (G + 1) bytes per sample, the pass 2 K D flop).  Both are timed: once a clean Yinyang
+  // iteration (no refresh in it) was slower than the fastest Lloyd iteration, the run continues with Lloyd passes --
+  // the assignments are the same either way (KMCUDA_B200_YY_ADAPTIVE=0 keeps Yinyang).
+  const char* ad = getenv("KMCUDA_B200_YY_ADAPTIVE");
+  const bool adaptive = !(ad && ad[0] == '0') && lloyd_iter_ms > 0;
+  auto t_prev = std::chrono::steady_clock::now();
+  bool clean = false;          // the iteration that just ended contained no refresh
+  for (;; iter++) {
+    if (!refresh) {
+      std::vector<uint32_t> c, p;
+      KMB_RET(gather([&](size_t i) { return devs[i].d_changed.get(); }, &c,
+                     [&](size_t i) { return devs[i].shard->yy_counters.get() + 1; }, &p));
+      uint32_t total_changed = 0, total_passed = 0;
+      for (size_t i = 0; i < devs.size(); i++) {
+        KMB_RET(devs[i].shard->check_pipeline());
+        total_changed += c[i];
+        total_passed += p[i];
+      }
+      KMB_INFO("iteration %d: %" PRIu32 " reassignments\n", iter, total_changed);
+      if (total_changed <= tolerance * N) return kmcudaSuccess;
+      {
+        const auto t_now = std::chrono::steady_clock::now();
+        const double ms = std::chrono::duration<double, std::milli>(t_now - t_prev).count();
+        t_prev = t_now;
+        if (adaptive && clean && ms > lloyd_iter_ms) {
+          KMB_INFO("a Yinyang iteration takes %.2f ms, a Lloyd iteration %.2f ms => Lloyd\n", ms, lloyd_iter_ms);
+          return lloyd_continue(tolerance, iter);
+        }
+        clean = true;
+      }
+      for (auto& d : devs) {
+        KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+        KMB_CU(cudaMemsetAsync(d.d_changed.get(), 0, sizeof(uint32_t), d.st), kmcudaRuntimeError);
+      }
+      KMB_DEBUG("passed number: %" PRIu32 "\n", total_passed);
+      if (1.f - (total_passed + 0.f) / N < kYinyangRefreshEpsilon) refresh = true;
+    }
+    if (refresh) {
+      KMB_INFO("refreshing Yinyang bounds...\n");
+      for (auto& d : devs) {
+        KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+        KMB_RET(d.shard->yy_refresh(d.len, d.X, d.C, d.assign, d.st));
+      }
+      refresh = false;
+      clean = false;
+      g_prof.mark("yinyang: bounds refresh");
+    }
+    for (auto& d : devs) {
+      KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+      KMB_CU(cudaMemcpyAsync(d.shard->oldC.get(), d.C.get(), sizeof(float) * static_cast<size_t>(K) * D,
+                             cudaMemcpyDeviceToDevice, d.st), kmcudaMemoryCopyError);
+    }
+    KMB_RET(update());
+    g_prof.mark("centroid update");
+    for (auto& d : devs) {
+      KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+      KMB_RET(d.shard->yy_step(d.len, d.X, d.C, d.assign, d.prev, d.d_changed, d.st));
+    }
+    g_prof.mark("yinyang: filter + local step");
+    if (g_prof.on) {   // marks synchronise, so the pinned counters of the last pass are valid
+      Shard* s0 = devs[0].shard.get();
+      uint32_t yc[4] = {0, 0, 0, 0}, rq = 0, ov = 0;
+      cudaSetDevice(devs[0].dev);
+      cudaMemcpy(yc, s0->yy_counters.get(), sizeof(yc), cudaMemcpyDeviceToHost);
+      if (s0->tc) tc_last_stats(s0->tc, &rq, &ov);
+      fprintf(stderr, "[kmcuda_b200 timing]   yy step (dev 0): tightened %u, passed %u, candidate rows %u, pairs %u, "
+              "reference-order scan rows %u\n", yc[0], yc[1], rq, s0->tc ? tc_last_pairs(s0->tc) : 0u, ov);
+    }
+  }
+}
+
+// Mini-batch k-means (DESIGN.md §4h): scikit-learn's MiniBatchKMeans steps with this library's draws, on one GPU.  Each
+// step draws b rows with replacement, assigns them exactly, blends the batch's weighted member sums into the centroids
+// with the running weight totals W, and on the steps scikit-learn's rule picks turns the centroids of low W into batch
+// rows.  The only host round trip of a step is the stop decision (batch inertia, sum of squared centroid moves, count of
+// W == 0).  After the last step one ordinary assignment pass gives the assignments.
+KMCUDAResult Job::minibatch(uint32_t batch_size, uint64_t max_steps, float tolerance, uint32_t seed) {
+  static const double kReassignmentRatio = 0.01;
+  static const int kMaxNoImprovement = 10;
+  Dev& d = devs[0];
+  KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+  const uint32_t b = std::min(batch_size, N);
+  const uint64_t steps = max_steps ? max_steps : 100ull * N / b;
+  Shard bs(metric, d.dev, b, D, K, verbosity);
+  KMB_RET(bs.create(true));
+  const size_t kd = static_cast<size_t>(K) * D;
+  DevBuf<float> Cn, S, Wb;
+  DevBuf<uint32_t> rows, result, row_result, keys, counts, cidx_in, cidx, pos_in, picked, small;
+  DevBuf<double> W, Wn, bsum, stats, dsq, wsorted, ekey_in, ekey, minkept;
+  DevBuf<char> tmp;
+  Drain drain{*this};
+  const uint32_t nb = mb_blocks(b);
+  const size_t tmp_bytes = mb_reassign_bytes(b, K);
+  KMB_CU(Cn.alloc(kd), kmcudaMemoryAllocationFailure);
+  KMB_CU(S.alloc(kd), kmcudaMemoryAllocationFailure);
+  KMB_CU(Wb.alloc(K), kmcudaMemoryAllocationFailure);
+  KMB_CU(rows.alloc(b), kmcudaMemoryAllocationFailure);
+  KMB_CU(result.alloc(b), kmcudaMemoryAllocationFailure);
+  KMB_CU(row_result.alloc(N), kmcudaMemoryAllocationFailure);
+  KMB_CU(keys.alloc(b), kmcudaMemoryAllocationFailure);
+  KMB_CU(counts.alloc(K), kmcudaMemoryAllocationFailure);
+  KMB_CU(cidx_in.alloc(K), kmcudaMemoryAllocationFailure);
+  KMB_CU(cidx.alloc(K), kmcudaMemoryAllocationFailure);
+  KMB_CU(pos_in.alloc(b), kmcudaMemoryAllocationFailure);
+  KMB_CU(picked.alloc(b), kmcudaMemoryAllocationFailure);
+  KMB_CU(small.alloc(2), kmcudaMemoryAllocationFailure);
+  KMB_CU(W.alloc(K), kmcudaMemoryAllocationFailure);
+  KMB_CU(Wn.alloc(K), kmcudaMemoryAllocationFailure);
+  KMB_CU(bsum.alloc(nb), kmcudaMemoryAllocationFailure);
+  KMB_CU(stats.alloc(3), kmcudaMemoryAllocationFailure);
+  KMB_CU(dsq.alloc(K), kmcudaMemoryAllocationFailure);
+  KMB_CU(wsorted.alloc(K), kmcudaMemoryAllocationFailure);
+  KMB_CU(ekey_in.alloc(b), kmcudaMemoryAllocationFailure);
+  KMB_CU(ekey.alloc(b), kmcudaMemoryAllocationFailure);
+  KMB_CU(minkept.alloc(1), kmcudaMemoryAllocationFailure);
+  KMB_CU(tmp.alloc(tmp_bytes), kmcudaMemoryAllocationFailure);
+  KMB_CU(cudaMemsetAsync(W.get(), 0, sizeof(double) * K, d.st), kmcudaRuntimeError);
+  // scikit-learn's _tolerance: tolerance times the mean of the unweighted per-feature variances
+  double tol_abs = 0;
+  if (tolerance > 0) {
+    DevBuf<double> work, var;
+    KMB_CU(work.alloc(mb_variance_doubles(D)), kmcudaMemoryAllocationFailure);
+    KMB_CU(var.alloc(D), kmcudaMemoryAllocationFailure);
+    KMB_CU(launch_mb_variance(d.X, N, D, work, var, d.st), kmcudaRuntimeError);
+    std::vector<double> hv(D);
+    KMB_CU(cudaMemcpyAsync(hv.data(), var.get(), sizeof(double) * D, cudaMemcpyDeviceToHost, d.st),
+           kmcudaMemoryCopyError);
+    KMB_CU(cudaStreamSynchronize(d.st), kmcudaRuntimeError);
+    double m = 0;
+    for (int f = 0; f < D; f++) m += hv[f];
+    tol_abs = m / D * static_cast<double>(tolerance);
+  }
+  g_prof.mark("mini-batch: setup");
+  MbReassign ra;
+  ra.K = K;
+  ra.b = b;
+  ra.D = D;
+  ra.ratio = kReassignmentRatio;
+  ra.w = d.w.get();
+  ra.X = d.X;
+  ra.rows = rows;
+  ra.cidx_in = cidx_in;
+  ra.cidx = cidx;
+  ra.pos_in = pos_in;
+  ra.picked = picked;
+  ra.npos = small.get();
+  ra.m = small.get() + 1;
+  ra.wsorted = wsorted;
+  ra.ekey_in = ekey_in;
+  ra.ekey = ekey;
+  ra.minkept = minkept;
+  ra.tmp = tmp.get();
+  ra.tmp_bytes = tmp_bytes;
+  float *cur = d.C.get(), *nxt = Cn.get();
+  double *wcur = W.get(), *wnxt = Wn.get();
+  const double alpha = std::min(1.0, 2.0 * b / (static_cast<double>(N) + 1));
+  double ewa = 0, ewa_min = 0, h[3] = {0, 0, static_cast<double>(K)};
+  bool have_ewa = false, have_min = false;
+  int no_improvement = 0;
+  uint64_t since_reassign = 0, s = 1;
+  for (; s <= steps; s++) {
+    // scikit-learn's _random_reassign, on the weight totals before this step
+    since_reassign += b;
+    const bool reassign = h[2] > 0 || since_reassign >= 10ull * K;
+    if (reassign) since_reassign = 0;
+    KMB_CU(launch_mb_draw(N, b, mb_step_key(seed, s, kMbTagBatch), rows, d.st), kmcudaRuntimeError);
+    KMB_RET(bs.assign_rows(b, d.X, N, rows, cur, row_result, result, d.st));
+    KMB_CU(launch_mb_inertia(d.X, rows, b, D, cur, K, result, d.w.get(), keys, bsum, d.st), kmcudaRuntimeError);
+    KMB_CU(launch_kmp_sum(bsum, nb, stats.get(), d.st), kmcudaRuntimeError);
+    // unweighted: the member counts are the weight totals (a weight of 1 per entry; all-ones weights give the same bits)
+    KMB_RET(bs.partial_sums_rows(b, d.X, rows, keys, S, counts, d.st, d.w.get(), weighted ? Wb.get() : nullptr));
+    KMB_CU(launch_mb_blend(cur, wcur, S, weighted ? Wb.get() : nullptr, counts, K, D, nxt, wnxt, d.st),
+           kmcudaRuntimeError);
+    if (reassign) {
+      ra.key = mb_step_key(seed, s, kMbTagReassign);
+      ra.C = nxt;
+      ra.W = wnxt;
+      KMB_CU(launch_mb_reassign(ra, d.st), kmcudaRuntimeError);
+    }
+    KMB_CU(launch_mb_stats(cur, nxt, wnxt, K, D, dsq, stats.get() + 1, d.st), kmcudaRuntimeError);
+    KMB_CU(cudaMemcpyAsync(h, stats.get(), sizeof(h), cudaMemcpyDeviceToHost, d.st), kmcudaMemoryCopyError);
+    KMB_CU(cudaStreamSynchronize(d.st), kmcudaRuntimeError);
+    KMB_RET(bs.check_pipeline());
+    std::swap(cur, nxt);
+    std::swap(wcur, wnxt);
+    // scikit-learn's _mini_batch_convergence
+    const double mean = h[0] / b;
+    if (s == 1) {
+      KMB_INFO("mini-batch step %" PRIu64 "/%" PRIu64 ": mean batch inertia %.17g\n", s, steps, mean);
+      continue;
+    }
+    ewa = have_ewa ? ewa * (1 - alpha) + mean * alpha : mean;
+    have_ewa = true;
+    KMB_INFO("mini-batch step %" PRIu64 "/%" PRIu64 ": mean batch inertia %.17g, ewa inertia %.17g\n", s, steps, mean,
+             ewa);
+    if (tol_abs > 0 && h[1] <= tol_abs) {
+      KMB_INFO("mini-batch: converged (small centers change) at step %" PRIu64 "/%" PRIu64 "\n", s, steps);
+      break;
+    }
+    if (!have_min || ewa < ewa_min) {
+      no_improvement = 0;
+      ewa_min = ewa;
+      have_min = true;
+    } else {
+      no_improvement++;
+    }
+    if (no_improvement >= kMaxNoImprovement) {
+      KMB_INFO("mini-batch: converged (lack of improvement in inertia) at step %" PRIu64 "/%" PRIu64 "\n", s, steps);
+      break;
+    }
+  }
+  if (s > steps) KMB_INFO("mini-batch: %" PRIu64 " steps\n", steps);
+  if (cur != d.C.get())
+    KMB_CU(cudaMemcpyAsync(d.C.get(), cur, sizeof(float) * kd, cudaMemcpyDeviceToDevice, d.st), kmcudaMemoryCopyError);
+  g_prof.mark("mini-batch: steps");
+  KMB_CU(cudaMemsetAsync(d.assign.get(), 0xff, sizeof(uint32_t) * d.len, d.st), kmcudaRuntimeError);
+  KMB_CU(cudaMemsetAsync(d.prev.get(), 0xff, sizeof(uint32_t) * d.len, d.st), kmcudaRuntimeError);
+  uint32_t changed = 0;
+  KMB_RET(assign_pass(&changed));
+  g_prof.mark("assign pass");
+  return kmcudaSuccess;
+}
+
+KMCUDAResult Job::average_distance(float* out) {
+  KMB_INFO("calculating the average distance...\n");
+  for (auto& d : devs) {
+    KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+    KMB_CU(cudaMemsetAsync(d.d_dsum.get(), 0, sizeof(double), d.st), kmcudaRuntimeError);
+    KMB_CU(launch_average_distance(metric, d.X, d.C, d.len, D, d.assign, d.d_dsum, d.st, d.w.get()), kmcudaRuntimeError);
+  }
+  std::vector<double> parts;
+  KMB_RET(gather([&](size_t i) { return devs[i].d_dsum.get(); }, &parts));
+  double sum = 0;
+  for (double part : parts) sum += part;
+  *out = static_cast<float>(sum / (weighted ? wtotal : N));   // weighted: sum w d / sum w
+  return kmcudaSuccess;
+}
+}  // namespace kmb

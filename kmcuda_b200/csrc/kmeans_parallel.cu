@@ -1,6 +1,6 @@
 // kmeans_parallel.cu -- device side of the k-means|| seeding (Bahmani et al., "Scalable K-Means++", VLDB 2012).
 //
-// A round of the seeding (Job::init_kmeans_parallel, api.cu) is
+// A round of the seeding (Job::init_kmeans_parallel, seeding.cu) is
 //   draw      every row i is drawn iff u(seed, r, i) < l * w_i d_i^2 / phi, u a stateless counter hash of the global
 //             row index, so the draws do not depend on the device split or the launch shape; the drawn local row ids
 //             are compacted in ascending order (cub::DeviceSelect::Flagged) and their rows gathered

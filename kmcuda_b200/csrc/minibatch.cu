@@ -1,5 +1,5 @@
 // minibatch.cu -- device side of mini-batch k-means (Sculley, "Web-scale k-means clustering", WWW 2010; the update and
-// reassignment rules of scikit-learn's MiniBatchKMeans).  A step of Job::minibatch (api.cu) is
+// reassignment rules of scikit-learn's MiniBatchKMeans).  A step of Job::minibatch (job.cu) is
 //   draw       row_j = floor(u(seed, s, j) * N) for the b batch entries j (with replacement), w_j = w[row_j]; u is a
 //              SplitMix64 counter hash with its own domain tag, so the draws depend on (seed, s, j) only
 //   assign     Shard::assign_rows: the exact argmin of every entry, the tensor-core pass reading X[row_j] itself

@@ -88,7 +88,7 @@ class DevBuf {
   bool owned_ = false;
 };
 
-// equal split of `amount` rows over the devices, chunk starts aligned to 512 bytes (api.cu)
+// equal split of `amount` rows over the devices, chunk starts aligned to 512 bytes (job.cu)
 std::vector<std::pair<uint32_t, uint32_t>> split_rows(uint32_t amount, uint32_t row_bytes, size_t ndev);
 
 class Shard {

@@ -544,7 +544,7 @@ def test_adaptive_yinyang_switch_and_fast_refresh_keep_the_clustering(ours, monk
 
 def test_staged_pageable_ingest_delivers_the_same_bytes(ours, monkeypatch):
     """host buffers >= 256 MB that are not pinned are copied by several host threads through pinned staging buffers
-    (api.cu::host_to_device); the result must be the one of the plain cudaMemcpy (ragged last chunk included)"""
+    (transfer.cu::host_to_device); the result must be the one of the plain cudaMemcpy (ragged last chunk included)"""
     rng = np.random.default_rng(5)
     n, d, k = 280001, 260, 300           # 291 MB (staged from 256 MB upwards), not a multiple of the 16 MB chunk
     X = rng.random((n, d), dtype=np.float32)

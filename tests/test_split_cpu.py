@@ -1,4 +1,4 @@
-"""The static sample split over devices (SURVEY.md 8 row a9): api.cu::split_rows against a pure-Python restatement of
+"""The static sample split over devices (SURVEY.md 8 row a9): job.cu::split_rows against a pure-Python restatement of
 the reference's distribute() (src/private.h:240-273), through the library's C ABI (no GPU needed)."""
 import ctypes
 import math
