@@ -26,9 +26,10 @@
 //   bit-identical to the reference kernel's, ties included.
 //
 // Shared memory (227 KB per block on H100) holds the whole fp16 A operand of a tile (16 KB per 64 features), so
-// the tensor-core path serves D <= 512.  The A region is a ring of K-block slots with room for more than one tile
+// 128-row tiles serve D <= 512.  The A region is a ring of K-block slots with room for more than one tile
 // (D <= 256), so the next tile's first K-blocks are converted while the current one is multiplied.  For D > 256 the
-// pipeline is shallower (see smem_layout).
+// pipeline is shallower (see smem_layout).  512 < D <= 1024 (MODE 0 only) uses tiles of 64 rows (8 KB per 64 features);
+// both consumer warpgroups then hold the same rows, each one 64-column half of every n-tile (tile64 below).
 //
 // The same kernel template serves two more callers (MODE template parameter, see tc::Params):
 //   MODE 1  Yinyang local step (reference kmeans.cu:584-672): the samples are a compacted row list; candidates =
@@ -62,13 +63,15 @@ constexpr int TM = 128;                 // samples per tile (two wgmma M = 64 ha
 constexpr int TN = 128;                 // centroids per n-tile (wgmma N)
 constexpr int KB = 64;                  // fp16 elements per K-block = one 128-byte swizzle row
 constexpr int MAX_NKB = 8;              // D <= 512: the A operand of a tile lives in shared memory, 16 KiB per K-block
+// 512 < D <= 1024 (MODE 0 only): tiles of 64 rows, both consumer warpgroups on the same rows, each on one 64-column
+// half of every n-tile (wgmma m64n64k16); an A K-block is 8 KiB, so the whole tile still stays resident
+constexpr int MAX_TILE64_NKB = 16;
+constexpr int MAX_A_SLOTS = 16;
 constexpr int WIDE_NKB = 4;             // D > 256 ("wide"): a 128 KiB A tile leaves room for a 2-stage B ring only
 constexpr int B_STAGES = 4;             // fp16 centroid stages of ONE K-block (64 features x 128 rows = 16 KiB): a stage is
                                         // refilled as soon as both warpgroups' wgmmas on it have retired
-constexpr int A_KB_BYTES = TM * 128;    // one K-block of the A operand: 16 KiB
 constexpr int B_KB_BYTES = TN * 128;    // one K-block of the centroid tile: 16 KiB
 constexpr int B_STAGE_BYTES = B_KB_BYTES;
-constexpr int AUG_A_BYTES = TM * 32;    // 4 KiB  (K=16 fp16, no swizzle)
 constexpr int AUG_B_BYTES = TN * 32;    // 4 KiB
 constexpr int LIST_LEN = 5;             // entries per epilogue thread: one per n-tile in which one of its two rows held a
                                         // candidate (2 x row maximum, 2 x 32-bit mask, 16-bit n-tile)
@@ -136,7 +139,12 @@ struct SmemLayout {  // byte offsets from the 1024-aligned dynamic smem base
 __host__ __device__ constexpr bool wide_nkb(int nkb) { return nkb > WIDE_NKB; }
 __host__ __device__ constexpr int b_stages(int nkb) { return wide_nkb(nkb) ? 2 : B_STAGES; }
 __host__ __device__ constexpr int aug_bufs(int nkb) { return nkb <= 2 ? 2 : 1; }
-__host__ __device__ constexpr int a_slots(int nkb) { return nkb <= 2 ? 4 : nkb == 3 ? 5 : nkb == 4 ? 6 : MAX_NKB; }
+// NKB 9..16: 16 slots of 64 rows (128 KiB), so NKB < 16 still converts the next tile's first K-blocks during this one
+__host__ __device__ constexpr int a_slots(int nkb) { return nkb <= 2 ? 4 : nkb == 3 ? 5 : nkb == 4 ? 6 : nkb <= MAX_NKB ? MAX_NKB : 2 * MAX_NKB; }
+__host__ __device__ constexpr bool tile64(int nkb) { return nkb > MAX_NKB; }
+__host__ __device__ constexpr int tile_rows(int nkb) { return tile64(nkb) ? 64 : TM; }
+__host__ __device__ constexpr int a_kb_bytes(int nkb) { return tile_rows(nkb) * 128; }   // one A K-block: 16 / 8 KiB
+__host__ __device__ constexpr int mu_features(int nkb) { return (nkb > MAX_NKB ? nkb : MAX_NKB) * KB; }
 // The converters write the norms of segment f + depth after waiting for the slot of its last K-block, i.e. after every
 // consumer warp released K-block (f + depth + 1) * nkb - 1 - a_slots; that K-block belongs to segment f + 1 or later
 // (so each warp has read the norms of f) exactly when depth * nkb > a_slots.
@@ -145,9 +153,9 @@ __host__ __device__ constexpr int norm_depth(int nkb) { return a_slots(nkb) / nk
 __host__ __device__ constexpr SmemLayout smem_layout(int nkb) {
   SmemLayout L{};
   uint32_t o = 0;
-  L.a = o; o += a_slots(nkb) * A_KB_BYTES;
+  L.a = o; o += a_slots(nkb) * a_kb_bytes(nkb);
   L.b = o; o += b_stages(nkb) * B_STAGE_BYTES;
-  L.aug_a = o; o += AUG_A_BYTES;
+  L.aug_a = o; o += tile_rows(nkb) * 32;   // constant A-side bias operand: K = 16 fp16 per row, no swizzle (4 / 2 KiB)
   L.aug_b = o; o += aug_bufs(nkb) * AUG_B_BYTES;
   // candidate lists (MODE 0 / 1): 4 arrays (maximum of row R0 | of row R1 | mask of R0 | mask of R1) of
   // [tile parity][entry][epilogue thread] words, LIST_ARRAY bytes apart, then the n-tiles as 16-bit [parity][entry][thread].
@@ -155,19 +163,27 @@ __host__ __device__ constexpr SmemLayout smem_layout(int nkb) {
   L.list = o; o += LIST_ARRAYS * LIST_ARRAY + LIST_NT_BYTES;
   L.fin = o; o += 2 * FIN_WORDS * 4;  // [tile parity][FIN_*]
   L.norms = o; o += norm_depth(nkb) * 4 * TM * 4;   // [segment % depth][x|d][row]  x~^2 | residual^2 | (k-NN) exact s^2|x-c|^2 | (k-NN) s^2(|x|+|c|)^2
-  L.mu = o; o += MAX_NKB * KB * 4;    // -mu * s per feature (zero padded): the converters' centring term
+  L.mu = o; o += mu_features(nkb) * 4;   // -mu * s per feature (zero padded): the converters' centring term
   L.bars = o; o += 64 * 8;
   L.total = o;
   return L;
 }
 static_assert(LIST_ARRAYS * LIST_ARRAY + LIST_NT_BYTES + 2 * FIN_WORDS * 4 >= 48 * 256 * 4, "k-NN scratch overlaps the norms");
 __host__ __device__ constexpr bool layouts_fit() {
-  for (int k = 1; k <= MAX_NKB; k++)
-    if (smem_layout(k).total + 1024 > 232448 || a_slots(k) < k || a_slots(k) > MAX_NKB || norm_depth(k) * k <= a_slots(k))
+  for (int k = 1; k <= MAX_TILE64_NKB; k++)
+    if (smem_layout(k).total + 1024 > 232448 || a_slots(k) < k || a_slots(k) > MAX_A_SLOTS || norm_depth(k) * k <= a_slots(k))
       return false;
   return true;
 }
 static_assert(layouts_fit(), "227 KiB of shared memory per block on H100; a whole tile in the A ring; norms ring depth");
+// the 64-row layout (A 128 KiB, B 32 KiB, bias 2 + 4 KiB, lists and per-tile state 50 KiB, norms 4 KiB, -mu s NKB / 4
+// KiB, barriers, alignment): 226816 + 256 NKB bytes of the 232448 an H100 block may opt in to
+__host__ __device__ constexpr bool tile64_budget() {
+  for (int k = MAX_NKB + 1; k <= MAX_TILE64_NKB; k++)
+    if (smem_layout(k).total + 1024 != 226816u + 256u * k) return false;
+  return true;
+}
+static_assert(tile64_budget(), "64-row tile budget");
 
 // barrier indices inside the bars[] array
 enum {
@@ -176,8 +192,8 @@ enum {
   BAR_AUG_FULL = BAR_B_EMPTY + B_STAGES,      // [2]
   BAR_AUG_EMPTY = BAR_AUG_FULL + 2,           // [2]
   BAR_A_FULL = BAR_AUG_EMPTY + 2,             // [a_slots] converters -> consumers, per A slot
-  BAR_A_FREE = BAR_A_FULL + MAX_NKB,          // [a_slots] consumers -> converters, per A slot
-  BAR_EMIT_FULL = BAR_A_FREE + MAX_NKB,       // [2] epilogue -> emitter (per tile parity)
+  BAR_A_FREE = BAR_A_FULL + MAX_A_SLOTS,      // [a_slots] consumers -> converters, per A slot
+  BAR_EMIT_FULL = BAR_A_FREE + MAX_A_SLOTS,   // [2] epilogue -> emitter (per tile parity)
   BAR_EMIT_EMPTY = BAR_EMIT_FULL + 2,         // [2]
   BAR_COUNT = BAR_EMIT_EMPTY + 2
 };
@@ -462,7 +478,7 @@ __global__ void tc_prep_table_kernel(int metric, const float* __restrict__ C, co
 // table) of 3-12 us each on a 1 MB centroid matrix: ~0.05 ms of dependent launches per pass, 1 % of the step of an
 // 8M-row shard and 8 % of the step of a 1M-row shard (8 GPUs).  Here the same arithmetic (the device bodies are shared
 // with the chain, which stays as the KMB_PREP_FUSED=0 build) runs as four phases of one small grid separated by a
-// sense-reversing grid barrier; every CTA is resident (grid <= number of SMs, 256 threads, 34 KB static shared memory),
+// sense-reversing grid barrier; every CTA is resident (grid <= number of SMs, 256 threads, 38 KB static shared memory),
 // so the barrier cannot deadlock.  Values produced by other CTAs in an earlier phase are read with ld.global.cg.
 // ---------------------------------------------------------------------------------------------------
 struct PrepArgs {
@@ -504,7 +520,7 @@ __device__ __forceinline__ void prep_grid_barrier(unsigned* bar, unsigned nblock
 __global__ void __launch_bounds__(256)
 tc_prep_fused_kernel(const PrepArgs a) {
   __shared__ float s_tile[8][32 * 33];   // ||c||^2: one 32 x 32 staging tile per warp
-  __shared__ float s_mu[MAX_NKB * KB];
+  __shared__ float s_mu[MAX_TILE64_NKB * KB];
   __shared__ float s_scale;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t gw = blockIdx.x * 8u + warp, nw = gridDim.x * 8u;
@@ -828,8 +844,12 @@ __device__ __forceinline__ void regroup_quad(const float (&acc)[64], int lane, u
 template <int NKB, int MODE, bool ROWS>
 __device__ __forceinline__ void
 tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
-  static_assert(NKB <= MAX_NKB, "the A operand of a tile must fit its shared-memory region");
+  static_assert(NKB <= MAX_NKB || (MODE == 0 && NKB <= MAX_TILE64_NKB), "the A operand of a tile must fit its shared-memory region");
   constexpr int BST = b_stages(NKB), AUGB = aug_bufs(NKB), NDEPTH = norm_depth(NKB), ASLOTS = a_slots(NKB);
+  // NKB 9..16 (T64): 64-row tiles; consumer warpgroup g holds all 64 rows at columns 64g .. 64g + 63 of every n-tile
+  constexpr bool T64 = tile64(NKB);
+  constexpr int TR = tile_rows(NKB), AKB = a_kb_bytes(NKB);
+  constexpr int NACC = T64 ? 32 : 64;   // accumulators per consumer thread: 2 rows x NACC / 2 columns
   // 1024-byte alignment (128B-swizzle atoms) by an OFFSET into the shared array: the pointer keeps its shared address
   // space, so every access below is LDS / STS
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -881,13 +901,13 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
     ptx::fence_mbar_init();
   }
   // constant A-side bias block: ones in the first three K positions of every row
-  for (int i = threadIdx.x; i < TM * 16; i += N_THREADS) {
+  for (int i = threadIdx.x; i < TR * 16; i += N_THREADS) {
     int r = i >> 4, k = i & 15;
     int j = k >> 3, e = k & 7;
-    reinterpret_cast<__half*>(smem + L.aug_a)[(j * (TM * 16) + (r >> 3) * 128 + (r & 7) * 16) / 2 + e] =
+    reinterpret_cast<__half*>(smem + L.aug_a)[(j * (TR * 16) + (r >> 3) * 128 + (r & 7) * 16) / 2 + e] =
         __float2half_rn(k < 3 ? 1.f : 0.f);
   }
-  for (int i = threadIdx.x; i < MAX_NKB * KB; i += N_THREADS)
+  for (int i = threadIdx.x; i < mu_features(NKB); i += N_THREADS)
     reinterpret_cast<float*>(smem + L.mu)[i] = (MODE != 2 && p.neg_mu_s && i < nkb * KB) ? p.neg_mu_s[i] : 0.f;
   ptx::fence_proxy_async_smem();
   __syncthreads();
@@ -934,6 +954,8 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
     } else if (MODE < 2) {
       // ================================ emitters: merge column halves, write results / queues ================================
       // three warps walk the tile's 128 rows with a stride of 96: warp 0 takes two rows per thread
+      // (T64: rows 64 and up are not live, so only warps 0 and 1 emit rows; every warp still takes part in the queue
+      // reservation and the release)
       const int row0 = (warp - FIRST_EMIT_WARP) * 32 + lane;
       const int nrows = row0 + N_EMIT_WARPS * 32 < TM ? 2 : 1;   // warp-uniform
       const float cap = p.metric == 1 ? p.stats->scale * p.stats->scale : INFINITY;
@@ -948,17 +970,21 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
         TC_WAIT(BAR_EMIT_FULL + par, (ti >> 1) & 1, 12);
         for (int ri = 0; ri < nrows; ri++) {
           const int row = row0 + ri * N_EMIT_WARPS * 32;
-          uint64_t grow = static_cast<uint64_t>(tile) * TM + row;
+          uint64_t grow = static_cast<uint64_t>(tile) * TR + row;
           uint32_t cand[MAX_CAND];
           uint32_t total = 0, fl = 0;
-          const bool live = grow < n_eff;
+          const bool live = (!T64 || row < TR) && grow < n_eff;
           if (MODE == 1 && live) grow = p.rows[grow];
           if (live) {
             // the row's four epilogue threads: lanes 4 (row % 8) + t of consumer warp row / 16; the row is their R0 or R1
+            // (T64: eight threads, the same four lanes in both warpgroups, 128 list columns apart)
             const int hh = (row >> 3) & 1;
             const int lid0 = (row >> 4) * 32 + (row & 7) * 4;
-            // MODE 1: the second largest of the row's chunk maxima (a lower bound of its second best score)
-            const float Mf = MODE == 1 ? fin[FIN_M2 + row] : fin[FIN_M + row];
+            // MODE 1: the second largest of the row's chunk maxima (a lower bound of its second best score).  T64: each
+            // warpgroup's maximum covers its own columns only, so each is <= the row maximum and every warpgroup's
+            // candidate set contains the one of the row maximum; the final threshold uses the larger of the two.
+            float Mf = MODE == 1 ? fin[FIN_M2 + row] : fin[FIN_M + row];
+            if (T64) Mf = fmaxf(Mf, fin[FIN_M + TR + row]);
             const float mg = fin[FIN_MARGIN + row];
             const float thr = fminf(Mf, cap) - mg;
             fl = force;
@@ -970,20 +996,22 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
             // Candidates reach cand[] ordered by (lane, entry, bit), not by column.  Nothing downstream depends on that
             // order: the re-check reduction picks the smallest index among equal scores (sc == best && c < arg), and the
             // Yinyang finish takes a warp minimum of the index.
-            for (int t = 0; t < 4; t++) {
-              const int sl = lid0 + t;
+            for (int t = 0; t < (T64 ? 8 : 4); t++) {
+              const int tq = T64 ? t & 3 : t, wg = T64 ? t >> 2 : 0;
+              const int sl = lid0 + wg * 128 + tq;
               const uint32_t st = finu[FIN_STATE + sl];
               fl |= (st >> (8 + 8 * hh)) & 0xffu;
               const uint32_t c2 = st & 0xffu;
               for (uint32_t i = 0; i < c2; i++) {
                 constexpr uint32_t A = LIST_ARRAY / 4;
                 if (!(__uint_as_float(lst[hh * A + i * 256 + sl]) >= thr)) continue;   // the row's chunk maximum
-                const uint32_t base = static_cast<uint32_t>(lnt[i * 256 + sl]) * TN + 2 * t;
+                const uint32_t base = static_cast<uint32_t>(lnt[i * 256 + sl]) * TN + 64 * wg + 2 * tq;
                 uint32_t m = lst[(2 + hh) * A + i * 256 + sl];
                 while (m) {
                   const int b = __ffs(m) - 1;
                   m &= m - 1;
-                  const uint32_t col = base + 8 * (b >> 1) + (b & 1);   // bit b = 2j + e: column 8j + 2t + e
+                  // bit b = 2j + e: column 8j + 2t + e (T64: 16-bit masks, j < 8, of the warpgroup's 64-column half)
+                  const uint32_t col = base + 8 * (b >> 1) + (b & 1);
                   if (col < p.K) {
                     if (total < MAX_CAND) cand[total] = col;
                     total++;
@@ -1053,7 +1081,9 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
     ptx::setmaxnreg_dec<REGS_CONV>();
     // ================================ converters: fp32 rows -> fp16 A operand in shared memory ================================
     const int q = warp & 3;
-    const int row = q * 32 + lane;          // this thread's sample row within the tile
+    // this thread's sample row within the tile; T64: two threads per row, each converting one half of every K-block
+    const int row = T64 ? q * 16 + (lane >> 1) : q * 32 + lane;
+    const int hsel = T64 ? lane & 1 : 0;
     const float s = p.stats->scale;
     uint32_t si = 0, as = 0, aph = 0;       // segments converted; A ring slot and phase of the next K-block
     for (uint32_t tile = tile_begin; tile < tile_end; tile += gridDim.x) {
@@ -1061,7 +1091,7 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
       const float* xrow = nullptr;
       bool xlive = true;                      // rows past the end of the samples convert as zeros
       if (MODE == 0 || MODE == 3) {
-        const uint64_t grow = static_cast<uint64_t>(tile) * TM + row;
+        const uint64_t grow = static_cast<uint64_t>(tile) * TR + row;
         xlive = grow < p.n;
         xrow = p.X + (xlive ? (ROWS ? static_cast<uint64_t>(p.rows[grow]) : grow) : 0ull) * p.D;
       }
@@ -1083,7 +1113,8 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
         for (int kb = 0; kb < nkb; kb++) {
           uint32_t pk[32];
 #pragma unroll
-          for (int half = 0; half < 2; half++) {
+          for (int hi = 0; hi < (T64 ? 1 : 2); hi++) {
+            const int half = T64 ? hsel : hi;
             float4 gv[8];
             const int f0 = kb * KB + half * 32;
 #pragma unroll
@@ -1129,8 +1160,8 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
                 a2c = (t - a2) - y;
                 a2 = t;
               }
-              pk[half * 16 + c * 2] = *reinterpret_cast<uint32_t*>(&h0);
-              pk[half * 16 + c * 2 + 1] = *reinterpret_cast<uint32_t*>(&h1);
+              pk[hi * 16 + c * 2] = *reinterpret_cast<uint32_t*>(&h0);
+              pk[hi * 16 + c * 2 + 1] = *reinterpret_cast<uint32_t*>(&h1);
             }
           }
           // only the stores wait for the slot: the loads of this K-block, possibly of the next tile, are already in
@@ -1139,11 +1170,13 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
 #if KMB_KO != 3
           // the row's 128 bytes of this K-block: 16-byte chunk c (features 8c .. 8c+7) at chunk position c ^ (row % 8)
           // (the 128-byte swizzle of a K-major wgmma operand; also spreads the warp's stores over all banks)
-          uint8_t* a_row = smem + L.a + as * A_KB_BYTES + row * 128;
+          uint8_t* a_row = smem + L.a + as * AKB + row * 128;
 #pragma unroll
-          for (int c = 0; c < 8; c++)
-            *reinterpret_cast<uint4*>(a_row + ((c ^ (row & 7)) << 4)) =
+          for (int c = 0; c < (T64 ? 4 : 8); c++) {
+            const int cc = T64 ? hsel * 4 + c : c;
+            *reinterpret_cast<uint4*>(a_row + ((cc ^ (row & 7)) << 4)) =
                 make_uint4(pk[4 * c], pk[4 * c + 1], pk[4 * c + 2], pk[4 * c + 3]);
+          }
 #else
           (void)pk;
 #endif
@@ -1152,8 +1185,17 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
             float nxl, nxh, ndl, ndh;
             ptx::unpack2(nx2, nxl, nxh);
             ptx::unpack2(nd2, ndl, ndh);
-            norms[row] = nxl + nxh;
-            if (MEASURED_RESIDUAL) norms[TM + row] = ndl + ndh;
+            if (T64) {   // the row's two halves (lanes 2r, 2r + 1) are combined with one 64-bit shuffle
+              const uint64_t o = __shfl_xor_sync(0xffffffffu, ptx::pack2(nxl + nxh, ndl + ndh), 1);
+              float onx, ond;
+              ptx::unpack2(o, onx, ond);
+              nxl += onx;
+              ndl += ond;
+            }
+            if (!T64 || hsel == 0) {
+              norms[row] = nxl + nxh;
+              if (MEASURED_RESIDUAL) norms[TM + row] = ndl + ndh;
+            }
             if (MODE == 2) {
               norms[2 * TM + row] = a2;
               norms[3 * TM + row] = nraw * s * s;
@@ -1180,14 +1222,19 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
     const int h = (lane & 3) >> 1;             // MODE 2 / 3: column half of every 128-column n-tile
     const int row = g * 64 + wq * 16 + (lane >> 2) + 8 * (lane & 1);
     const int slot = h * TM + row;             // 0..255
-    const int qrow = g * 64 + wq * 16 + (lane >> 2);   // MODE 0 / 1: R0
+    // T64: both warpgroups hold the same rows R0 / R1 (at columns 64g + 8j + 2t + e, j < 8) and keep their own per-row
+    // maximum and margin in the per-tile state at frow = 64g + R0 (the emitters merge the two)
+    const int qrow = (T64 ? 0 : g * 64) + wq * 16 + (lane >> 2);   // MODE 0 / 1: R0
+    const int frow = T64 ? g * TR + qrow : qrow;
     const int lid = e * 32 + lane;                     // MODE 0 / 1: this thread's column of the lists, 0..255
-    // K-major 128-byte-swizzled operands: 8-row groups 1024 bytes apart; +32 bytes (2 in the address field) per K=16
-    const uint64_t adesc0 = ptx::make_smem_desc(ptx::smem_u32(smem + L.a + g * (64 * 128)), 16, 1024, 1);
-    const uint64_t bdesc0 = ptx::make_smem_desc(ptx::smem_u32(smem + L.b), 16, 1024, 1);
-    // bias blocks (no swizzle): core matrices of 8 rows x 16 bytes, 8-row groups 128 bytes apart, K halves 2 KiB apart
-    const uint64_t aug_ad = ptx::make_smem_desc(ptx::smem_u32(smem + L.aug_a + g * 1024), TM * 16, 128, 0);
-    const uint64_t aug_bd0 = ptx::make_smem_desc(ptx::smem_u32(smem + L.aug_b), TN * 16, 128, 0);
+    // K-major 128-byte-swizzled operands: 8-row groups 1024 bytes apart; +32 bytes (2 in the address field) per K=16.
+    // T64: the whole A slot, and the 64 centroid rows (8 KiB) of this warpgroup's column half of the B stage
+    const uint64_t adesc0 = ptx::make_smem_desc(ptx::smem_u32(smem + L.a + (T64 ? 0 : g * (64 * 128))), 16, 1024, 1);
+    const uint64_t bdesc0 = ptx::make_smem_desc(ptx::smem_u32(smem + L.b + (T64 ? g * (64 * 128) : 0)), 16, 1024, 1);
+    // bias blocks (no swizzle): core matrices of 8 rows x 16 bytes, 8-row groups 128 bytes apart, K halves TR * 16 /
+    // TN * 16 bytes apart
+    const uint64_t aug_ad = ptx::make_smem_desc(ptx::smem_u32(smem + L.aug_a + (T64 ? 0 : g * 1024)), TR * 16, 128, 0);
+    const uint64_t aug_bd0 = ptx::make_smem_desc(ptx::smem_u32(smem + L.aug_b + (T64 ? g * 1024 : 0)), TN * 16, 128, 0);
     uint32_t bs = 0, bph = 0;                  // B ring stage / phase
     uint32_t a_ready_si = 0xFFFFFFFFu;         // segment whose A operand this warp has already waited for
     uint32_t a0 = 0, aph0 = 0;                 // A ring slot and phase of the current segment's first K-block
@@ -1257,7 +1304,7 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
         const bool free_a = it.seg_last();         // last n-tile of this segment: release each A slot once read
         a_ready_si = si;
         __syncwarp();                              // wgmma is .aligned: the warp issues it converged
-        float acc[64];
+        float acc[NACC];
         uint32_t sa_prev = 0;                      // A slot of the previous K-block
 #pragma unroll
         for (int kb = 0; kb < NKB; kb++) {
@@ -1270,10 +1317,13 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
 #if KMB_KO != 2
           ptx::wgmma_fence_acc(acc);
           ptx::wgmma_fence();
-          const uint64_t ad = adesc0 + ((sa * A_KB_BYTES) >> 4);
+          const uint64_t ad = adesc0 + ((sa * AKB) >> 4);
           const uint64_t bd = bdesc0 + ((bs * B_STAGE_BYTES) >> 4);
 #pragma unroll
-          for (int k = 0; k < 4; k++) ptx::wgmma_m64n128k16(acc, ad + 2 * k, bd + 2 * k, (kb | k) ? 1u : 0u);
+          for (int k = 0; k < 4; k++) {
+            if constexpr (T64) ptx::wgmma_m64n64k16(acc, ad + 2 * k, bd + 2 * k, (kb | k) ? 1u : 0u);
+            else ptx::wgmma_m64n128k16(acc, ad + 2 * k, bd + 2 * k, (kb | k) ? 1u : 0u);
+          }
           ptx::wgmma_commit();
           ptx::wgmma_fence_acc(acc);
 #endif
@@ -1295,7 +1345,8 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
 #if KMB_KO != 2
         ptx::wgmma_fence_acc(acc);
         ptx::wgmma_fence();
-        ptx::wgmma_m64n128k16(acc, aug_ad, aug_bd0 + buf * (AUG_B_BYTES >> 4), 1u);
+        if constexpr (T64) ptx::wgmma_m64n64k16(acc, aug_ad, aug_bd0 + buf * (AUG_B_BYTES >> 4), 1u);
+        else ptx::wgmma_m64n128k16(acc, aug_ad, aug_bd0 + buf * (AUG_B_BYTES >> 4), 1u);
         ptx::wgmma_commit();
 #endif
         ptx::wgmma_wait<0>();
@@ -1314,10 +1365,10 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
 #if KMB_KO == 1
         if (MODE < 2)   // stand-in values: strictly decreasing along the row, 64 apart -> one candidate per row
 #pragma unroll
-          for (int j = 0; j < 16; j++)
+          for (int j = 0; j < NACC / 4; j++)
 #pragma unroll
             for (int q = 0; q < 4; q++)
-              acc[j * 4 + q] = -64.f * static_cast<float>(n * TN + 8 * j + 2 * (lane & 3) + (q & 1) + 1);
+              acc[j * 4 + q] = -64.f * static_cast<float>(n * TN + (T64 ? 64 * g : 0) + 8 * j + 2 * (lane & 3) + (q & 1) + 1);
 #endif
         if (it.seg_first()) {
           const float* norms = reinterpret_cast<const float*>(smem + L.norms) + (si % NDEPTH) * 4 * TM;
@@ -1378,7 +1429,7 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
             for (int hh = 0; hh < 2; hh++) {
               uint32_t fl = 0;
               const float mg = row_margin(qrow + 8 * hh, fl);
-              if ((lane & 3) == 0) fin[FIN_MARGIN + qrow + 8 * hh] = mg;
+              if ((lane & 3) == 0) fin[FIN_MARGIN + frow + 8 * hh] = mg;
               *fst |= fl << (8 + 8 * hh);
             }
             __syncwarp();
@@ -1405,7 +1456,7 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
           // acc[j*4 + hh*2 + e], column 8j + 2t + e of the n-tile.  Any fixed column order would do: the running row
           // maximum and the "within margin" bits do not depend on it, and the emitter decodes bits into columns.
 #ifdef KMB_DEBUG_SCORES   // bring-up builds only: 64 stores per n-tile bloat the hot loop's instruction footprint
-          if (MODE == 0 && p.dbg_scores)
+          if (MODE == 0 && !T64 && p.dbg_scores)
             for (int hh = 0; hh < 2; hh++) {
               const uint64_t grow = static_cast<uint64_t>(tile) * TM + qrow + 8 * hh;
               float* dst = p.dbg_scores + grow * (static_cast<uint64_t>(nt) * TN) + n * TN + 2 * (lane & 3);
@@ -1420,29 +1471,36 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
           if (MODE == 0) {   // timing build: the accumulators are loaded, the ALU work on them is skipped
             uint32_t x0 = 0, x1 = 0;
 #pragma unroll
-            for (int j = 0; j < 16; j += 4) { x0 ^= __float_as_uint(acc[j * 4]); x1 ^= __float_as_uint(acc[j * 4 + 2]); }
+            for (int j = 0; j < NACC / 4; j += 4) { x0 ^= __float_as_uint(acc[j * 4]); x1 ^= __float_as_uint(acc[j * 4 + 2]); }
             Mr[0] = fmaxf(Mr[0], __uint_as_float(x0 & 0x3fffffffu));
             Mr[1] = fmaxf(Mr[1], __uint_as_float(x1 & 0x3fffffffu));
             continue;
           }
 #endif
-          float cm[2], thr[2];    // this lane's chunk maximum (32 columns) and the row's threshold
+          float cm[2], thr[2];    // this lane's chunk maximum (32 columns; T64: 16) and the row's threshold
           uint32_t mask[2];
 #pragma unroll
           for (int hh = 0; hh < 2; hh++) {
             auto v = [&](int b) { return acc[(b >> 1) * 4 + hh * 2 + (b & 1)]; };
             // chunk maximum with three-input maxima: 15 instructions per 32 columns
-            float u[10];
+            if constexpr (T64) {
+              float u[5];
 #pragma unroll
-            for (int i = 0; i < 10; i++) u[i] = ptx::fmax3(v(3 * i), v(3 * i + 1), v(3 * i + 2));
-            cm[hh] = fmaxf(ptx::fmax3(ptx::fmax3(u[0], u[1], u[2]), ptx::fmax3(u[3], u[4], u[5]), ptx::fmax3(u[6], u[7], u[8])),
-                           ptx::fmax3(u[9], v(30), v(31)));
+              for (int i = 0; i < 5; i++) u[i] = ptx::fmax3(v(3 * i), v(3 * i + 1), v(3 * i + 2));
+              cm[hh] = fmaxf(ptx::fmax3(u[0], u[1], u[2]), ptx::fmax3(u[3], u[4], v(15)));
+            } else {
+              float u[10];
+#pragma unroll
+              for (int i = 0; i < 10; i++) u[i] = ptx::fmax3(v(3 * i), v(3 * i + 1), v(3 * i + 2));
+              cm[hh] = fmaxf(ptx::fmax3(ptx::fmax3(u[0], u[1], u[2]), ptx::fmax3(u[3], u[4], u[5]), ptx::fmax3(u[6], u[7], u[8])),
+                             ptx::fmax3(u[9], v(30), v(31)));
+            }
             if (MODE == 0) {
-              // quad all-reduce: the running maximum of the whole row
+              // quad all-reduce: the running maximum of the whole row (T64: of the warpgroup's columns of the row)
               float qm = fmaxf(cm[hh], __shfl_xor_sync(0xffffffffu, cm[hh], 1));
               qm = fmaxf(qm, __shfl_xor_sync(0xffffffffu, qm, 2));
               Mr[hh] = fmaxf(Mr[hh], qm);
-              thr[hh] = fminf(Mr[hh], cap) - fin[FIN_MARGIN + qrow + 8 * hh];
+              thr[hh] = fminf(Mr[hh], cap) - fin[FIN_MARGIN + frow + 8 * hh];
             } else {
               // (largest, second largest) of the quad's four chunk maxima, merged into the row's running pair.  The
               // chunks of the four lanes and of different n-tiles are disjoint column sets, so two distinct columns
@@ -1460,12 +1518,12 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
             // column; bit (31 - b) of (c0 << 16 | c1) = sign of d_b = "bit b is below the threshold".  NaN scores only
             // occur in rows whose margin is not finite (flag 1).
             const uint64_t nthr2 = ptx::pack2(-thr[hh], -thr[hh]);
-            uint32_t c0 = 0, c1 = 0;   // two 16-column chains (shorter dependency chains)
+            uint32_t c0 = 0, c1 = 0;   // two 16-column chains (shorter dependency chains; T64: two 8-column chains)
 #pragma unroll
-            for (int j = 0; j < 16; j++) {
+            for (int j = 0; j < NACC / 4; j++) {
               float x, y;
               ptx::unpack2(ptx::fadd2(ptx::pack2(v(2 * j), v(2 * j + 1)), nthr2), x, y);
-              if (j < 8) {
+              if (j < NACC / 8) {
                 c0 = __funnelshift_l(__float_as_uint(x), c0, 1);
                 c0 = __funnelshift_l(__float_as_uint(y), c0, 1);
               } else {
@@ -1473,7 +1531,9 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
                 c1 = __funnelshift_l(__float_as_uint(y), c1, 1);
               }
             }
-            mask[hh] = __brev(~((c0 << 16) | c1));
+            // T64: bit (15 - b) of (c0 << 8 | c1) is the sign of d_b; shifted to the top so the reversal leaves 16 bits
+            if constexpr (T64) mask[hh] = __brev(~((c0 << 8) | c1) << 16);
+            else mask[hh] = __brev(~((c0 << 16) | c1));
           }
           // one entry per n-tile in which either row holds a candidate in this lane's columns
           if (mask[0] | mask[1]) {
@@ -1497,7 +1557,7 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
         // MODE 2 / 3: this thread gets columns h*64 .. h*64+63 of its row (quad shuffles, see regroup_quad)
         uint32_t r0[32], r1[32];
 #if KMB_KO != 1
-        regroup_quad(acc, lane, r0, r1);
+        if constexpr (MODE >= 2) regroup_quad(acc, lane, r0, r1);   // (MODE 0 / 1 never reach this point)
 #else
         for (int jj = 0; jj < 32; jj++) {   // stand-in values: strictly decreasing, 64 apart -> one candidate per row
           r0[jj] = __float_as_uint(-64.f * static_cast<float>(n * 128 + h * 64 + jj + 1));
@@ -1655,7 +1715,7 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
       if ((lane & 3) == 0) {
 #pragma unroll
         for (int hh = 0; hh < 2; hh++) {
-          fin[FIN_M + qrow + 8 * hh] = Mr[hh];
+          fin[FIN_M + frow + 8 * hh] = Mr[hh];
           if (MODE == 1) fin[FIN_M2 + qrow + 8 * hh] = M2r[hh];
         }
       }
@@ -1862,6 +1922,27 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
+// MODE 0 and the row list at NKB 9..16 (64-row tiles)
+template <bool ROWS, int NKB>
+static void tc_launch_t64_one(unsigned grid, size_t smem, cudaStream_t st, const CUtensorMap& tb, const tc::Params& prm) {
+  if constexpr (ROWS) tc::tc_assign_rows_kernel<NKB><<<grid, tc::N_THREADS, smem, st>>>(tb, prm);
+  else tc::tc_assign_kernel<NKB, 0><<<grid, tc::N_THREADS, smem, st>>>(tb, prm);
+}
+template <bool ROWS>
+static void tc_launch_t64(int nkb, unsigned grid, size_t smem, cudaStream_t st, const CUtensorMap& tb,
+                          const tc::Params& prm) {
+  switch (nkb) {
+    case 9: tc_launch_t64_one<ROWS, 9>(grid, smem, st, tb, prm); break;
+    case 10: tc_launch_t64_one<ROWS, 10>(grid, smem, st, tb, prm); break;
+    case 11: tc_launch_t64_one<ROWS, 11>(grid, smem, st, tb, prm); break;
+    case 12: tc_launch_t64_one<ROWS, 12>(grid, smem, st, tb, prm); break;
+    case 13: tc_launch_t64_one<ROWS, 13>(grid, smem, st, tb, prm); break;
+    case 14: tc_launch_t64_one<ROWS, 14>(grid, smem, st, tb, prm); break;
+    case 15: tc_launch_t64_one<ROWS, 15>(grid, smem, st, tb, prm); break;
+    default: tc_launch_t64_one<ROWS, 16>(grid, smem, st, tb, prm); break;
+  }
+}
+
 template <int MODE>
 static void tc_launch_mode(int nkb, unsigned grid, size_t smem, cudaStream_t st, const CUtensorMap& tb,
                            const tc::Params& prm) {
@@ -1880,6 +1961,7 @@ static void tc_launch_mode(int nkb, unsigned grid, size_t smem, cudaStream_t st,
 static void tc_launch_rows(int nkb, unsigned grid, size_t smem, cudaStream_t st, const CUtensorMap& tb,
                            const tc::Params& prm) {
   using namespace tc;
+  if (tile64(nkb)) return tc_launch_t64<true>(nkb, grid, smem, st, tb, prm);
   switch (nkb) {
     case 1: tc_assign_rows_kernel<1><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
     case 2: tc_assign_rows_kernel<2><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
@@ -1893,7 +1975,8 @@ static void tc_launch_rows(int nkb, unsigned grid, size_t smem, cudaStream_t st,
 }
 static void tc_launch_main(int mode, int nkb, unsigned grid, size_t smem, cudaStream_t st, const CUtensorMap& tb,
                            const tc::Params& prm) {
-  if (mode == 3) tc_launch_mode<3>(nkb, grid, smem, st, tb, prm);
+  if (tc::tile64(nkb)) tc_launch_t64<false>(nkb, grid, smem, st, tb, prm);   // MODE 0 only (tc_yy_supported)
+  else if (mode == 3) tc_launch_mode<3>(nkb, grid, smem, st, tb, prm);
   else if (mode == 2) tc_launch_mode<2>(nkb, grid, smem, st, tb, prm);
   else if (mode == 1) tc_launch_mode<1>(nkb, grid, smem, st, tb, prm);
   else tc_launch_mode<0>(nkb, grid, smem, st, tb, prm);
@@ -1936,8 +2019,22 @@ static cudaError_t tc_set_smem_attr_one(int bytes) {
   if (e != cudaSuccess) return e;
   return cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
 }
+template <int NKB>
+static cudaError_t tc_set_smem_attr_t64(int bytes) {
+  cudaError_t e = cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) return e;
+  return cudaFuncSetAttribute(tc::tc_assign_rows_kernel<NKB>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+}
 static cudaError_t tc_set_smem_attr(int bytes, int nkb) {   // only the instantiation this shape launches
   switch (nkb) {
+    case 9: return tc_set_smem_attr_t64<9>(bytes);
+    case 10: return tc_set_smem_attr_t64<10>(bytes);
+    case 11: return tc_set_smem_attr_t64<11>(bytes);
+    case 12: return tc_set_smem_attr_t64<12>(bytes);
+    case 13: return tc_set_smem_attr_t64<13>(bytes);
+    case 14: return tc_set_smem_attr_t64<14>(bytes);
+    case 15: return tc_set_smem_attr_t64<15>(bytes);
+    case 16: return tc_set_smem_attr_t64<16>(bytes);
     case 1: return tc_set_smem_attr_one<1>(bytes);
     case 2: return tc_set_smem_attr_one<2>(bytes);
     case 3: return tc_set_smem_attr_one<3>(bytes);
@@ -1949,8 +2046,9 @@ static cudaError_t tc_set_smem_attr(int bytes, int nkb) {   // only the instanti
   }
 }
 
+// D <= 512: every mode; 512 < D <= 1024: the Lloyd pass and its row list only (64-row tiles, see tc_yy_supported)
 bool tc_supported(int metric, uint32_t n, int D, uint32_t K) {
-  if (D < 4 || D % 4 != 0 || D > tc::MAX_NKB * tc::KB) return false;   // TMA row pitch must be 16-byte aligned
+  if (D < 4 || D % 4 != 0 || D > tc::MAX_TILE64_NKB * tc::KB) return false;   // TMA row pitch must be 16-byte aligned
   if (K < 2 || K > 16383u * 128u) return false;        // chunk ids are 16 bit (4 per n-tile)
   if (n == 0) return false;
   return true;
@@ -2008,7 +2106,7 @@ cudaError_t tc_plan_create(TcPlan** out, int metric, uint32_t max_n, int D, uint
   TC_TRY(pool_alloc(reinterpret_cast<void**>(&p->cnorm2), sizeof(float) * K));
   TC_TRY(pool_alloc(reinterpret_cast<void**>(&p->musum), sizeof(double) * (D + 1)));
   TC_TRY(pool_alloc(reinterpret_cast<void**>(&p->mu), sizeof(float) * D));
-  TC_TRY(pool_alloc(reinterpret_cast<void**>(&p->neg_mu_s), sizeof(float) * MAX_NKB * KB));
+  TC_TRY(pool_alloc(reinterpret_cast<void**>(&p->neg_mu_s), sizeof(float) * mu_features(p->nkb)));
   {
     const char* nc = getenv("KMCUDA_B200_NO_CENTER");   // A/B switch: uncentred operands (the round-1 filter)
     p->centred = metric == 0 && !(nc && nc[0] == '1');
@@ -2122,7 +2220,7 @@ static cudaError_t tc_prepare(TcPlan* p, const float* C, const float* csq, uint3
   prm.K = p->K;
   prm.nkb = p->nkb;
   prm.nt = p->nt;
-  prm.ntiles = (n + TM - 1) / TM;
+  prm.ntiles = (n + tile_rows(p->nkb) - 1) / tile_rows(p->nkb);
   prm.aug_blob = p->aug_blob;
   prm.stats = p->stats;
   prm.result = nullptr;
@@ -2262,6 +2360,7 @@ cudaError_t tc_assign_rows(TcPlan* p, const float* X, uint32_t nX, const uint32_
 cudaError_t tc_yy_candidates(TcPlan* p, const float* X, const float* C, const float* csq, uint32_t n,
                              const uint32_t* rows, const uint32_t* d_nrows, cudaStream_t st) {
   using namespace tc;
+  if (!tc_yy_supported(p)) return cudaErrorNotSupported;
   if (n > p->max_n) return cudaErrorInvalidValue;
   if ((reinterpret_cast<uintptr_t>(X) & 15) || (reinterpret_cast<uintptr_t>(C) & 15)) return cudaErrorMisalignedAddress;
   cudaError_t e;
@@ -2406,6 +2505,7 @@ void tc_yy_layout_host(const uint32_t* host_groups, uint32_t K, uint32_t G, std:
 
 cudaError_t tc_yy_layout(TcPlan* p, const uint32_t* host_groups, uint32_t G) {
   using namespace tc;
+  if (!tc_yy_supported(p)) return cudaErrorNotSupported;
   std::vector<uint32_t> perm, qgroup, goff, gmem;
   int nt3 = 0;
   tc_yy_layout_host(host_groups, p->K, G, &perm, &qgroup, &goff, &gmem, &nt3);
@@ -2446,6 +2546,7 @@ cudaError_t tc_yy_layout(TcPlan* p, const uint32_t* host_groups, uint32_t G) {
 }
 
 bool tc_yy_layout_ready(TcPlan* p, uint32_t G) { return p && p->table3 && p->G3 == G; }
+bool tc_yy_supported(TcPlan* p) { return p && !tc::tile64(p->nkb); }
 
 // One bounds refresh: bounds[row] = {ub exact, lb[g] valid lower bounds} (see Params, MODE 3).  Rows the filter
 // cannot bound are left on the overflow list (tc_queues) for the caller's exact row refresh.

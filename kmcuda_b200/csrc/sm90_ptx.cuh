@@ -182,9 +182,27 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // keeps the compiler from moving accesses of the accumulator registers across an asynchronous wgmma
-__device__ __forceinline__ void wgmma_fence_acc(float (&d)[64]) {
+template <int N>
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[N]) {
 #pragma unroll
-  for (int i = 0; i < 64; i++) asm volatile("" : "+f"(d[i])::"memory");
+  for (int i = 0; i < N; i++) asm volatile("" : "+f"(d[i])::"memory");
+}
+// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, the same fragment layout as below with j < 8:
+// d[j*4 + h*2 + e] = (row warp*16 + h*8 + lane/4, column 8j + 2*(lane%4) + e)
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
+      : "memory");
 }
 // D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, fp16 operands from shared memory (both K-major), fp32 accumulators in
 // the registers of the warpgroup: d[j*4 + h*2 + e] = (row warp*16 + h*8 + lane/4, column 8j + 2*(lane%4) + e)
