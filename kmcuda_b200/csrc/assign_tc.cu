@@ -28,8 +28,8 @@
 // Shared memory (227 KB per block on H100) holds the whole fp16 A operand of a tile (16 KB per 64 features), so
 // 128-row tiles serve D <= 512.  The A region is a ring of K-block slots with room for more than one tile
 // (D <= 256), so the next tile's first K-blocks are converted while the current one is multiplied.  For D > 256 the
-// pipeline is shallower (see smem_layout).  512 < D <= 1024 (MODE 0 only) uses tiles of 64 rows (8 KB per 64 features);
-// both consumer warpgroups then hold the same rows, each one 64-column half of every n-tile (tile64 below).
+// pipeline is shallower (see smem_layout).  512 < D <= 1024 (MODE 0 and MODE 2) uses tiles of 64 rows (8 KB per 64
+// features); both consumer warpgroups then hold the same rows, each one 64-column half of every n-tile (tile64 below).
 //
 // The same kernel template serves two more callers (MODE template parameter, see tc::Params):
 //   MODE 1  Yinyang local step (reference kmeans.cu:584-672): the samples are a compacted row list; candidates =
@@ -39,6 +39,7 @@
 //           a tile is multiplied with one segment per candidate cluster, both operands centred on that
 //           cluster's centroid; the epilogue keeps the k+1 largest 4-column-group maxima per half-row as its
 //           threshold and records candidate masks in global lists (namespace knn below has the passes around it).
+//           64-row tiles: a row has four parts of 32 columns (two per warpgroup) instead of two halves.
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -104,7 +105,7 @@ static_assert(REGS_WG0 >= 24 && REGS_CONV >= 24 && REGS_EPI >= 24 && REGS_WG0 <=
               REGS_EPI <= 256, "setmaxnreg counts lie in [24, 256]");
 static_assert(REGS_WG0 + REGS_CONV + 2 * REGS_EPI <= 512, "one warp of each warpgroup per 16K-register sub-partition");
 constexpr int MAX_CAND = 32;            // candidates per row before falling back to the full exact pass (one per lane of the finishing warp)
-constexpr int KNN_CAP = 40;             // k-NN: (chunk, mask) entries per half-row in global memory
+constexpr int KNN_CAP = 40;             // k-NN: (chunk, mask) entries per row part (half; NKB 9..16: quarter) in global memory
 constexpr int KNN_MAX_KK = 16;          // k + 1 <= 16 on the tensor-core path
 constexpr float SENTINEL_GUARD = -65000.f;   // padded / dead centroids score exactly -65504: thresholds below this are not trusted
 
@@ -251,6 +252,8 @@ struct Params {
   // constant s^2 |x - c_B|^2 / 2 is folded into the threshold, so everything the epilogue keeps (top-kk list, entry
   // maxima) lives in the translation-invariant score g = -s^2 d^2 / 2.  Every column within the margin of the row's
   // kk-th largest 4-column-group maximum (kk = k + 1, self included) is recorded as (max, mask, chunk id, margin).
+  // 64-row tiles (NKB 9..16): query tile t is half t & 1 of block t >> 1; the per-tile arrays below stay per block and
+  // are read at t >> 1, so the kernel runs 2 * (blocks) tiles and skips a second half without live rows.
   const uint32_t* d_ntiles;
   const uint32_t* tile_nrows;
   const uint32_t* blk_cluster;
@@ -262,8 +265,9 @@ struct Params {
   int kk;
   int knn_first_pass;            // 1: the per-row state starts empty; the tile has TWO segments, both its own cluster:
                                  //    the first sweep only builds the top-kk threshold, the second one only records
-  uint32_t knn_stride;           // = 2 * (table rows): stride of the [kk][stride] top-kk state
-  float* knn_topk;               // [kk][stride] descending group maxima (g-space) of half-row (table row * 2 + h)
+  uint32_t knn_stride;           // = parts * (table rows): stride of the [kk][stride] top-kk state (2 parts per row, 4 at
+                                 //   NKB 9..16)
+  float* knn_topk;               // [kk][stride] descending group maxima (g-space) of part (table row * parts + part)
   uint32_t* knn_cnt;             // [stride] entries used
   uint32_t* knn_flags;           // [stride]
   float* knn_dub;                // [stride] upper bound of the exact distance to the kk-th nearest candidate seen so far
@@ -732,16 +736,24 @@ __device__ __forceinline__ uint32_t compact_list(uint32_t* lst, uint16_t* lnt, u
   return w;
 }
 
+// MODE 2: the n-tiles query tile `tile` is multiplied with, 0 = nothing to do.  T64: tile t is half t & 1 of table
+// block t >> 1 (the per-block arrays are read there); a half without live rows has nothing to do
+template <bool T64>
+__device__ __forceinline__ uint32_t knn_tile_nblk(const Params& p, uint32_t tile) {
+  if (!T64) return p.knn_nblk[tile];
+  return (tile & 1u) * 64u < p.tile_nrows[tile >> 1] ? p.knn_nblk[tile >> 1] : 0u;
+}
+
 // enumerates the n-tiles (blocks of 128 table rows) one sample tile is multiplied with, segment by segment
 // (MODE 0 / 1: one segment = the whole table; MODE 2: one segment per candidate cluster)
-template <int MODE>
+template <int MODE, bool T64 = false>
 struct BlockIter {
   uint32_t cur, lo, hi, left;    // current block, bounds of the current segment, blocks left including cur
   const uint2* rg;
   __device__ __forceinline__ BlockIter(const Params& p, uint32_t tile) {
     if (MODE == 2) {
-      left = p.knn_nblk[tile];
-      rg = p.knn_ranges + p.knn_roff[tile];
+      left = knn_tile_nblk<T64>(p, tile);
+      rg = p.knn_ranges + p.knn_roff[T64 ? tile >> 1 : tile];
       if (left) { lo = cur = rg->x; hi = rg->y; } else { lo = cur = hi = 0; }
     } else {
       left = static_cast<uint32_t>(p.nt);
@@ -784,6 +796,26 @@ __device__ __noinline__ void knn_select_buckets(const float* mine, const float* 
       if (!((taken >> j) & 1ull) && v > best) { best = v; bi = j; }
     }
     if (bi >= 0) taken |= 1ull << bi;
+    out[o] = best - goff;
+  }
+}
+// the same at 64-row tiles: the kk largest of the row's 128 buckets, 32 in each of its four parts (b = bucket 0 of part
+// 0; part q is TR = 64 columns of the scratch further on)
+__device__ __noinline__ void knn_select_buckets4(const float* b, int kk, float goff, float* out) {
+  unsigned long long taken0 = 0ull, taken1 = 0ull;   // parts 0-1 | parts 2-3
+  for (int o = 0; o < kk; o++) {
+    float best = -INFINITY;
+    int bi = -1;
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+      const unsigned long long tk = q < 2 ? taken0 : taken1;
+      for (int j = 0; j < 32; j++) {
+        const float v = b[q * 64 + j * 256];
+        if (!((tk >> ((q & 1) * 32 + j)) & 1ull) && v > best) { best = v; bi = q * 32 + j; }
+      }
+    }
+    if (bi >= 64) taken1 |= 1ull << (bi - 64);
+    else if (bi >= 0) taken0 |= 1ull << bi;
     out[o] = best - goff;
   }
 }
@@ -834,6 +866,34 @@ __device__ __forceinline__ void regroup_quad(const float (&acc)[64], int lane, u
       }
     }
 }
+// MODE 2 at 64-row tiles: the same for one warp's m64n64 fragment, acc[j*4 + hh*2 + e] = (row hh*8 + lane/4, column
+// 8j + 2t + e of the warpgroup's 64-column half), j < 8.  Lane t takes combination c = t of (row hh = c % 2, quarter
+// c / 2) and receives its columns 8jj + 2s + e (jj = 0..3) of the quarter from each quad partner s: r = the quarter's
+// 32 consecutive columns.
+__device__ __forceinline__ void regroup_quad_t64(const float (&acc)[32], int lane, uint32_t (&r)[32]) {
+  const int t = lane & 3;
+#pragma unroll
+  for (int jj = 0; jj < 4; jj++)
+#pragma unroll
+    for (int e2 = 0; e2 < 2; e2++) {
+      // block value of combination c at (jj, e2): acc[((c / 2) * 4 + jj) * 4 + (c % 2) * 2 + e2]
+      const float b00 = acc[jj * 4 + e2], b10 = acc[jj * 4 + 2 + e2];
+      const float b01 = acc[(4 + jj) * 4 + e2], b11 = acc[(4 + jj) * 4 + 2 + e2];
+      float got[4];
+#pragma unroll
+      for (int k = 0; k < 4; k++) {
+        const int c = t ^ k;
+        const float v = (c & 2) ? ((c & 1) ? b11 : b01) : ((c & 1) ? b10 : b00);
+        got[k] = k ? __shfl_xor_sync(0xffffffffu, v, k) : v;
+      }
+#pragma unroll
+      for (int s = 0; s < 4; s++) {
+        const int k = s ^ t;
+        const float v = (k & 2) ? ((k & 1) ? got[3] : got[2]) : ((k & 1) ? got[1] : got[0]);
+        r[8 * jj + 2 * s + e2] = __float_as_uint(v);
+      }
+    }
+}
 
 // NKB: K-blocks of 64 features (compile-time: the MMA issue loop must be branch- and address-arithmetic-free); MODE 0 =
 // Lloyd assignment, 1 = Yinyang local step, 2 = k-NN, 3 = Yinyang bounds refresh (see Params); the kernels below wrap
@@ -844,7 +904,8 @@ __device__ __forceinline__ void regroup_quad(const float (&acc)[64], int lane, u
 template <int NKB, int MODE, bool ROWS>
 __device__ __forceinline__ void
 tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
-  static_assert(NKB <= MAX_NKB || (MODE == 0 && NKB <= MAX_TILE64_NKB), "the A operand of a tile must fit its shared-memory region");
+  static_assert(NKB <= MAX_NKB || ((MODE == 0 || MODE == 2) && NKB <= MAX_TILE64_NKB),
+                "the A operand of a tile must fit its shared-memory region");
   constexpr int BST = b_stages(NKB), AUGB = aug_bufs(NKB), NDEPTH = norm_depth(NKB), ASLOTS = a_slots(NKB);
   // NKB 9..16 (T64): 64-row tiles; consumer warpgroup g holds all 64 rows at columns 64g .. 64g + 63 of every n-tile
   constexpr bool T64 = tile64(NKB);
@@ -870,13 +931,16 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
 #endif
   [[maybe_unused]] const int nt = p.nt;
   const uint32_t n_eff = MODE == 1 ? min(*p.d_nrows, p.n) : p.n;
-  const uint32_t ntiles = MODE == 1 ? (n_eff + TM - 1) / TM : (MODE == 2 ? *p.d_ntiles : p.ntiles);
+  constexpr uint32_t KNN_TPB = T64 ? 2u : 1u;   // MODE 2: query tiles per 128-row table block
+  const uint32_t ntiles = MODE == 1 ? (n_eff + TM - 1) / TM : (MODE == 2 ? *p.d_ntiles * KNN_TPB : p.ntiles);
   // MODE 2 on several GPUs: this device serves the query tiles of part knn_part of knn_nparts (every GPU holds the
-  // whole candidate table; tiles are independent)
+  // whole candidate table; tiles are independent).  The shards are whole blocks, as in range_build_kernel and
+  // expand_kernel.
   uint32_t tile_lo = 0, tile_end = ntiles;
   if (MODE == 2 && p.knn_nparts > 1) {
-    tile_lo = static_cast<uint32_t>(static_cast<uint64_t>(ntiles) * p.knn_part / p.knn_nparts);
-    tile_end = static_cast<uint32_t>(static_cast<uint64_t>(ntiles) * (p.knn_part + 1) / p.knn_nparts);
+    const uint32_t nblk = ntiles / KNN_TPB;
+    tile_lo = static_cast<uint32_t>(static_cast<uint64_t>(nblk) * p.knn_part / p.knn_nparts) * KNN_TPB;
+    tile_end = static_cast<uint32_t>(static_cast<uint64_t>(nblk) * (p.knn_part + 1) / p.knn_nparts) * KNN_TPB;
   }
   const uint32_t tile_begin = tile_lo + blockIdx.x;
 
@@ -921,7 +985,7 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
       if (lane == 0) {
         uint32_t bs = 0, bph = 0, ac = 0;      // B ring stage / phase, bias blocks issued
         for (uint32_t tile = tile_begin; tile < tile_end; tile += gridDim.x) {
-          for (BlockIter<MODE> it(p, tile); it.valid(); it.next()) {
+          for (BlockIter<MODE, T64> it(p, tile); it.valid(); it.next()) {
             const int n = static_cast<int>(it.cur);
 #pragma unroll
             for (int kb = 0; kb < NKB; kb++) {
@@ -1087,7 +1151,7 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
     const float s = p.stats->scale;
     uint32_t si = 0, as = 0, aph = 0;       // segments converted; A ring slot and phase of the next K-block
     for (uint32_t tile = tile_begin; tile < tile_end; tile += gridDim.x) {
-      if (MODE == 2 && p.knn_nblk[tile] == 0) continue;
+      if (MODE == 2 && knn_tile_nblk<T64>(p, tile) == 0) continue;
       const float* xrow = nullptr;
       bool xlive = true;                      // rows past the end of the samples convert as zeros
       if (MODE == 0 || MODE == 3) {
@@ -1100,8 +1164,9 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
         xrow = p.X + static_cast<size_t>(p.rows[li]) * p.D;
       }
       if (MODE == 2)   // padding rows of the table repeat sample 0; they are never recorded
-        xrow = p.X + static_cast<size_t>(min(p.rows[tile * TM + row], p.n - 1)) * p.D;
-      const uint32_t nseg = MODE == 2 ? p.knn_rcount[tile] : 1u;
+        xrow = p.X + static_cast<size_t>(min(p.rows[tile * TR + row], p.n - 1)) * p.D;
+      const uint32_t kblk = T64 ? tile >> 1 : tile;   // MODE 2: the table block of this tile (knn_tile_nblk)
+      const uint32_t nseg = MODE == 2 ? p.knn_rcount[kblk] : 1u;
       for (uint32_t seg = 0; seg < nseg; seg++, si++) {
         // ||x~||^2 and ||s(x - mu) - x~||^2 as even/odd partial sums
         uint64_t nx2 = 0ull, nd2 = 0ull;
@@ -1109,7 +1174,7 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
         const float* mu = reinterpret_cast<const float*>(smem + L.mu);
         float a2 = 0.f, a2c = 0.f, nraw = 0.f;     // MODE 2: Kahan sum of the exact (x-c)^2 s^2, and s^2 (|x|+|c|)^2
         const float* crow = nullptr;
-        if (MODE == 2) crow = p.C + static_cast<size_t>(p.blk_cluster[p.knn_ranges[p.knn_roff[tile] + seg].x]) * p.D;
+        if (MODE == 2) crow = p.C + static_cast<size_t>(p.blk_cluster[p.knn_ranges[p.knn_roff[kblk] + seg].x]) * p.D;
         for (int kb = 0; kb < nkb; kb++) {
           uint32_t pk[32];
 #pragma unroll
@@ -1191,12 +1256,20 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
               ptx::unpack2(o, onx, ond);
               nxl += onx;
               ndl += ond;
+              if (MODE == 2) {   // the k-NN sums too: the two compensated halves meet in one rounding (see row_margin)
+                const uint64_t o2 = __shfl_xor_sync(0xffffffffu, ptx::pack2(a2, a2c), 1);
+                const float onr = __shfl_xor_sync(0xffffffffu, nraw, 1);
+                float oa2, oa2c;
+                ptx::unpack2(o2, oa2, oa2c);
+                a2 = (a2 + oa2) - (a2c + oa2c);
+                nraw += onr;
+              }
             }
             if (!T64 || hsel == 0) {
               norms[row] = nxl + nxh;
               if (MEASURED_RESIDUAL) norms[TM + row] = ndl + ndh;
             }
-            if (MODE == 2) {
+            if (MODE == 2 && (!T64 || hsel == 0)) {
               norms[2 * TM + row] = a2;
               norms[3 * TM + row] = nraw * s * s;
             }
@@ -1216,12 +1289,15 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
     // rows R0 = g*64 + wq*16 + l / 4 and R1 = R0 + 8 at columns 8j + 2t + e (t = l % 4, j < 16, e < 2), so the four
     // lanes of a quad hold all 128 columns of their two rows.  MODE 2 / 3 regroup the fragment with quad shuffles
     // first: each lane then owns one row and one 64-column half of every n-tile, lane l takes the row it already
-    // holds, g*64 + wq*16 + l / 4 + 8 * (l % 2), and half (l % 4) / 2.
+    // holds, g*64 + wq*16 + l / 4 + 8 * (l % 2), and half (l % 4) / 2.  T64 (MODE 2): the same within warpgroup g's
+    // 64-column half, so lane l holds row wq*16 + l / 4 + 8 * (l % 2) at columns 64g + 32 * ((l % 4) / 2) .. +31, part
+    // 2g + (l % 4) / 2 of the row's four.
     const int e = warp - FIRST_EPI_WARP;       // 0..7
     const int g = e >> 2, wq = e & 3;
-    const int h = (lane & 3) >> 1;             // MODE 2 / 3: column half of every 128-column n-tile
-    const int row = g * 64 + wq * 16 + (lane >> 2) + 8 * (lane & 1);
-    const int slot = h * TM + row;             // 0..255
+    const int h = (lane & 3) >> 1;             // MODE 2 / 3: column half of every 128-column n-tile (T64: of g's half)
+    const int row = (T64 ? 0 : g * 64) + wq * 16 + (lane >> 2) + 8 * (lane & 1);
+    const int kpart = T64 ? 2 * g + h : h;     // MODE 2: this thread's part of the row
+    const int slot = kpart * TR + row;         // 0..255
     // T64: both warpgroups hold the same rows R0 / R1 (at columns 64g + 8j + 2t + e, j < 8) and keep their own per-row
     // maximum and margin in the per-tile state at frow = 64g + R0 (the emitters merge the two)
     const int qrow = (T64 ? 0 : g * 64) + wq * 16 + (lane >> 2);   // MODE 0 / 1: R0
@@ -1243,7 +1319,7 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
     const float cap = p.metric == 1 ? p.stats->scale * p.stats->scale : INFINITY;
     uint32_t ac = 0, ti = 0, si = 0;
     for (uint32_t tile = tile_begin; tile < tile_end; tile += gridDim.x) {
-      if (MODE == 2 && p.knn_nblk[tile] == 0) continue;
+      if (MODE == 2 && knn_tile_nblk<T64>(p, tile) == 0) continue;
       const int par = ti & 1;
       uint32_t* lst = reinterpret_cast<uint32_t*>(smem + L.list) + par * LIST_LEN * 256 + lid;   // this thread's entries
       uint16_t* lnt = reinterpret_cast<uint16_t*>(smem + L.list + LIST_ARRAYS * LIST_ARRAY) + par * LIST_LEN * 256 + lid;
@@ -1280,23 +1356,23 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
       }
       uint32_t seg = 0;
       if (MODE == 2) {
-        klive = static_cast<uint32_t>(row) < p.tile_nrows[tile];
-        kslot = (tile * TM + row) * 2u + h;
+        klive = static_cast<uint32_t>(T64 ? (tile & 1) * TR + row : row) < p.tile_nrows[T64 ? tile >> 1 : tile];
+        kslot = (tile * TR + row) * (T64 ? 4u : 2u) + kpart;
         kent = p.knn_entries + static_cast<size_t>(kslot) * KNN_CAP;
         if (p.knn_first_pass || !klive) {
           for (int j = 0; j < p.kk; j++) topk[j * 256] = -INFINITY;
           if (p.knn_first_pass)
             for (int j = 0; j < 32; j++) topk[(16 + j) * 256] = -INFINITY;   // bucket maxima: rows 16..47 of the region
         } else {
-          // second pass: both halves saved the same merged list at the end of the first pass (no insertion happens
-          // in the recording sweep); from here on each half adds its own, disjoint, columns
+          // second pass: every part saved the same merged list at the end of the first pass (no insertion happens
+          // in the recording sweep); from here on each part adds its own, disjoint, columns
           for (int j = 0; j < p.kk; j++) topk[j * 256] = p.knn_topk[static_cast<size_t>(j) * p.knn_stride + kslot];
           cnt = p.knn_cnt[kslot];
           flags = p.knn_flags[kslot];
         }
         M = topk[(p.kk - 1) * 256];                 // MODE 2: M holds the kk-th largest group maximum (g-space)
       }
-      for (BlockIter<MODE> it(p, tile); it.valid(); it.next(), ac++) {
+      for (BlockIter<MODE, T64> it(p, tile); it.valid(); it.next(), ac++) {
         const int n = static_cast<int>(it.cur);
         const int buf = ac % AUGB;
         const uint32_t aph = (ac / AUGB) & 1;
@@ -1416,8 +1492,9 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
             if (MODE == 2) {
               goff = 0.5f * norms[2 * TM + r];
               // centring x - c_B and y - c_B rounds in fp32 (relative to |x|+|c|), and the row constant is subtracted
-              // from scores of its own magnitude
-              E += 1.2e-7f * (__fsqrt_ru(norms[3 * TM + r]) * cmax + p.stats->yabs * xn) + 4.8e-7f * (goff + xn * cmax);
+              // from scores of its own magnitude (T64: + one rounding where the converters add the row's two halves)
+              E += 1.2e-7f * (__fsqrt_ru(norms[3 * TM + r]) * cmax + p.stats->yabs * xn) +
+                   (T64 ? 6.0e-7f : 4.8e-7f) * (goff + xn * cmax);
             }
             float mg = 2.f * E * 1.001f + 1e-30f;
             if (MODE == 2) mg += knn_extra;
@@ -1442,10 +1519,18 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
               // threshold sweep done: both column halves of the row adopt the merged top-kk (the partner half is
               // lane ^ 2 of the same warp)
               float mg[KNN_MAX_KK];
-              __syncwarp();
-              knn_select_buckets(topk + 16 * 256, reinterpret_cast<float*>(smem + L.list) + ((1 - h) * TM + row) + 16 * 256,
-                                 p.kk, goff, mg);
-              __syncwarp();
+              if constexpr (T64) {
+                // the row's four parts sit in both consumer warpgroups: every part's buckets are complete before any
+                // is read, and read before a warpgroup starts its next tile, which resets them
+                ptx::named_bar_sync(1, N_EPI_WARPS * 32);
+                knn_select_buckets4(reinterpret_cast<float*>(smem + L.list) + row + 16 * 256, p.kk, goff, mg);
+                ptx::named_bar_sync(1, N_EPI_WARPS * 32);
+              } else {
+                __syncwarp();
+                knn_select_buckets(topk + 16 * 256, reinterpret_cast<float*>(smem + L.list) + ((1 - h) * TM + row) + 16 * 256,
+                                   p.kk, goff, mg);
+                __syncwarp();
+              }
               for (int j = 0; j < p.kk; j++) topk[j * 256] = mg[j];
               M = mg[p.kk - 1];
             }
@@ -1554,10 +1639,56 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
           }
           continue;
         }
+        if constexpr (MODE == 2 && T64) {
+          // 64-row tiles: this thread gets the 32 columns of its part (regroup_quad_t64) and runs the steps of the
+          // 128-row epilogue below on that one chunk; threshold buckets (n-tile % 4, 4-column group), 32 per part
+          uint32_t r[32];
+#if KMB_KO != 1
+          regroup_quad_t64(acc, lane, r);
+#else
+          for (int jj = 0; jj < 32; jj++) r[jj] = __float_as_uint(-64.f * static_cast<float>(n * 128 + kpart * 32 + jj + 1));
+#endif
+          float t0[8];
+#pragma unroll
+          for (int i = 0; i < 8; i++)
+            t0[i] = fmaxf(fmaxf(__uint_as_float(r[4 * i]), __uint_as_float(r[4 * i + 1])),
+                          fmaxf(__uint_as_float(r[4 * i + 2]), __uint_as_float(r[4 * i + 3])));
+          const float cm0 = fmaxf(fmaxf(fmaxf(t0[0], t0[1]), fmaxf(t0[2], t0[3])), fmaxf(fmaxf(t0[4], t0[5]), fmaxf(t0[6], t0[7])));
+          if (p.knn_first_pass && seg == 0) {
+            float* bk = topk + (16 + 8 * (n & 3)) * 256;
+#pragma unroll
+            for (int i = 0; i < 8; i++) bk[i * 256] = fmaxf(bk[i * 256], t0[i]);
+          } else if (!p.knn_first_pass && cm0 > M + goff) {
+#pragma unroll
+            for (int i = 0; i < 8; i++)
+              if (t0[i] - goff > M) M = knn_topk_insert(topk, p.kk, t0[i] - goff);
+          }
+          const float thr = (M - margin) + goff;
+          const uint64_t nthr2 = ptx::pack2(-thr, -thr);
+          uint32_t c00 = 0, c01 = 0;
+#pragma unroll
+          for (int jj = 0; jj < 32; jj += 2) {
+            float x0, y0;
+            ptx::unpack2(ptx::fadd2(ptx::pack2(__uint_as_float(r[jj]), __uint_as_float(r[jj + 1])), nthr2), x0, y0);
+            if (jj < 16) {
+              c00 = __funnelshift_l(__float_as_uint(x0), c00, 1);
+              c00 = __funnelshift_l(__float_as_uint(y0), c00, 1);
+            } else {
+              c01 = __funnelshift_l(__float_as_uint(x0), c01, 1);
+              c01 = __funnelshift_l(__float_as_uint(y0), c01, 1);
+            }
+          }
+          const uint32_t mask0 = __brev(~((c00 << 16) | c01));
+          // chunk id n * 4 + part: the column decode of expand_kernel (128 n + 64 (part >> 1) + 32 (part & 1)) holds
+          if (klive && !(p.knn_first_pass && seg == 0) && mask0)
+            cnt = knn_append(kent, cnt, M, cm0 - goff, mask0, static_cast<uint32_t>(n) * 4 + kpart, margin, &flags);
+          if (it.seg_last()) { si++; seg++; }
+          continue;
+        }
         // MODE 2 / 3: this thread gets columns h*64 .. h*64+63 of its row (quad shuffles, see regroup_quad)
         uint32_t r0[32], r1[32];
 #if KMB_KO != 1
-        if constexpr (MODE >= 2) regroup_quad(acc, lane, r0, r1);   // (MODE 0 / 1 never reach this point)
+        if constexpr (MODE >= 2 && !T64) regroup_quad(acc, lane, r0, r1);   // (MODE 0 / 1 never reach this point)
 #else
         for (int jj = 0; jj < 32; jj++) {   // stand-in values: strictly decreasing, 64 apart -> one candidate per row
           r0[jj] = __float_as_uint(-64.f * static_cast<float>(n * 128 + h * 64 + jj + 1));
@@ -1922,24 +2053,24 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// MODE 0 and the row list at NKB 9..16 (64-row tiles)
-template <bool ROWS, int NKB>
+// MODE 0, MODE 2 and the row list at NKB 9..16 (64-row tiles)
+template <bool ROWS, int MODE, int NKB>
 static void tc_launch_t64_one(unsigned grid, size_t smem, cudaStream_t st, const CUtensorMap& tb, const tc::Params& prm) {
   if constexpr (ROWS) tc::tc_assign_rows_kernel<NKB><<<grid, tc::N_THREADS, smem, st>>>(tb, prm);
-  else tc::tc_assign_kernel<NKB, 0><<<grid, tc::N_THREADS, smem, st>>>(tb, prm);
+  else tc::tc_assign_kernel<NKB, MODE><<<grid, tc::N_THREADS, smem, st>>>(tb, prm);
 }
-template <bool ROWS>
+template <bool ROWS, int MODE = 0>
 static void tc_launch_t64(int nkb, unsigned grid, size_t smem, cudaStream_t st, const CUtensorMap& tb,
                           const tc::Params& prm) {
   switch (nkb) {
-    case 9: tc_launch_t64_one<ROWS, 9>(grid, smem, st, tb, prm); break;
-    case 10: tc_launch_t64_one<ROWS, 10>(grid, smem, st, tb, prm); break;
-    case 11: tc_launch_t64_one<ROWS, 11>(grid, smem, st, tb, prm); break;
-    case 12: tc_launch_t64_one<ROWS, 12>(grid, smem, st, tb, prm); break;
-    case 13: tc_launch_t64_one<ROWS, 13>(grid, smem, st, tb, prm); break;
-    case 14: tc_launch_t64_one<ROWS, 14>(grid, smem, st, tb, prm); break;
-    case 15: tc_launch_t64_one<ROWS, 15>(grid, smem, st, tb, prm); break;
-    default: tc_launch_t64_one<ROWS, 16>(grid, smem, st, tb, prm); break;
+    case 9: tc_launch_t64_one<ROWS, MODE, 9>(grid, smem, st, tb, prm); break;
+    case 10: tc_launch_t64_one<ROWS, MODE, 10>(grid, smem, st, tb, prm); break;
+    case 11: tc_launch_t64_one<ROWS, MODE, 11>(grid, smem, st, tb, prm); break;
+    case 12: tc_launch_t64_one<ROWS, MODE, 12>(grid, smem, st, tb, prm); break;
+    case 13: tc_launch_t64_one<ROWS, MODE, 13>(grid, smem, st, tb, prm); break;
+    case 14: tc_launch_t64_one<ROWS, MODE, 14>(grid, smem, st, tb, prm); break;
+    case 15: tc_launch_t64_one<ROWS, MODE, 15>(grid, smem, st, tb, prm); break;
+    default: tc_launch_t64_one<ROWS, MODE, 16>(grid, smem, st, tb, prm); break;
   }
 }
 
@@ -1975,8 +2106,10 @@ static void tc_launch_rows(int nkb, unsigned grid, size_t smem, cudaStream_t st,
 }
 static void tc_launch_main(int mode, int nkb, unsigned grid, size_t smem, cudaStream_t st, const CUtensorMap& tb,
                            const tc::Params& prm) {
-  if (tc::tile64(nkb)) tc_launch_t64<false>(nkb, grid, smem, st, tb, prm);   // MODE 0 only (tc_yy_supported)
-  else if (mode == 3) tc_launch_mode<3>(nkb, grid, smem, st, tb, prm);
+  if (tc::tile64(nkb)) {   // MODE 0 and MODE 2 only (tc_yy_supported)
+    if (mode == 2) tc_launch_t64<false, 2>(nkb, grid, smem, st, tb, prm);
+    else tc_launch_t64<false, 0>(nkb, grid, smem, st, tb, prm);
+  } else if (mode == 3) tc_launch_mode<3>(nkb, grid, smem, st, tb, prm);
   else if (mode == 2) tc_launch_mode<2>(nkb, grid, smem, st, tb, prm);
   else if (mode == 1) tc_launch_mode<1>(nkb, grid, smem, st, tb, prm);
   else tc_launch_mode<0>(nkb, grid, smem, st, tb, prm);
@@ -2022,6 +2155,8 @@ static cudaError_t tc_set_smem_attr_one(int bytes) {
 template <int NKB>
 static cudaError_t tc_set_smem_attr_t64(int bytes) {
   cudaError_t e = cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) return e;
+  e = cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
   if (e != cudaSuccess) return e;
   return cudaFuncSetAttribute(tc::tc_assign_rows_kernel<NKB>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
 }
@@ -2788,7 +2923,9 @@ __global__ void prep_table_kernel(const float* __restrict__ X, const float* __re
   }
 }
 
-// one warp per tile: the clusters pass 2 must visit, one segment (block range) per cluster
+// one warp per tile: the clusters pass 2 must visit, one segment (block range) per cluster.  P = parts per row of the
+// candidate pass (2; 4 on 64-row tiles): the tightest of the parts' bounds is the row's
+template <int P>
 __global__ void __launch_bounds__(256)
 range_build_kernel(const uint32_t* __restrict__ d_ntiles, const uint32_t* __restrict__ tile_nrows,
                    const uint32_t* __restrict__ blk_cluster, const uint32_t* __restrict__ blk_first,
@@ -2810,7 +2947,10 @@ range_build_kernel(const uint32_t* __restrict__ d_ntiles, const uint32_t* __rest
     float W = 0.f;
     for (uint32_t r = lane; r < nr; r += 32) {
       const uint32_t row = t * tc::TM + r;
-      const float w = __fsqrt_ru(ysq[row]) * 1.00001f + fminf(dub[2 * row], dub[2 * row + 1]);
+      float ub = dub[P * row];
+#pragma unroll
+      for (int q = 1; q < P; q++) ub = fminf(ub, dub[P * row + q]);
+      const float w = __fsqrt_ru(ysq[row]) * 1.00001f + ub;
       W = (w == w) ? fmaxf(W, w) : INFINITY;
     }
     for (int o = 16; o > 0; o >>= 1) W = fmaxf(W, __shfl_xor_sync(0xffffffffu, W, o));
@@ -2862,7 +3002,9 @@ range_build_kernel(const uint32_t* __restrict__ d_ntiles, const uint32_t* __rest
   }
 }
 
-// one warp per query (table row): final threshold, expansion of the recorded entries into candidate pairs
+// one warp per query (table row): final threshold, expansion of the recorded entries into candidate pairs.  P = parts
+// per row (2 halves; 4 quarters on 64-row tiles), whose lists are merged here
+template <int P>
 __global__ void __launch_bounds__(256)
 expand_kernel(const uint32_t* __restrict__ d_ntiles, int kk, uint32_t stride, const float* __restrict__ topk,
               const uint32_t* __restrict__ cnts, const uint32_t* __restrict__ flags,
@@ -2878,11 +3020,29 @@ expand_kernel(const uint32_t* __restrict__ d_ntiles, int kk, uint32_t stride, co
   for (uint32_t row = row_lo + warp; row < nrows; row += nwarps) {
     const uint32_t self = tab2orig[row];
     if (self == UINT32_MAX) continue;   // padding
-    const uint32_t s0 = 2 * row, s1 = 2 * row + 1;
-    const float k0 = topk[static_cast<size_t>(kk - 1) * stride + s0], k1 = topk[static_cast<size_t>(kk - 1) * stride + s1];
-    const float kth = fmaxf(k0, k1);   // each half saw kk distinct columns at or above its own value
-    const uint32_t fl = flags[s0] | flags[s1];
-    const uint32_t c0 = cnts[s0], c1 = cnts[s1];
+    const uint32_t s0 = P * row;
+    float kq[P];
+#pragma unroll
+    for (int q = 0; q < P; q++) kq[q] = topk[static_cast<size_t>(kk - 1) * stride + s0 + q];
+    float kth = kq[0];   // each part saw kk distinct columns at or above its own value
+#pragma unroll
+    for (int q = 1; q < P; q++) kth = fmaxf(kth, kq[q]);
+    uint32_t fl = flags[s0], cs[P];
+#pragma unroll
+    for (int q = 1; q < P; q++) fl |= flags[s0 + q];
+#pragma unroll
+    for (int q = 0; q < P; q++) cs[q] = cnts[s0 + q];
+    // entry i of the concatenated (part 0, part 1, ...) lists
+    auto entry = [&](uint32_t i) {
+      if constexpr (P == 2)
+        return i < cs[0] ? entries[static_cast<size_t>(s0) * tc::KNN_CAP + i]
+                         : entries[static_cast<size_t>(s0 + 1) * tc::KNN_CAP + (i - cs[0])];
+      uint32_t s = s0;
+#pragma unroll
+      for (int q = 0; q < P - 1; q++)
+        if (s == s0 + q && i >= cs[q]) { i -= cs[q]; s++; }
+      return entries[static_cast<size_t>(s) * tc::KNN_CAP + i];
+    };
     bool fallback = fl != 0 || !(kth > -INFINITY);
     if (lane == 0 && dbg) {
       if (fl & 1) atomicAdd(dbg + 0, 1u);
@@ -2890,13 +3050,13 @@ expand_kernel(const uint32_t* __restrict__ d_ntiles, int kk, uint32_t stride, co
       if (fl & 4) atomicAdd(dbg + 2, 1u);
       if (!(kth > -INFINITY)) atomicAdd(dbg + 3, 1u);
     }
-    // each lane takes entries lane, lane+32, ... of the concatenated (half 0, half 1) lists; an entry survives if
-    // its group maximum is within ITS margin of the final kk-th best
-    uint32_t mine = 0;
-    const uint32_t total_e = c0 + c1;
+    // each lane takes entries lane, lane+32, ... of the concatenated lists; an entry survives if its group maximum is
+    // within ITS margin of the final kk-th best
+    uint32_t mine = 0, total_e = 0;
+#pragma unroll
+    for (int q = 0; q < P; q++) total_e += cs[q];
     for (uint32_t i = lane; i < total_e && !fallback; i += 32) {
-      const uint4 e = i < c0 ? entries[static_cast<size_t>(s0) * tc::KNN_CAP + i]
-                             : entries[static_cast<size_t>(s1) * tc::KNN_CAP + (i - c0)];
+      const uint4 e = entry(i);
       if (__uint_as_float(e.x) >= kth - __uint_as_float(e.w)) {
         uint32_t m = e.y;
         const uint32_t p0 = (e.z >> 2) * 128u + ((e.z >> 1) & 1u) * 64u + (e.z & 1u) * 32u;
@@ -2931,8 +3091,7 @@ expand_kernel(const uint32_t* __restrict__ d_ntiles, int kk, uint32_t stride, co
     }
     uint32_t w = base + pre - mine;
     for (uint32_t i = lane; i < total_e; i += 32) {
-      const uint4 e = i < c0 ? entries[static_cast<size_t>(s0) * tc::KNN_CAP + i]
-                             : entries[static_cast<size_t>(s1) * tc::KNN_CAP + (i - c0)];
+      const uint4 e = entry(i);
       if (__uint_as_float(e.x) >= kth - __uint_as_float(e.w)) {
         uint32_t m = e.y;
         const uint32_t p0 = (e.z >> 2) * 128u + ((e.z >> 1) & 1u) * 64u + (e.z & 1u) * 32u;
@@ -3001,7 +3160,7 @@ select_kernel(int k, const uint32_t* __restrict__ rowq, const uint32_t* __restri
 bool tc_knn_supported(int metric, int k, uint32_t N, int D, uint32_t K) {
   // (the angular metric is served through the L2 pass when the samples have unit length, see tc_knn_search)
   if (k + 1 > tc::KNN_MAX_KK) return false;
-  if (D < 4 || D % 4 != 0 || D > tc::MAX_NKB * tc::KB) return false;
+  if (D < 4 || D % 4 != 0 || D > tc::MAX_TILE64_NKB * tc::KB) return false;   // D > 512: 64-row tiles
   if (N < 4096 || N > (1u << 30)) return false;                    // tiny inputs: not worth the set-up
   if (static_cast<uint64_t>(K) * K > (1ull << 31)) return false;
   return true;
@@ -3027,7 +3186,10 @@ cudaError_t tc_knn_search(int metric, int k, const float* X, const float* C, uin
   const int nkb = (D + KB - 1) / KB, kk = k + 1;
   const uint32_t tmax = nv / TM + K + 1;                 // upper bound of the number of cluster-aligned blocks
   const uint32_t rows_max = tmax * TM;
-  const uint32_t stride = 2 * rows_max;
+  // per-part state of the candidate pass: a row has two 64-column halves, or four 32-column parts on the 64-row tiles
+  // of D > 512 (tc_assign_body); range_build_kernel / expand_kernel merge the parts of a row
+  const bool t64 = tile64(nkb);
+  const uint32_t stride = (t64 ? 4u : 2u) * rows_max;
   const uint64_t want_pool = static_cast<uint64_t>(tmax) * K;
   const uint32_t pool_cap = static_cast<uint32_t>(want_pool < (48u << 20) ? want_pool : (48u << 20));
   const uint32_t pair_cap = static_cast<uint32_t>(std::min<uint64_t>(40ull * nv + 4096, 0xFFFFFFF0ull));
@@ -3126,14 +3288,14 @@ cudaError_t tc_knn_search(int metric, int k, const float* X, const float* C, uin
   prm.knn_part = part; prm.knn_nparts = nparts ? nparts : 1;
   tc_launch_main(2, nkb, grid, smem_bytes, st, tmap, prm);
   KNN_TRY(cudaGetLastError());
-  knn::range_build_kernel<<<num_sms * 4, 256, 0, st>>>(d_ntiles, t_nrows, blk_cluster, blk_first, off, K, cd, radii, ysq,
+  (t64 ? knn::range_build_kernel<4> : knn::range_build_kernel<2>)<<<num_sms * 4, 256, 0, st>>>(d_ntiles, t_nrows, blk_cluster, blk_first, off, K, cd, radii, ysq,
                                                        dub, pool, pool_cap, pool_used, roff2, rcount2, nblk2, d_err,
                                                        d_pairs, part, prm.knn_nparts);
   KNN_TRY(cudaGetLastError());
   prm.knn_ranges = pool; prm.knn_roff = roff2; prm.knn_rcount = rcount2; prm.knn_nblk = nblk2; prm.knn_first_pass = 0;
   tc_launch_main(2, nkb, grid, smem_bytes, st, tmap, prm);
   KNN_TRY(cudaGetLastError());
-  knn::expand_kernel<<<num_sms * 8, 256, 0, st>>>(d_ntiles, kk, stride, topk, kcnt, kflags, entries, tab2orig, pair_cap,
+  (t64 ? knn::expand_kernel<4> : knn::expand_kernel<2>)<<<num_sms * 8, 256, 0, st>>>(d_ntiles, kk, stride, topk, kcnt, kflags, entries, tab2orig, pair_cap,
                                                   pair_row, pair_cand, rowq, fb_rows, counters, pool_used + 2, part,
                                                   prm.knn_nparts);
   KNN_TRY(cudaGetLastError());

@@ -22,6 +22,10 @@ __device__ __forceinline__ void fence_mbar_init() {
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// named barrier `id` (1..15; 0 is __syncthreads) among `nthreads` threads of the CTA, a multiple of 32
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
                : "memory");
