@@ -28,7 +28,7 @@
 // Shared memory (227 KB per block on H100) holds the whole fp16 A operand of a tile (16 KB per 64 features), so
 // 128-row tiles serve D <= 512.  The A region is a ring of K-block slots with room for more than one tile
 // (D <= 256), so the next tile's first K-blocks are converted while the current one is multiplied.  For D > 256 the
-// pipeline is shallower (see smem_layout).  512 < D <= 1024 (MODE 0 and MODE 2) uses tiles of 64 rows (8 KB per 64
+// pipeline is shallower (see smem_layout).  512 < D <= 1024 (every MODE) uses tiles of 64 rows (8 KB per 64
 // features); both consumer warpgroups then hold the same rows, each one 64-column half of every n-tile (tile64 below).
 //
 // The same kernel template serves two more callers (MODE template parameter, see tc::Params):
@@ -64,7 +64,7 @@ constexpr int TM = 128;                 // samples per tile (two wgmma M = 64 ha
 constexpr int TN = 128;                 // centroids per n-tile (wgmma N)
 constexpr int KB = 64;                  // fp16 elements per K-block = one 128-byte swizzle row
 constexpr int MAX_NKB = 8;              // D <= 512: the A operand of a tile lives in shared memory, 16 KiB per K-block
-// 512 < D <= 1024 (MODE 0 only): tiles of 64 rows, both consumer warpgroups on the same rows, each on one 64-column
+// 512 < D <= 1024 (every MODE): tiles of 64 rows, both consumer warpgroups on the same rows, each on one 64-column
 // half of every n-tile (wgmma m64n64k16); an A K-block is 8 KiB, so the whole tile still stays resident
 constexpr int MAX_TILE64_NKB = 16;
 constexpr int MAX_A_SLOTS = 16;
@@ -895,6 +895,41 @@ __device__ __forceinline__ void regroup_quad_t64(const float (&acc)[32], int lan
     }
 }
 
+// MODE 3: folds one row's NQ consecutive quad maxima qm (table quads with group ids gq) into per-group maxima and
+// turns every finished run into a lower bound of the distance to the nearest centroid of that group, merged into
+// yb[g] with an atomic minimum.  A group's run may continue in the other lanes, warpgroups or n-tiles of the row: each
+// piece flushes its own bound, and since the bound never increases with the maximum, the smallest of them is the bound
+// of the group's true maximum.  Eb >= E (the row's score error), xa2lo = lower bound of |s (x - mu)|^2.
+template <int NQ>
+__device__ __forceinline__ void yy_fold_groups(const Params& p, const float (&qm)[NQ], const uint32_t (&gq)[NQ],
+                                               bool emit_ok, uint32_t gown, float Eb, float xa2lo, uint32_t* yb) {
+  const float sc = p.stats->scale;
+  const float inv_s = 1.f / sc, inv_s2 = inv_s * inv_s;   // s is a power of two: exact
+  float run = qm[0];
+#pragma unroll
+  for (int i = 1; i <= NQ; i++) {
+    if (i == NQ || gq[i] != gq[i - 1]) {
+      const uint32_t g = gq[i - 1];
+      if (emit_ok && g < p.G && g != gown) {
+        float v;
+        if (p.metric == 1) {
+          // angular: every dot of the group <= (run + E) / s^2; acos is decreasing; libdevice acosf is good to 2 ulp
+          const float dot = fminf(1.f, fmaxf(-1.f, (run + Eb) * inv_s2));
+          v = fmaxf(0.f, acosf(dot) - 4.0e-6f);
+        } else {
+          // L2: s^2 d^2 = |x^|^2 - 2 score  >=  |x^|^2 - 2 (run + E)
+          const float t = xa2lo - 2.f * (run + Eb);
+          v = t > 0.f ? __fsqrt_rd(t) * inv_s * (1.f - 4.0e-6f) : 0.f;
+        }
+        atomicMin(yb + g, __float_as_uint(v));        // bounds are >= +0: ordered like unsigned integers
+      }
+      if (i < NQ) run = qm[i];
+    } else {
+      run = fmaxf(run, qm[i]);
+    }
+  }
+}
+
 // NKB: K-blocks of 64 features (compile-time: the MMA issue loop must be branch- and address-arithmetic-free); MODE 0 =
 // Lloyd assignment, 1 = Yinyang local step, 2 = k-NN, 3 = Yinyang bounds refresh (see Params); the kernels below wrap
 // it as tc_assign_kernel<NKB, MODE> and tc_assign_rows_kernel<NKB>.  ROWS (MODE 0 only): the
@@ -904,8 +939,7 @@ __device__ __forceinline__ void regroup_quad_t64(const float (&acc)[32], int lan
 template <int NKB, int MODE, bool ROWS>
 __device__ __forceinline__ void
 tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
-  static_assert(NKB <= MAX_NKB || ((MODE == 0 || MODE == 2) && NKB <= MAX_TILE64_NKB),
-                "the A operand of a tile must fit its shared-memory region");
+  static_assert(NKB <= MAX_TILE64_NKB, "the A operand of a tile must fit its shared-memory region");
   constexpr int BST = b_stages(NKB), AUGB = aug_bufs(NKB), NDEPTH = norm_depth(NKB), ASLOTS = a_slots(NKB);
   // NKB 9..16 (T64): 64-row tiles; consumer warpgroup g holds all 64 rows at columns 64g .. 64g + 63 of every n-tile
   constexpr bool T64 = tile64(NKB);
@@ -932,7 +966,7 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
   [[maybe_unused]] const int nt = p.nt;
   const uint32_t n_eff = MODE == 1 ? min(*p.d_nrows, p.n) : p.n;
   constexpr uint32_t KNN_TPB = T64 ? 2u : 1u;   // MODE 2: query tiles per 128-row table block
-  const uint32_t ntiles = MODE == 1 ? (n_eff + TM - 1) / TM : (MODE == 2 ? *p.d_ntiles * KNN_TPB : p.ntiles);
+  const uint32_t ntiles = MODE == 1 ? (n_eff + TR - 1) / TR : (MODE == 2 ? *p.d_ntiles * KNN_TPB : p.ntiles);
   // MODE 2 on several GPUs: this device serves the query tiles of part knn_part of knn_nparts (every GPU holds the
   // whole candidate table; tiles are independent).  The shards are whole blocks, as in range_build_kernel and
   // expand_kernel.
@@ -1047,8 +1081,17 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
             // MODE 1: the second largest of the row's chunk maxima (a lower bound of its second best score).  T64: each
             // warpgroup's maximum covers its own columns only, so each is <= the row maximum and every warpgroup's
             // candidate set contains the one of the row maximum; the final threshold uses the larger of the two.
-            float Mf = MODE == 1 ? fin[FIN_M2 + row] : fin[FIN_M + row];
-            if (T64) Mf = fmaxf(Mf, fin[FIN_M + TR + row]);
+            float Mf;
+            if constexpr (T64 && MODE == 1) {
+              // T64, MODE 1: warpgroup g keeps its own pair (M1_g, M2_g) over its 64 columns of every n-tile.  Two
+              // distinct columns reach each M2_g, and M1_0 / M1_1 come from disjoint columns, so the row's second best
+              // score is >= max(M2_0, M2_1, min(M1_0, M1_1)) (DESIGN §4k).  The MODE 0 merge max(M2_0, M1_1) is not a
+              // lower bound: M1_1 may be the row's best score.
+              Mf = ptx::fmax3(fin[FIN_M2 + row], fin[FIN_M2 + TR + row], fminf(fin[FIN_M + row], fin[FIN_M + TR + row]));
+            } else {
+              Mf = MODE == 1 ? fin[FIN_M2 + row] : fin[FIN_M + row];
+              if (T64) Mf = fmaxf(Mf, fin[FIN_M + TR + row]);
+            }
             const float mg = fin[FIN_MARGIN + row];
             const float thr = fminf(Mf, cap) - mg;
             fl = force;
@@ -1160,7 +1203,7 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
         xrow = p.X + (xlive ? (ROWS ? static_cast<uint64_t>(p.rows[grow]) : grow) : 0ull) * p.D;
       }
       if (MODE == 1) {
-        const uint32_t li = min(tile * TM + row, n_eff - 1);   // ragged tail: repeat the last listed row
+        const uint32_t li = min(tile * TR + row, n_eff - 1);   // ragged tail: repeat the last listed row
         xrow = p.X + static_cast<size_t>(p.rows[li]) * p.D;
       }
       if (MODE == 2)   // padding rows of the table repeat sample 0; they are never recorded
@@ -1289,17 +1332,17 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
     // rows R0 = g*64 + wq*16 + l / 4 and R1 = R0 + 8 at columns 8j + 2t + e (t = l % 4, j < 16, e < 2), so the four
     // lanes of a quad hold all 128 columns of their two rows.  MODE 2 / 3 regroup the fragment with quad shuffles
     // first: each lane then owns one row and one 64-column half of every n-tile, lane l takes the row it already
-    // holds, g*64 + wq*16 + l / 4 + 8 * (l % 2), and half (l % 4) / 2.  T64 (MODE 2): the same within warpgroup g's
+    // holds, g*64 + wq*16 + l / 4 + 8 * (l % 2), and half (l % 4) / 2.  T64 (MODE 2 / 3): the same within warpgroup g's
     // 64-column half, so lane l holds row wq*16 + l / 4 + 8 * (l % 2) at columns 64g + 32 * ((l % 4) / 2) .. +31, part
     // 2g + (l % 4) / 2 of the row's four.
     const int e = warp - FIRST_EPI_WARP;       // 0..7
     const int g = e >> 2, wq = e & 3;
     const int h = (lane & 3) >> 1;             // MODE 2 / 3: column half of every 128-column n-tile (T64: of g's half)
     const int row = (T64 ? 0 : g * 64) + wq * 16 + (lane >> 2) + 8 * (lane & 1);
-    const int kpart = T64 ? 2 * g + h : h;     // MODE 2: this thread's part of the row
+    const int kpart = T64 ? 2 * g + h : h;     // MODE 2 / 3: this thread's part of the row
     const int slot = kpart * TR + row;         // 0..255
     // T64: both warpgroups hold the same rows R0 / R1 (at columns 64g + 8j + 2t + e, j < 8) and keep their own per-row
-    // maximum and margin in the per-tile state at frow = 64g + R0 (the emitters merge the two)
+    // maximum, MODE 1 second-best bound and margin in the per-tile state at frow = 64g + R0 (the emitters merge the two)
     const int qrow = (T64 ? 0 : g * 64) + wq * 16 + (lane >> 2);   // MODE 0 / 1: R0
     const int frow = T64 ? g * TR + qrow : qrow;
     const int lid = e * 32 + lane;                     // MODE 0 / 1: this thread's column of the lists, 0..255
@@ -1346,7 +1389,7 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
       uint32_t* yb = nullptr;
       bool ylive = false;
       if (MODE == 3) {
-        const uint64_t grow = static_cast<uint64_t>(tile) * TM + row;
+        const uint64_t grow = static_cast<uint64_t>(tile) * TR + row;
         ylive = grow < p.n;
         if (ylive) {
           const uint32_t a = p.yy_assign[grow];
@@ -1597,7 +1640,7 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
               const float q1 = fmaxf(a1, b1), q2 = fmaxf(fminf(a1, b1), fmaxf(a2, b2));
               M2r[hh] = ptx::fmax3(M2r[hh], q2, fminf(Mr[hh], q1));
               Mr[hh] = fmaxf(Mr[hh], q1);
-              thr[hh] = fminf(M2r[hh], cap) - fin[FIN_MARGIN + qrow + 8 * hh];
+              thr[hh] = fminf(M2r[hh], cap) - fin[FIN_MARGIN + frow + 8 * hh];
             }
             // candidate mask: d = v - thr as packed pairs, then the sign bits are shifted in with one funnel shift per
             // column; bit (31 - b) of (c0 << 16 | c1) = sign of d_b = "bit b is below the threshold".  NaN scores only
@@ -1685,6 +1728,33 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
           if (it.seg_last()) { si++; seg++; }
           continue;
         }
+        if constexpr (MODE == 3 && T64) {
+          // 64-row tiles: this thread's part 2g + h of the row is 32 consecutive columns (regroup_quad_t64), the table
+          // quads 8 (2g + h) .. +7 of the n-tile.  The lanes of one warp hold two different quarters (h = (l % 4) / 2),
+          // so every lane folds its own 8 quads along its own group ids; the runs of a group split at part boundaries
+          // and each piece flushes its own bound (yy_fold_groups)
+          uint32_t r[32];
+#if KMB_KO != 1
+          regroup_quad_t64(acc, lane, r);
+#else
+          for (int jj = 0; jj < 32; jj++) r[jj] = __float_as_uint(-64.f * static_cast<float>(n * 128 + kpart * 32 + jj + 1));
+#endif
+          float qm[8];
+#pragma unroll
+          for (int i = 0; i < 8; i++)
+            qm[i] = fmaxf(ptx::fmax3(__uint_as_float(r[4 * i]), __uint_as_float(r[4 * i + 1]), __uint_as_float(r[4 * i + 2])),
+                          __uint_as_float(r[4 * i + 3]));
+          uint32_t gq[8];
+          {
+            const uint4* src = reinterpret_cast<const uint4*>(p.yy_qgroup) + static_cast<size_t>(n) * 8 + kpart * 2;
+            const uint4 v0 = __ldg(src), v1 = __ldg(src + 1);
+            gq[0] = v0.x; gq[1] = v0.y; gq[2] = v0.z; gq[3] = v0.w;
+            gq[4] = v1.x; gq[5] = v1.y; gq[6] = v1.z; gq[7] = v1.w;
+          }
+          yy_fold_groups<8>(p, qm, gq, ylive && !(flags & 1u), gown, 0.5f * margin /* >= E */, xa2lo, yb);
+          if (it.seg_last()) si++;
+          continue;
+        }
         // MODE 2 / 3: this thread gets columns h*64 .. h*64+63 of its row (quad shuffles, see regroup_quad)
         uint32_t r0[32], r1[32];
 #if KMB_KO != 1
@@ -1715,33 +1785,8 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
               gq[4 * i] = v.x; gq[4 * i + 1] = v.y; gq[4 * i + 2] = v.z; gq[4 * i + 3] = v.w;
             }
           }
-          const float Eb = 0.5f * margin;                       // >= E
-          const float sc = p.stats->scale;
-          const float inv_s = 1.f / sc, inv_s2 = inv_s * inv_s;   // s is a power of two: exact
-          const bool emit_ok = ylive && !(flags & 1u);
-          float run = qm[0];
-#pragma unroll
-          for (int i = 1; i <= 16; i++) {
-            if (i == 16 || gq[i] != gq[i - 1]) {                // warp-uniform: the table layout is the same for every row
-              const uint32_t g = gq[i - 1];
-              if (emit_ok && g < p.G && g != gown) {
-                float v;
-                if (p.metric == 1) {
-                  // angular: every dot of the group <= (run + E) / s^2; acos is decreasing; libdevice acosf is good to 2 ulp
-                  const float dot = fminf(1.f, fmaxf(-1.f, (run + Eb) * inv_s2));
-                  v = fmaxf(0.f, acosf(dot) - 4.0e-6f);
-                } else {
-                  // L2: s^2 d^2 = |x^|^2 - 2 score  >=  |x^|^2 - 2 (run + E)
-                  const float t = xa2lo - 2.f * (run + Eb);
-                  v = t > 0.f ? __fsqrt_rd(t) * inv_s * (1.f - 4.0e-6f) : 0.f;
-                }
-                atomicMin(yb + g, __float_as_uint(v));        // bounds are >= +0: ordered like unsigned integers
-              }
-              if (i < 16) run = qm[i];
-            } else {
-              run = fmaxf(run, qm[i]);
-            }
-          }
+          // (the group ids are the same in every lane of one column half: the table layout is the same for every row)
+          yy_fold_groups<16>(p, qm, gq, ylive && !(flags & 1u), gown, 0.5f * margin /* >= E */, xa2lo, yb);
           if (it.seg_last()) si++;
           continue;
         }
@@ -1835,9 +1880,10 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
         continue;
       }
       if (MODE == 3) {
-        // rows the filter cannot bound (non-finite data, scores beyond the sentinel range): exact refresh of the row
-        if (ylive && (flags & 1u) && h == 0)
-          p.ovf_rows[atomicAdd(&p.counters[CNT_OVF], 1u)] = static_cast<uint32_t>(tile * TM + row);
+        // rows the filter cannot bound (non-finite data, scores beyond the sentinel range): exact refresh of the row, listed
+        // once, by its part 0 (the flag comes from the row's norms, the same in every part)
+        if (ylive && (flags & 1u) && kpart == 0)
+          p.ovf_rows[atomicAdd(&p.counters[CNT_OVF], 1u)] = static_cast<uint32_t>(tile * TR + row);
         ti++;
         continue;
       }
@@ -1847,7 +1893,7 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
 #pragma unroll
         for (int hh = 0; hh < 2; hh++) {
           fin[FIN_M + frow + 8 * hh] = Mr[hh];
-          if (MODE == 1) fin[FIN_M2 + qrow + 8 * hh] = M2r[hh];
+          if (MODE == 1) fin[FIN_M2 + frow + 8 * hh] = M2r[hh];   // T64: one pair per (row, warpgroup)
         }
       }
       __syncwarp();
@@ -2106,8 +2152,10 @@ static void tc_launch_rows(int nkb, unsigned grid, size_t smem, cudaStream_t st,
 }
 static void tc_launch_main(int mode, int nkb, unsigned grid, size_t smem, cudaStream_t st, const CUtensorMap& tb,
                            const tc::Params& prm) {
-  if (tc::tile64(nkb)) {   // MODE 0 and MODE 2 only (tc_yy_supported)
-    if (mode == 2) tc_launch_t64<false, 2>(nkb, grid, smem, st, tb, prm);
+  if (tc::tile64(nkb)) {
+    if (mode == 3) tc_launch_t64<false, 3>(nkb, grid, smem, st, tb, prm);
+    else if (mode == 2) tc_launch_t64<false, 2>(nkb, grid, smem, st, tb, prm);
+    else if (mode == 1) tc_launch_t64<false, 1>(nkb, grid, smem, st, tb, prm);
     else tc_launch_t64<false, 0>(nkb, grid, smem, st, tb, prm);
   } else if (mode == 3) tc_launch_mode<3>(nkb, grid, smem, st, tb, prm);
   else if (mode == 2) tc_launch_mode<2>(nkb, grid, smem, st, tb, prm);
@@ -2156,7 +2204,11 @@ template <int NKB>
 static cudaError_t tc_set_smem_attr_t64(int bytes) {
   cudaError_t e = cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
   if (e != cudaSuccess) return e;
+  e = cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) return e;
   e = cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) return e;
+  e = cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
   if (e != cudaSuccess) return e;
   return cudaFuncSetAttribute(tc::tc_assign_rows_kernel<NKB>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
 }
@@ -2181,7 +2233,7 @@ static cudaError_t tc_set_smem_attr(int bytes, int nkb) {   // only the instanti
   }
 }
 
-// D <= 512: every mode; 512 < D <= 1024: the Lloyd pass and its row list only (64-row tiles, see tc_yy_supported)
+// every mode up to D = 1024 (512 < D <= 1024 on 64-row tiles; k-NN keeps its own checks in tc_knn_supported)
 bool tc_supported(int metric, uint32_t n, int D, uint32_t K) {
   if (D < 4 || D % 4 != 0 || D > tc::MAX_TILE64_NKB * tc::KB) return false;   // TMA row pitch must be 16-byte aligned
   if (K < 2 || K > 16383u * 128u) return false;        // chunk ids are 16 bit (4 per n-tile)
@@ -2681,7 +2733,8 @@ cudaError_t tc_yy_layout(TcPlan* p, const uint32_t* host_groups, uint32_t G) {
 }
 
 bool tc_yy_layout_ready(TcPlan* p, uint32_t G) { return p && p->table3 && p->G3 == G; }
-bool tc_yy_supported(TcPlan* p) { return p && !tc::tile64(p->nkb); }
+// the Yinyang local step (MODE 1) and bounds refresh (MODE 3) run on every plan (NKB 9..16 on 64-row tiles)
+bool tc_yy_supported(TcPlan* p) { return p != nullptr; }
 
 // One bounds refresh: bounds[row] = {ub exact, lb[g] valid lower bounds} (see Params, MODE 3).  Rows the filter
 // cannot bound are left on the overflow list (tc_queues) for the caller's exact row refresh.

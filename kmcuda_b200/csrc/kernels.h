@@ -257,8 +257,8 @@ struct TcQueues {
   const uint32_t* ovf_rows;   // rows the filter could not bound
   const uint32_t* d_novf;
 };
-// the plan also serves the Yinyang local step and bounds refresh (MODE 1 / 3), i.e. D <= 512; at 512 < D <= 1024 only
-// the Lloyd pass and its row list run on the tensor cores, and the Yinyang steps take the exact kernels
+// the plan also serves the Yinyang local step and bounds refresh (MODE 1 / 3), at every D it supports (512 < D <= 1024
+// on 64-row tiles)
 bool tc_yy_supported(TcPlan* plan);
 cudaError_t tc_yy_candidates(TcPlan* plan, const float* X, const float* C, const float* csq, uint32_t n,
                              const uint32_t* rows, const uint32_t* d_nrows, cudaStream_t st);

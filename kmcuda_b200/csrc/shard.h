@@ -171,7 +171,7 @@ class Shard {
   DevBuf<float> prev_sums;   // cosine update: member sums of the previous iteration
   DevBuf<char> ws_cub;
   TcPlan* tc = nullptr;
-  // the plan of the Yinyang local step and bounds refresh: nullptr (exact kernels) when the plan serves the Lloyd pass only
+  // the plan of the Yinyang local step and bounds refresh: nullptr (exact kernels) when the plan does not serve them
   TcPlan* yy_tc() const { return tc_yy_supported(tc) ? tc : nullptr; }
 
   // Yinyang state (per shard)
