@@ -58,6 +58,26 @@ KMCUDAResult kmcuda_b200_kmeans_weighted(KMCUDAInitMethod init, const void *init
                                          const float *samples, const float *weights, float *centroids,
                                          uint32_t *assignments, float *average_distance);
 
+/* kmcuda_b200_kmeans_weighted() (weights == NULL: the unweighted run) that relocates empty clusters, as scikit-learn's
+ * KMeans does, instead of the reference's rule.  In every centroid update, after the member sums of all devices are
+ * added and before they are normalised, the clusters whose weight total (member count without weights) is 0 are empty;
+ * in ascending order they take the rows of a walk over (d desc, row asc), d = a row's exact distance to the centroid it
+ * is assigned to (L2: the Kahan sum of squared differences before the square root; angular: the angle).  Rows without a
+ * centroid, of weight 0 or with a non-finite d are never taken, nor is a row whose removal would leave its cluster a
+ * weight total <= 0 (fp32, in walk order; without weights: its last member).  A taken row x of weight w leaves the
+ * donor's sums, count and weight total and becomes the empty cluster's only member: the L2 centroid is w x / w, the
+ * angular one x / ||x||.  The assignments are not changed; the next assignment pass moves the rows.  Clusters left
+ * empty when the walk runs out keep the reference rule (L2: NaN).  Verbosity >= 1 logs "iteration %d: %u empty
+ * clusters relocated" (", %u left empty" when the walk ran out), verbosity >= 2 one line per relocation.  With
+ * KMCUDA_B200_STRICT_UPDATE=1 the call returns kmcudaInvalidArguments.  Without empty clusters the result is
+ * bit-identical to kmcuda_b200_kmeans_weighted(). */
+KMCUDAResult kmcuda_b200_kmeans_relocate(KMCUDAInitMethod init, const void *init_params, float tolerance,
+                                         float yinyang_t, KMCUDADistanceMetric metric, uint32_t samples_size,
+                                         uint16_t features_size, uint32_t clusters_size, uint32_t seed,
+                                         uint32_t device, int32_t device_ptrs, int32_t fp16x2, int32_t verbosity,
+                                         const float *samples, const float *weights, float *centroids,
+                                         uint32_t *assignments, float *average_distance);
+
 /* Mini-batch k-means (Sculley, "Web-scale k-means clustering", WWW 2010), scikit-learn's MiniBatchKMeans with this
  * library's draws.  init, init_params, tolerance, metric ... weights and the outputs are those of
  * kmcuda_b200_kmeans_weighted(); `init` runs on the full data exactly as there.  Then step s = 1, 2, ... draws

@@ -5,7 +5,8 @@ Python surface = the reference's `libKMCUDA` module (reference src/python.cc:33-
     kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1, metric="L2",
                 average_distance=False, seed=time(), device=0, verbosity=0,   # python.cc:159-410
                 sample_weight=None,                                           # extension: per-sample weights
-                batch_size=None, max_steps=0)                                 # extension: mini-batch k-means
+                batch_size=None, max_steps=0,                                 # extension: mini-batch k-means
+                relocate_empty_clusters=False)                                # extension: scikit-learn's relocation
                 init="k-means||" / ("k-means||", rounds)                      # extension: k-means|| seeding
     knn_cuda(k, samples, centroids, assignments, metric="L2", device=0, verbosity=0)  # python.cc:412-632
     supports_fp16                                                             # python.cc:52
@@ -40,6 +41,8 @@ _lib.kmeans_cuda.argtypes = [
 _lib.kmcuda_b200_kmeans_weighted.restype = ctypes.c_int
 _lib.kmcuda_b200_kmeans_weighted.argtypes = _lib.kmeans_cuda.argtypes[:14] + [ctypes.c_void_p] + \
     _lib.kmeans_cuda.argtypes[14:]
+_lib.kmcuda_b200_kmeans_relocate.restype = ctypes.c_int
+_lib.kmcuda_b200_kmeans_relocate.argtypes = _lib.kmcuda_b200_kmeans_weighted.argtypes
 _lib.kmcuda_b200_kmeans_minibatch.restype = ctypes.c_int
 _lib.kmcuda_b200_kmeans_minibatch.argtypes = _lib.kmeans_cuda.argtypes[:3] + _lib.kmeans_cuda.argtypes[4:14] + \
     [ctypes.c_void_p, ctypes.c_uint32, ctypes.c_uint32] + _lib.kmeans_cuda.argtypes[14:]
@@ -158,7 +161,7 @@ def _raise_for(result, fn):
 
 def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1, metric="L2",
                 average_distance=False, seed=None, device=0, verbosity=0, sample_weight=None, batch_size=None,
-                max_steps=0):
+                max_steps=0, relocate_empty_clusters=False):
     """K-means on the GPU(s); see the module docstring.  Returns (centroids, assignments[, avg_distance]).
 
     sample_weight: one non-negative weight per sample (include/kmcuda_b200.h, kmcuda_b200_kmeans_weighted), a 1-D
@@ -166,7 +169,17 @@ def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1
 
     batch_size: an int >= 1 runs mini-batch k-means (kmcuda_b200_kmeans_minibatch, scikit-learn's MiniBatchKMeans)
     with batches of min(batch_size, N) rows for at most max_steps steps (0 = 100 * N // batch size) on one GPU, L2
-    only; yinyang_t is ignored.  None = the Lloyd / Yinyang run."""
+    only; yinyang_t is ignored.  None = the Lloyd / Yinyang run.
+
+    relocate_empty_clusters: True moves every cluster that ends an update without members to one of the samples
+    farthest from their centroids (kmcuda_b200_kmeans_relocate, scikit-learn's KMeans rule) instead of leaving a NaN
+    centroid; not with batch_size (mini-batch has its own reassignment)."""
+    if not isinstance(relocate_empty_clusters, (bool, np.bool_)):
+        raise TypeError("\"relocate_empty_clusters\" must be a bool, got %r" % (relocate_empty_clusters,))
+    relocate_empty_clusters = bool(relocate_empty_clusters)
+    if relocate_empty_clusters and batch_size is not None:
+        raise ValueError("\"relocate_empty_clusters\" applies to Lloyd / Yinyang runs: mini-batch k-means "
+                         "(\"batch_size\") reassigns its clusters itself")
     clusters = int(clusters)
     if batch_size is not None:
         batch_size = _count(batch_size, "batch_size", 1)
@@ -258,6 +271,8 @@ def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1
             print("mini-batch k-means: yinyang_t is ignored", flush=True)
         result = _lib.kmcuda_b200_kmeans_minibatch(*common[:3], *common[4:], weights_ptr, batch_size, max_steps,
                                                    *outputs)
+    elif relocate_empty_clusters:
+        result = _lib.kmcuda_b200_kmeans_relocate(*common, weights_ptr, *outputs)
     elif weights_ptr is None:
         result = _lib.kmeans_cuda(*common, *outputs)
     else:

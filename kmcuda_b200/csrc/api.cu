@@ -63,14 +63,14 @@ static KMCUDAResult print_memory_stats(const std::vector<int>& devs) {
 
 using namespace kmb;
 
-// kmeans_cuda and kmcuda_b200_kmeans_weighted (weights == nullptr: the unweighted run)
+// kmeans_cuda, kmcuda_b200_kmeans_weighted and kmcuda_b200_kmeans_relocate (weights == nullptr: the unweighted run)
 static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, float tolerance,
                                 float yinyang_t, KMCUDADistanceMetric metric, uint32_t samples_size,
                                 uint16_t features_size, uint32_t clusters_size, uint32_t seed,
                                 uint32_t device, int32_t device_ptrs, int32_t fp16x2, int32_t verbosity,
                                 const float* samples, const float* weights, float* centroids,
                                 uint32_t* assignments, float* average_distance, bool minibatch = false,
-                                uint32_t batch_size = 0, uint32_t max_steps = 0) {
+                                uint32_t batch_size = 0, uint32_t max_steps = 0, bool relocate = false) {
   KMB_DEBUG("arguments: %d %p %.3f %.2f %d %" PRIu32 " %" PRIu16 " %" PRIu32 " %" PRIu32 " %" PRIu32
             " %d %" PRIi32 " %p %p %p %p\n", init, init_params, tolerance, yinyang_t, metric, samples_size,
             features_size, clusters_size, seed, device, fp16x2, verbosity, samples, centroids, assignments,
@@ -109,6 +109,14 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
       return kmcudaInvalidArguments;
     }
   }
+  if (relocate) {
+    // strict mode replays the reference's update, which leaves empty clusters alone
+    const char* su = getenv("KMCUDA_B200_STRICT_UPDATE");
+    if (su && su[0] == '1') {
+      KMB_INFO("relocating empty clusters cannot be combined with KMCUDA_B200_STRICT_UPDATE=1\n");
+      return kmcudaInvalidArguments;
+    }
+  }
   KMB_INFO("reassignments threshold: %" PRIu32 "\n", static_cast<uint32_t>(tolerance * samples_size));
   const uint32_t yy_groups_size = static_cast<uint32_t>(yinyang_t * clusters_size);
   KMB_DEBUG("yinyang groups: %" PRIu32 "\n", yy_groups_size);
@@ -120,6 +128,7 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
   g_prof.begin(dev_ids);
   Job job(m, samples_size, D, clusters_size, verbosity);
   job.weighted = weights != nullptr;
+  job.relocate_empty = relocate;
   KMB_RET(job.setup(dev_ids));
   g_prof.mark("setup: exchange (peer / nccl)");
   KMB_RET(job.ingest(samples, weights, device_ptrs, fp16x2 != 0));
@@ -174,6 +183,17 @@ KMCUDAResult kmcuda_b200_kmeans_weighted(KMCUDAInitMethod init, const void* init
   return kmeans_impl(init, init_params, tolerance, yinyang_t, metric, samples_size, features_size, clusters_size, seed,
                      device, device_ptrs, fp16x2, verbosity, samples, weights, centroids, assignments,
                      average_distance);
+}
+
+KMCUDAResult kmcuda_b200_kmeans_relocate(KMCUDAInitMethod init, const void* init_params, float tolerance,
+                                         float yinyang_t, KMCUDADistanceMetric metric, uint32_t samples_size,
+                                         uint16_t features_size, uint32_t clusters_size, uint32_t seed,
+                                         uint32_t device, int32_t device_ptrs, int32_t fp16x2, int32_t verbosity,
+                                         const float* samples, const float* weights, float* centroids,
+                                         uint32_t* assignments, float* average_distance) {
+  return kmeans_impl(init, init_params, tolerance, yinyang_t, metric, samples_size, features_size, clusters_size, seed,
+                     device, device_ptrs, fp16x2, verbosity, samples, weights, centroids, assignments,
+                     average_distance, false, 0, 0, true);
 }
 
 KMCUDAResult kmcuda_b200_kmeans_minibatch(KMCUDAInitMethod init, const void* init_params, float tolerance,

@@ -83,4 +83,51 @@ __device__ __forceinline__ float distance_exact(const float* __restrict__ a,
   return finalize_distance<METRIC>(k.sum);
 }
 
+// Staged pass body of the per-row kernels that need each row's exact distance to its own centroid (mini-batch inertia,
+// relocation keys): kStagedRows rows per CTA, one thread per row, 32-feature slices of the rows staged through padded
+// shared memory (coalesced loads), the own centroid `c` read as float4 when VEC4 (D % 4 == 0).  s_row[r] is the
+// sample of CTA row r (rows row0 + r >= n are padding); tile holds kStagedRows * 33 floats.  Returns the Kahan sum of
+// (x - c)^2 (METRIC 0) or of x * c (METRIC 1) in the reference's order; meaningful only where `live`.
+constexpr int kStagedRows = 128;
+
+template <bool VEC4, int METRIC>
+__device__ __forceinline__ float staged_own_sum(const float* __restrict__ X, const uint32_t* s_row, uint32_t row0,
+                                                uint32_t n, int D, const float* __restrict__ c, bool live,
+                                                float* tile) {
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  Kahan k;
+  for (int f0 = 0; f0 < D; f0 += 32) {
+    const int fl = min(32, D - f0);
+#pragma unroll 8
+    for (int rr = 0; rr < 32; rr++) {
+      const int r = warp + 4 * rr;
+      tile[r * 33 + lane] = (row0 + r < n && lane < fl) ? X[static_cast<size_t>(s_row[r]) * D + f0 + lane] : 0.f;
+    }
+    __syncthreads();
+    if (live) {
+      const float* xs = tile + t * 33;
+      if (VEC4 && fl == 32) {
+#pragma unroll
+        for (int q = 0; q < 8; q++) {
+          const float4 cv = __ldg(reinterpret_cast<const float4*>(c + f0) + q);
+          if (METRIC == 1) {
+            k.mac(xs[4 * q], cv.x); k.mac(xs[4 * q + 1], cv.y);
+            k.mac(xs[4 * q + 2], cv.z); k.mac(xs[4 * q + 3], cv.w);
+          } else {
+            k.sqdiff(xs[4 * q], cv.x); k.sqdiff(xs[4 * q + 1], cv.y);
+            k.sqdiff(xs[4 * q + 2], cv.z); k.sqdiff(xs[4 * q + 3], cv.w);
+          }
+        }
+      } else {
+        for (int f = 0; f < fl; f++) {
+          if (METRIC == 1) k.mac(xs[f], __ldg(c + f0 + f));
+          else k.sqdiff(xs[f], __ldg(c + f0 + f));
+        }
+      }
+    }
+    __syncthreads();
+  }
+  return k.sum;
+}
+
 }  // namespace kmb

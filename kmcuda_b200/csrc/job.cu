@@ -253,7 +253,7 @@ KMCUDAResult Job::assign_pass(uint32_t* changed) {
 }
 
 // centroid update: shard partial sums -> exchange (peer-memory reduce, or NCCL all-reduce) -> normalise on every GPU
-KMCUDAResult Job::update() {
+KMCUDAResult Job::update(int iter) {
   if (devs.size() == 1 && devs[0].shard->strict_update) {
     // strict parity mode: the reference's running sums in sample order (bit-identical centroids, one GPU)
     Dev& d = devs[0];
@@ -289,11 +289,12 @@ KMCUDAResult Job::update() {
       KMB_CU(launch_peer_reduce(pb, K, D, d.rsums, d.rcounts, d.st), kmcudaRuntimeError);
       if (weighted) KMB_CU(launch_peer_sum_f32(pw, K, d.rweights, d.st), kmcudaRuntimeError);
       KMB_CU(cudaEventRecord(d.ev_reduced, d.st), kmcudaRuntimeError);
-      KMB_RET(d.shard->finish_update(d.rsums, d.rcounts, d.C, d.ccounts, d.st, d.rweights.get(), d.cweights.get()));
+      if (!relocate_empty)
+        KMB_RET(d.shard->finish_update(d.rsums, d.rcounts, d.C, d.ccounts, d.st, d.rweights.get(), d.cweights.get()));
     }
-    return kmcudaSuccess;
+    if (!relocate_empty) return kmcudaSuccess;
   }
-  if (devs.size() > 1) {
+  if (devs.size() > 1 && !peer_exchange) {
     const NcclApi& nc = nccl_api();
     ncclResult_t r = nc.GroupStart();
     for (auto& d : devs) {
@@ -312,9 +313,191 @@ KMCUDAResult Job::update() {
       return kmcudaRuntimeError;
     }
   }
+  if (relocate_empty) KMB_RET(relocate(iter));
+  const bool pe = devs.size() > 1 && peer_exchange;
   for (auto& d : devs) {
     KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
-    KMB_RET(d.shard->finish_update(d.sums, d.counts, d.C, d.ccounts, d.st, d.wsums.get(), d.cweights.get()));
+    if (pe) KMB_RET(d.shard->finish_update(d.rsums, d.rcounts, d.C, d.ccounts, d.st, d.rweights.get(), d.cweights.get()));
+    else KMB_RET(d.shard->finish_update(d.sums, d.counts, d.C, d.ccounts, d.st, d.wsums.get(), d.cweights.get()));
+    if (metric == 1 && relocated)
+      KMB_CU(launch_reloc_cos_overwrite(d.C, D, d.rl_x, d.rl_meta, relocated, d.st), kmcudaRuntimeError);
+  }
+  return kmcudaSuccess;
+}
+
+// Empty-cluster relocation (DESIGN.md §4l), between the exchange and the normalisation: d.C still holds the centroids
+// the assignments were made against.  The empty clusters E (exchanged weight total, or count, 0; ascending) take, in
+// order, the rows of the walk over (d desc, global row asc) that leave their donor a weight total > 0.  Every device
+// offers its top T rows; the merged list is trusted down to the last key of any device that has more eligible rows, and
+// T doubles while the walk runs out above that point.  All devices then apply the same records to the same totals.
+KMCUDAResult Job::relocate(int iter) {
+  relocated = 0;
+  const bool pe = devs.size() > 1 && peer_exchange;
+  Dev& d0 = devs[0];
+  std::vector<float> W(K);
+  KMB_CU(cudaSetDevice(d0.dev), kmcudaRuntimeError);
+  if (weighted) {
+    KMB_CU(cudaMemcpyAsync(W.data(), pe ? d0.rweights.get() : d0.wsums.get(), sizeof(float) * K,
+                           cudaMemcpyDeviceToHost, d0.st), kmcudaMemoryCopyError);
+    KMB_CU(cudaStreamSynchronize(d0.st), kmcudaRuntimeError);
+  } else {
+    std::vector<uint32_t> cnt(K);
+    KMB_CU(cudaMemcpyAsync(cnt.data(), pe ? d0.rcounts.get() : d0.counts.get(), sizeof(uint32_t) * K,
+                           cudaMemcpyDeviceToHost, d0.st), kmcudaMemoryCopyError);
+    KMB_CU(cudaStreamSynchronize(d0.st), kmcudaRuntimeError);
+    for (uint32_t c = 0; c < K; c++) W[c] = static_cast<float>(cnt[c]);
+  }
+  std::vector<uint32_t> E;
+  for (uint32_t c = 0; c < K; c++)
+    if (W[c] == 0) E.push_back(c);
+  if (E.empty()) return kmcudaSuccess;
+  const uint32_t m = static_cast<uint32_t>(E.size());
+  for (auto& d : devs) {
+    if (d.len == 0) continue;
+    KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+    if (!d.rl_keys.get()) {
+      KMB_CU(d.rl_keys.alloc(d.len), kmcudaMemoryAllocationFailure);
+      KMB_CU(d.rl_state.alloc(sizeof(RelocState) / sizeof(uint64_t)), kmcudaMemoryAllocationFailure);
+      KMB_CU(d.rl_hist.alloc(256), kmcudaMemoryAllocationFailure);
+      KMB_CU(d.rl_nsel.alloc(1), kmcudaMemoryAllocationFailure);
+    }
+    KMB_CU(launch_reloc_keys(metric, d.X, d.len, D, d.C, K, d.assign, d.w.get(), d.off, d.rl_keys, d.st),
+           kmcudaRuntimeError);
+  }
+  struct Cand {
+    uint64_t key;
+    uint32_t dev, donor;
+    float w;
+  };
+  std::vector<Cand> taken;
+  std::vector<std::vector<uint64_t>> tops(devs.size());
+  std::vector<std::vector<uint32_t>> metas(devs.size());
+  std::vector<RelocState> states(devs.size());
+  for (uint32_t T = 2 * m + 32;; T *= 2) {
+    for (size_t i = 0; i < devs.size(); i++) {
+      Dev& d = devs[i];
+      tops[i].clear();
+      if (d.len == 0) continue;
+      KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+      RelocSelect s;
+      s.n = d.len;
+      s.T = std::min(T, d.len);
+      s.cap = reloc_cap(s.T);
+      if (s.cap > d.rl_cap) {
+        KMB_CU(d.rl_sel.alloc(s.cap), kmcudaMemoryAllocationFailure);
+        KMB_CU(d.rl_top.alloc(s.cap), kmcudaMemoryAllocationFailure);
+        KMB_CU(d.rl_meta.alloc(2 * static_cast<size_t>(s.cap)), kmcudaMemoryAllocationFailure);
+        KMB_CU(d.rl_tmp.alloc(reloc_select_bytes(d.len, s.cap)), kmcudaMemoryAllocationFailure);
+        d.rl_cap = s.cap;
+      }
+      s.keys = d.rl_keys;
+      s.state = reinterpret_cast<RelocState*>(d.rl_state.get());
+      s.hist = d.rl_hist;
+      s.sel = d.rl_sel;
+      s.top = d.rl_top;
+      s.nsel = d.rl_nsel;
+      s.tmp = d.rl_tmp.get();
+      s.tmp_bytes = reloc_select_bytes(d.len, s.cap);
+      KMB_CU(launch_reloc_select(s, d.st), kmcudaRuntimeError);
+      KMB_CU(launch_reloc_gather(d.rl_top, s.T, d.off, d.assign, d.w.get(), d.rl_meta, d.st), kmcudaRuntimeError);
+      tops[i].resize(s.T);
+      metas[i].resize(2 * static_cast<size_t>(s.T));
+      KMB_CU(cudaMemcpyAsync(tops[i].data(), d.rl_top.get(), sizeof(uint64_t) * s.T, cudaMemcpyDeviceToHost, d.st),
+             kmcudaMemoryCopyError);
+      KMB_CU(cudaMemcpyAsync(metas[i].data(), d.rl_meta.get(), sizeof(uint32_t) * 2 * s.T, cudaMemcpyDeviceToHost,
+                             d.st), kmcudaMemoryCopyError);
+      KMB_CU(cudaMemcpyAsync(&states[i], s.state, sizeof(RelocState), cudaMemcpyDeviceToHost, d.st),
+             kmcudaMemoryCopyError);
+    }
+    KMB_RET(sync_all());
+    std::vector<Cand> list;
+    uint64_t cutoff = 0;   // keys below the last one listed by a device with more eligible rows are not trusted
+    for (size_t i = 0; i < devs.size(); i++) {
+      uint32_t listed = 0;
+      for (; listed < tops[i].size() && tops[i][listed]; listed++) {
+        float wj;
+        memcpy(&wj, &metas[i][2 * listed + 1], sizeof(wj));
+        list.push_back({tops[i][listed], static_cast<uint32_t>(i), metas[i][2 * listed], wj});
+      }
+      if (!tops[i].empty() && states[i].eligible > listed && listed > 0)
+        cutoff = std::max(cutoff, tops[i][listed - 1]);
+    }
+    std::sort(list.begin(), list.end(), [](const Cand& a, const Cand& b) { return a.key > b.key; });
+    std::vector<float> Wrun(W);
+    taken.clear();
+    for (const Cand& c : list) {
+      if (c.key < cutoff || taken.size() == m) break;
+      const float left = Wrun[c.donor] - c.w;
+      if (!(left > 0.f)) continue;   // the donor would be left without weight
+      Wrun[c.donor] = left;
+      taken.push_back(c);
+    }
+    if (taken.size() == m || cutoff == 0) break;
+  }
+  const uint32_t r = static_cast<uint32_t>(taken.size());
+  if (r == 0) {
+    KMB_INFO("iteration %d: 0 empty clusters relocated, %" PRIu32 " left empty\n", iter, m);
+    return kmcudaSuccess;
+  }
+  // the taken rows, gathered on their devices and broadcast through the host with their records
+  std::vector<float> xs(static_cast<size_t>(r) * D);
+  std::vector<uint32_t> meta(3 * static_cast<size_t>(r));
+  for (uint32_t j = 0; j < r; j++) {
+    meta[3 * j] = E[j];
+    meta[3 * j + 1] = taken[j].donor;
+    memcpy(&meta[3 * j + 2], &taken[j].w, sizeof(float));
+  }
+  for (auto& d : devs) {
+    KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+    KMB_CU(d.rl_x.alloc(static_cast<size_t>(r) * D), kmcudaMemoryAllocationFailure);
+    KMB_CU(d.rl_idx.alloc(r), kmcudaMemoryAllocationFailure);
+  }
+  for (size_t i = 0; i < devs.size(); i++) {
+    Dev& d = devs[i];
+    std::vector<uint32_t> pos, idx;
+    for (uint32_t j = 0; j < r; j++)
+      if (taken[j].dev == i) {
+        pos.push_back(j);
+        idx.push_back(~static_cast<uint32_t>(taken[j].key) - d.off);
+      }
+    if (idx.empty()) continue;
+    const uint32_t cnt = static_cast<uint32_t>(idx.size());
+    std::vector<float> part(static_cast<size_t>(cnt) * D);
+    KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+    KMB_CU(cudaMemcpyAsync(d.rl_idx.get(), idx.data(), sizeof(uint32_t) * cnt, cudaMemcpyHostToDevice, d.st),
+           kmcudaMemoryCopyError);
+    KMB_CU(launch_kmp_gather(d.X, D, d.rl_idx, cnt, d.rl_x, d.st), kmcudaRuntimeError);
+    KMB_CU(cudaMemcpyAsync(part.data(), d.rl_x.get(), sizeof(float) * part.size(), cudaMemcpyDeviceToHost, d.st),
+           kmcudaMemoryCopyError);
+    KMB_CU(cudaStreamSynchronize(d.st), kmcudaRuntimeError);
+    for (uint32_t q = 0; q < cnt; q++)
+      std::copy(part.begin() + static_cast<size_t>(q) * D, part.begin() + static_cast<size_t>(q + 1) * D,
+                xs.begin() + static_cast<size_t>(pos[q]) * D);
+  }
+  for (auto& d : devs) {
+    KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+    KMB_CU(d.rl_meta.alloc(std::max<size_t>(3 * static_cast<size_t>(r), 2 * static_cast<size_t>(d.rl_cap))),
+           kmcudaMemoryAllocationFailure);
+    KMB_CU(cudaMemcpyAsync(d.rl_x.get(), xs.data(), sizeof(float) * xs.size(), cudaMemcpyHostToDevice, d.st),
+           kmcudaMemoryCopyError);
+    KMB_CU(cudaMemcpyAsync(d.rl_meta.get(), meta.data(), sizeof(uint32_t) * meta.size(), cudaMemcpyHostToDevice,
+                           d.st), kmcudaMemoryCopyError);
+    if (pe) KMB_CU(launch_reloc_apply(d.rsums, d.rcounts, d.rweights.get(), D, d.rl_x, d.rl_meta, r, d.st),
+                   kmcudaRuntimeError);
+    else KMB_CU(launch_reloc_apply(d.sums, d.counts, d.wsums.get(), D, d.rl_x, d.rl_meta, r, d.st),
+                kmcudaRuntimeError);
+  }
+  KMB_RET(sync_all());   // the host copies above are pageable and die with this frame
+  relocated = r;
+  if (r < m) KMB_INFO("iteration %d: %" PRIu32 " empty clusters relocated, %" PRIu32 " left empty\n", iter, r, m - r);
+  else KMB_INFO("iteration %d: %" PRIu32 " empty clusters relocated\n", iter, r);
+  for (uint32_t j = 0; j < r; j++) {
+    const uint32_t ob = static_cast<uint32_t>(taken[j].key >> 32);
+    const uint32_t b = (ob & 0x80000000u) ? (ob & 0x7FFFFFFFu) : ~ob;
+    float key;
+    memcpy(&key, &b, sizeof(key));
+    KMB_DEBUG("relocated cluster %" PRIu32 ": sample %" PRIu32 ", key %.9g, donor %" PRIu32 "\n", E[j],
+              ~static_cast<uint32_t>(taken[j].key), key, taken[j].donor);
   }
   return kmcudaSuccess;
 }
@@ -346,7 +529,7 @@ KMCUDAResult Job::lloyd(float tolerance, int* iter_out, uint32_t* changed_out) {
     if (iter_out) *iter_out = iter;
     if (changed_out) *changed_out = changed;
     if (changed <= tolerance * N) return kmcudaSuccess;  // float compare, kmeans.cu:707
-    KMB_RET(update());
+    KMB_RET(update(iter));
     g_prof.mark("centroid update");
   }
 }
@@ -355,7 +538,7 @@ KMCUDAResult Job::lloyd(float tolerance, int* iter_out, uint32_t* changed_out) {
 // the Yinyang iterations of a run turn out slower than its Lloyd passes (Job::yinyang)
 KMCUDAResult Job::lloyd_continue(float tolerance, int iter) {
   for (;;) {
-    KMB_RET(update());
+    KMB_RET(update(iter));
     g_prof.mark("centroid update");
     iter++;
     uint32_t changed = 0;
@@ -484,7 +667,7 @@ KMCUDAResult Job::yinyang(float tolerance, uint32_t G) {
       KMB_CU(cudaMemcpyAsync(d.shard->oldC.get(), d.C.get(), sizeof(float) * static_cast<size_t>(K) * D,
                              cudaMemcpyDeviceToDevice, d.st), kmcudaMemoryCopyError);
     }
-    KMB_RET(update());
+    KMB_RET(update(iter));
     g_prof.mark("centroid update");
     for (auto& d : devs) {
       KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);

@@ -47,6 +47,13 @@ struct Dev {
   // sample weights (weighted jobs only): this shard's slice, the per-cluster weight totals of the shard (wsums), of all
   // shards (rweights, peer exchange) and of the previous update (cweights, the cosine recurrence's old count)
   DevBuf<float> w, wsums, rweights, cweights;
+  // relocation of empty clusters (Job::relocate; allocated at the first update that has an empty cluster): the row keys
+  // of this shard, the top-T selection's scratch, and the relocated rows with their (cluster, donor, weight) records
+  DevBuf<uint64_t> rl_keys, rl_state, rl_sel, rl_top;
+  DevBuf<uint32_t> rl_hist, rl_nsel, rl_meta, rl_idx;
+  DevBuf<float> rl_x;
+  DevBuf<char> rl_tmp;
+  uint32_t rl_cap = 0;
   cudaEvent_t ev_partial = nullptr;   // this device's partial sums are complete
   cudaEvent_t ev_reduced = nullptr;   // this device has finished reading every peer's partial sums
   ncclComm_t comm = nullptr;          // owned by the per-process cache (Job::setup)
@@ -122,6 +129,8 @@ class Job {
   std::vector<Dev> devs;        // sized once by setup()
   bool peer_exchange = false;   // multi-GPU update through peer memory (NVLink / NVSwitch) instead of NCCL
   bool weighted = false;        // per-sample weights (kmcuda_b200_kmeans_weighted); set before setup()
+  bool relocate_empty = false;  // relocate empty clusters in update() (kmcuda_b200_kmeans_relocate)
+  uint32_t relocated = 0;       // rows relocated by the last relocate(), still in every device's rl_x / rl_meta
   double wtotal = 0;            // sum of the weights (check_weights)
   std::vector<float> host_w;    // host copy of the weights for the host-side seeding steps (load_host_weights)
 
@@ -168,7 +177,8 @@ class Job {
   KMCUDAResult init_afkmc2(uint32_t m, uint32_t seed);
   KMCUDAResult init_kmeans_parallel(uint32_t rounds, uint32_t seed);
   KMCUDAResult assign_pass(uint32_t* changed);
-  KMCUDAResult update();
+  KMCUDAResult update(int iter);
+  KMCUDAResult relocate(int iter);
   KMCUDAResult lloyd(float tolerance, int* iter_out, uint32_t* changed_out);
   KMCUDAResult lloyd_continue(float tolerance, int iter);
   KMCUDAResult yinyang(float tolerance, uint32_t G);

@@ -204,6 +204,44 @@ cudaError_t launch_mb_stats(const float* Cold, const float* Cnew, const double* 
 size_t mb_variance_doubles(int D);
 cudaError_t launch_mb_variance(const float* X, uint32_t n, int D, double* work, double* var, cudaStream_t st);
 
+// ---- relocation of empty clusters (relocate.cu) ------------------------------------------------------------------------
+// keys[i] of the shard rows i < n (global row off + i): orderable bits of d_i (L2: the Kahan sum of squared differences
+// to C[assign[i]] before the square root; angular: distance_exact<1>) << 32 | ~(off + i), so that a descending order is
+// (d desc, row asc); 0 when assign[i] >= K, w[i] <= 0 (w optional) or d_i is not finite
+cudaError_t launch_reloc_keys(int metric, const float* X, uint32_t n, int D, const float* C, uint32_t K,
+                              const uint32_t* assign, const float* w, uint32_t off, uint64_t* keys, cudaStream_t st);
+struct RelocState {
+  uint64_t prefix, thr;   // digits fixed so far; the selection threshold
+  uint32_t above, done, eligible, pad;
+};
+// top[0 .. T) = the T largest non-zero keys of keys[n], descending, 0 after the last one; state->eligible = the number
+// of non-zero keys.  Buffers: state [1], hist [256], sel / top [cap = reloc_cap(T)], nsel [1], tmp of
+// reloc_select_bytes(n, cap) bytes
+struct RelocSelect {
+  uint32_t n, T, cap;
+  const uint64_t* keys;
+  RelocState* state;
+  uint32_t* hist;
+  uint64_t *sel, *top;
+  uint32_t* nsel;
+  void* tmp;
+  size_t tmp_bytes;
+};
+uint32_t reloc_cap(uint32_t T);
+size_t reloc_select_bytes(uint32_t n, uint32_t cap);
+cudaError_t launch_reloc_select(const RelocSelect& s, cudaStream_t st);
+// meta[2j] = assign of the row of top[j] (local row ~low word - off), meta[2j + 1] = its weight's bits (1 without w)
+cudaError_t launch_reloc_gather(const uint64_t* top, uint32_t T, uint32_t off, const uint32_t* assign, const float* w,
+                                uint32_t* meta, cudaStream_t st);
+// the r relocations in walk order, meta[3j] = empty cluster, [3j + 1] = donor, [3j + 2] = weight bits, xs [r][D] the
+// rows: sums[donor] -= w x, counts[donor] -= 1, wsums[donor] -= w (wsums optional); sums[e] = w x, counts[e] = 1,
+// wsums[e] = w
+cudaError_t launch_reloc_apply(float* sums, uint32_t* counts, float* wsums, int D, const float* xs,
+                               const uint32_t* meta, uint32_t r, cudaStream_t st);
+// angular, after the normalisation: C[e] = x / ||x|| in the reference's order
+cudaError_t launch_reloc_cos_overwrite(float* C, int D, const float* xs, const uint32_t* meta, uint32_t r,
+                                       cudaStream_t st);
+
 cudaError_t launch_half_to_float(const void* src, float* dst, size_t n, cudaStream_t st);
 cudaError_t launch_float_to_half(const float* src, void* dst, size_t n, cudaStream_t st);
 cudaError_t launch_fill_u32(uint32_t* p, uint32_t v, size_t n, cudaStream_t st);

@@ -22,7 +22,7 @@ namespace kmb {
 
 namespace {
 
-constexpr int kMbRows = 128;   // rows per CTA of the inertia kernel (= threads)
+constexpr int kMbRows = kStagedRows;   // rows per CTA of the inertia kernel (= threads)
 
 inline unsigned cdiv(size_t a, size_t b) { return static_cast<unsigned>((a + b - 1) / b); }
 
@@ -62,34 +62,11 @@ mb_inertia_kernel(const float* __restrict__ X, const uint32_t* __restrict__ rows
   const float* c = C + static_cast<size_t>(live ? a : 0) * D;
   s_row[t] = i < n ? rows[i] : 0u;
   __syncthreads();
-  Kahan k;
-  for (int f0 = 0; f0 < D; f0 += 32) {
-    const int fl = min(32, D - f0);
-#pragma unroll 8
-    for (int rr = 0; rr < 32; rr++) {
-      const int r = warp + 4 * rr;
-      tile[r * 33 + lane] = (row0 + r < n && lane < fl) ? X[static_cast<size_t>(s_row[r]) * D + f0 + lane] : 0.f;
-    }
-    __syncthreads();
-    if (live) {
-      const float* xs = tile + t * 33;
-      if (VEC4 && fl == 32) {
-#pragma unroll
-        for (int q = 0; q < 8; q++) {
-          const float4 cv = __ldg(reinterpret_cast<const float4*>(c + f0) + q);
-          k.sqdiff(xs[4 * q], cv.x); k.sqdiff(xs[4 * q + 1], cv.y);
-          k.sqdiff(xs[4 * q + 2], cv.z); k.sqdiff(xs[4 * q + 3], cv.w);
-        }
-      } else {
-        for (int f = 0; f < fl; f++) k.sqdiff(xs[f], __ldg(c + f0 + f));
-      }
-    }
-    __syncthreads();
-  }
+  const float sum = staged_own_sum<VEC4, 0>(X, s_row, row0, n, D, c, live, tile);
   double m = 0.0;
   if (i < n) {
     keys[i] = a;
-    if (live) m = static_cast<double>(w ? w[s_row[t]] : 1.f) * static_cast<double>(k.sum);
+    if (live) m = static_cast<double>(w ? w[s_row[t]] : 1.f) * static_cast<double>(sum);
   }
   for (int o = 16; o > 0; o >>= 1) m += __shfl_down_sync(0xffffffffu, m, o);
   if (lane == 0) s_part[warp] = m;

@@ -164,14 +164,20 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
   int adflag = 0;
   float tolerance = .01f, yinyang_t = .1f;
   PyObject *samples_obj, *init_obj = Py_None, *metric_obj = Py_None, *weight_obj = Py_None, *batch_obj = Py_None;
-  PyObject* steps_obj = nullptr;
+  PyObject *steps_obj = nullptr, *relocate_obj = Py_False;
   static const char* kwlist[] = {"samples", "clusters", "tolerance", "init", "yinyang_t", "metric",
                                  "average_distance", "seed", "device", "verbosity", "sample_weight", "batch_size",
-                                 "max_steps", nullptr};
-  if (!PyArg_ParseTupleAndKeywords(args, kwargs, "OI|fOfOpIIiOOO", const_cast<char**>(kwlist), &samples_obj,
+                                 "max_steps", "relocate_empty_clusters", nullptr};
+  if (!PyArg_ParseTupleAndKeywords(args, kwargs, "OI|fOfOpIIiOOOO", const_cast<char**>(kwlist), &samples_obj,
                                    &clusters, &tolerance, &init_obj, &yinyang_t, &metric_obj, &adflag, &seed,
-                                   &device, &verbosity, &weight_obj, &batch_obj, &steps_obj))
+                                   &device, &verbosity, &weight_obj, &batch_obj, &steps_obj, &relocate_obj))
     return nullptr;
+  // relocation of empty clusters (kmcuda_b200.h, kmcuda_b200_kmeans_relocate): a bool, not with mini-batch
+  if (!(PyBool_Check(relocate_obj) || PyArray_IsScalar(relocate_obj, Bool))) {
+    PyErr_SetString(PyExc_TypeError, "\"relocate_empty_clusters\" must be a bool");
+    return nullptr;
+  }
+  const bool relocate = PyObject_IsTrue(relocate_obj) == 1;
   // mini-batch k-means (kmcuda_b200.h): batch_size an integer >= 1, max_steps an integer >= 0
   uint32_t batch_size = 0, max_steps = 0;
   auto take_count = [](PyObject* o, const char* name, unsigned long lo, uint32_t* out) {
@@ -193,6 +199,11 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
   if (steps_obj && !take_count(steps_obj, "max_steps", 0, &max_steps)) return nullptr;
   if (max_steps && !batch_size) {
     PyErr_SetString(PyExc_ValueError, "\"max_steps\" applies to mini-batch runs only: pass \"batch_size\" too");
+    return nullptr;
+  }
+  if (relocate && batch_obj != Py_None) {
+    PyErr_SetString(PyExc_ValueError, "\"relocate_empty_clusters\" applies to Lloyd / Yinyang runs: mini-batch "
+                                      "k-means (\"batch_size\") reassigns its clusters itself");
     return nullptr;
   }
   KMCUDAInitMethod init = kmcudaInitMethodPlusPlus;
@@ -348,6 +359,10 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
     result = kmcuda_b200_kmeans_minibatch(init, &afkmc2_m, tolerance, metric, n, static_cast<uint16_t>(d), clusters,
                                           seed, device, device_ptrs, fp16x2, verbosity, samples, weights, batch_size,
                                           max_steps, centroids, assignments, adflag ? &average_distance : nullptr);
+  else if (relocate)
+    result = kmcuda_b200_kmeans_relocate(init, &afkmc2_m, tolerance, yinyang_t, metric, n, static_cast<uint16_t>(d),
+                                         clusters, seed, device, device_ptrs, fp16x2, verbosity, samples, weights,
+                                         centroids, assignments, adflag ? &average_distance : nullptr);
   else if (weights)
     result = kmcuda_b200_kmeans_weighted(init, &afkmc2_m, tolerance, yinyang_t, metric, n, static_cast<uint16_t>(d),
                                          clusters, seed, device, device_ptrs, fp16x2, verbosity, samples, weights,
@@ -481,7 +496,7 @@ PyObject* py_knn_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
 char module_doc[] = "K-means and K-nn on NVIDIA H100 (drop-in for src-d/kmcuda's libKMCUDA).";
 char kmeans_doc[] = "kmeans_cuda(samples, clusters, tolerance=.01, init=\"k-means++\", yinyang_t=.1, metric=\"L2\", "
                     "average_distance=False, seed=time(), device=0, verbosity=0, sample_weight=None, batch_size=None, "
-                    "max_steps=0) -> "
+                    "max_steps=0, relocate_empty_clusters=False) -> "
                     "(centroids, assignments[, avg])";
 char knn_doc[] = "knn_cuda(k, samples, centroids, assignments, metric=\"L2\", device=0, verbosity=0) -> neighbors";
 
