@@ -117,6 +117,14 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
       return kmcudaInvalidArguments;
     }
   }
+  {
+    // strict mode's update keeps a [D][32] centroid tile in shared memory: wider samples would fail after the setup
+    const char* su = getenv("KMCUDA_B200_STRICT_UPDATE");
+    if (su && su[0] == '1' && static_cast<uint64_t>(features_size) * (fp16x2 ? 2 : 1) > kStrictMaxD) {
+      KMB_INFO("KMCUDA_B200_STRICT_UPDATE=1 takes at most %d features\n", kStrictMaxD);
+      return kmcudaInvalidArguments;
+    }
+  }
   KMB_INFO("reassignments threshold: %" PRIu32 "\n", static_cast<uint32_t>(tolerance * samples_size));
   const uint32_t yy_groups_size = static_cast<uint32_t>(yinyang_t * clusters_size);
   KMB_DEBUG("yinyang groups: %" PRIu32 "\n", yy_groups_size);

@@ -24,6 +24,11 @@ void pool_trim();
 constexpr uint32_t kUntouched = 0xFFFFFFFEu;  // "no centroid won": leave the assignment alone
 constexpr uint32_t kOverflowRow = 0xFFFFFFFDu;  // row-list pass: this position waits for the exact list pass
 
+// The one-CTA-per-row exact kernels (exact_rows_few_kernel, yy_rows_cta_kernel) stage the sample row in shared memory
+// up to this many features (64 KB, past the 48 KB a launch gets without opting in) and read longer rows from global
+// memory, where every thread of the CTA loads the same address at each step.  The arithmetic is the same either way.
+constexpr int kRowStageMaxD = 16384;
+
 // ---- exact Lloyd assignment (all K centroids), optional row list -------------------------------
 // result[i] = argmin (strict <, ascending index), K for "insane" rows, kUntouched if nothing wins.
 // rows == nullptr: rows 0..n-1; else the n row ids in rows[] (device), results still indexed by row.
@@ -60,7 +65,9 @@ size_t update_cub_bytes(uint32_t n);
 cudaError_t launch_partial_sums(const float* X, uint32_t n, int D, uint32_t K, const uint32_t* assign,
                                 UpdateWorkspace& ws, float* sums, uint32_t* counts, cudaStream_t st,
                                 const float* w = nullptr, float* wsums = nullptr, const uint32_t* vals = nullptr);
-// strict parity mode: the reference's running-sum update replayed in sample order (simt_kernels.cu)
+// strict parity mode: the reference's running-sum update replayed in sample order (simt_kernels.cu).  Each 32-thread
+// CTA keeps its centroids as a [D][32] tile in at most 200 KB of shared memory, hence the feature limit.
+constexpr int kStrictMaxD = 200 * 1024 / (32 * sizeof(float));   // 1600
 size_t strict_update_cub_bytes(uint32_t n);
 cudaError_t launch_strict_update(int metric, const float* X, uint32_t n, int D, uint32_t K, const uint32_t* prev,
                                  const uint32_t* cur, float* C, uint32_t* ccounts, uint32_t* keys_in,

@@ -203,18 +203,22 @@ __global__ void __launch_bounds__(512)
 exact_rows_few_kernel(const float* __restrict__ X, const float* __restrict__ C,
                       const float* __restrict__ csq, int D, uint32_t K,
                       const uint32_t* __restrict__ rows, const uint32_t* __restrict__ d_nrows,
-                      uint32_t* __restrict__ result) {
-  extern __shared__ float sx[];
+                      uint32_t* __restrict__ result, int smem_d) {
+  extern __shared__ float sx[];   // [smem_d]: the row (smem_d == D), or nothing (smem_d == 0: read X directly)
   __shared__ float s_best[512];
   __shared__ uint32_t s_arg[512];
   const uint32_t nrows = *d_nrows;
   if (nrows > kFewRows) return;  // the tiled kernel takes over
   for (uint32_t e = blockIdx.x; e < nrows; e += gridDim.x) {
     const uint32_t row = rows[e];
+    const float* xs = X + static_cast<size_t>(row) * D;
     __syncthreads();
-    for (int f = threadIdx.x; f < D; f += 512) sx[f] = X[static_cast<size_t>(row) * D + f];
+    if (smem_d) {
+      for (int f = threadIdx.x; f < D; f += 512) sx[f] = xs[f];
+      xs = sx;
+    }
     __syncthreads();
-    if (sx[0] != sx[0]) {
+    if (xs[0] != xs[0]) {
       if (threadIdx.x == 0) result[row] = K;
       continue;
     }
@@ -223,7 +227,7 @@ exact_rows_few_kernel(const float* __restrict__ X, const float* __restrict__ C,
     for (uint32_t c = threadIdx.x; c < K; c += 512) {
       const float* cp = C + static_cast<size_t>(c) * D;
       Kahan k;
-      for (int f = 0; f < D; f++) k.mac(sx[f], __ldg(cp + f));
+      for (int f = 0; f < D; f++) k.mac(xs[f], __ldg(cp + f));
       float score = lloyd_score<METRIC>(k.sum, csq[c]);
       if (score < best) {
         best = score;
@@ -285,11 +289,13 @@ cudaError_t launch_assign_exact(int metric, const float* X, const float* C, cons
                                 uint32_t n, int D, uint32_t K, const uint32_t* rows,
                                 const uint32_t* d_nrows, uint32_t* result, cudaStream_t st) {
   if (d_nrows) {  // list mode: short lists go to the one-CTA-per-row kernel (decided on the device)
-    const size_t smem = sizeof(float) * D;
-    if (metric == 1) exact_rows_few_kernel<1><<<device_sms() * 4, 512, smem, st>>>(X, C, csq, D, K, rows, d_nrows, result);
-    else exact_rows_few_kernel<0><<<device_sms() * 4, 512, smem, st>>>(X, C, csq, D, K, rows, d_nrows, result);
-    cudaError_t e = cudaGetLastError();
+    const int smem_d = D <= kRowStageMaxD ? D : 0;
+    const size_t smem = sizeof(float) * smem_d;
+    auto kern = metric == 1 ? exact_rows_few_kernel<1> : exact_rows_few_kernel<0>;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
     if (e != cudaSuccess) return e;
+    kern<<<device_sms() * 4, 512, smem, st>>>(X, C, csq, D, K, rows, d_nrows, result, smem_d);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
   }
   if (metric == 1)
     return launch_exact_pass<1, 0>(X, C, csq, n, D, K, rows, d_nrows, result, 0, nullptr, nullptr,
@@ -707,7 +713,7 @@ cudaError_t launch_strict_update(int metric, const float* X, uint32_t n, int D, 
                                  uint32_t* vals_in, uint32_t* keys_out, uint32_t* vals_out, uint32_t* offsets,
                                  void* cub_tmp, size_t cub_bytes, cudaStream_t st) {
   if (n == 0) return cudaSuccess;
-  if (static_cast<size_t>(D) * 32 * sizeof(float) > 200 * 1024) return cudaErrorInvalidValue;
+  if (D > kStrictMaxD) return cudaErrorInvalidValue;   // rejected up front by kmeans_cuda
   strict_events_kernel<<<cdiv(n, 256), 256, 0, st>>>(n, K, prev, cur, keys_in, vals_in);
   int bits = 1;
   while ((1ull << bits) <= K) bits++;  // keys are in [0, K]

@@ -244,8 +244,8 @@ __global__ void __launch_bounds__(256)
 yy_rows_cta_kernel(const float* __restrict__ X, const float* __restrict__ C, int D, uint32_t K, uint32_t G,
                    const uint32_t* __restrict__ groups, const uint32_t* __restrict__ rows,
                    const uint32_t* __restrict__ d_nrows, uint32_t* __restrict__ assign, float* __restrict__ bounds,
-                   uint32_t* __restrict__ d_changed) {
-  extern __shared__ float sx[];
+                   uint32_t* __restrict__ d_changed, int smem_d) {
+  extern __shared__ float sx[];   // [smem_d]: the row (smem_d == D), or nothing (smem_d == 0: read X directly)
   __shared__ float s_d1[256], s_d2[256], s_p[256];
   __shared__ uint32_t s_c1[256];
   const uint32_t nrows = *d_nrows;
@@ -253,8 +253,12 @@ yy_rows_cta_kernel(const float* __restrict__ X, const float* __restrict__ C, int
   for (uint32_t e = blockIdx.x; e < nrows; e += gridDim.x) {
     const uint32_t row = rows[e];
     float* b = bounds + static_cast<size_t>(row) * (G + 1);
+    const float* xs = X + static_cast<size_t>(row) * D;
     __syncthreads();
-    for (int f = tid; f < D; f += 256) sx[f] = X[static_cast<size_t>(row) * D + f];
+    if (smem_d) {
+      for (int f = tid; f < D; f += 256) sx[f] = xs[f];
+      xs = sx;
+    }
     const float ub = b[0];
     const uint32_t a = assign[row];
     __syncthreads();
@@ -285,7 +289,7 @@ yy_rows_cta_kernel(const float* __restrict__ X, const float* __restrict__ C, int
       if (!(live[0] || live[1] || live[2] || live[3])) continue;
       Kahan k[4];
       for (int f = 0; f < D; f++) {
-        const float x = sx[f];
+        const float x = xs[f];
 #pragma unroll
         for (int j = 0; j < 4; j++) {
           const float cv = __ldg(cp[j] + f);
@@ -406,11 +410,14 @@ cudaError_t launch_yy_step(int metric, TcPlan* plan, const float* X, const float
       yy_local_scan_kernel<0><<<sgrid, 128, 0, st>>>(X, C, D, K, G, groups, drift, maxdrift, scan_rows, scan_n, assign,
                                                      bounds, d_changed);
   } else {
-    const size_t smem = sizeof(float) * D;
-    if (metric == 1)
-      yy_rows_cta_kernel<1><<<device_sms() * 8, 256, smem, st>>>(X, C, D, K, G, groups, scan_rows, scan_n, assign, bounds, d_changed);
-    else
-      yy_rows_cta_kernel<0><<<device_sms() * 8, 256, smem, st>>>(X, C, D, K, G, groups, scan_rows, scan_n, assign, bounds, d_changed);
+    const int smem_d = D <= kRowStageMaxD ? D : 0;
+    const size_t smem = sizeof(float) * smem_d;
+    auto kern = metric == 1 ? yy_rows_cta_kernel<1> : yy_rows_cta_kernel<0>;
+    if ((e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem))) !=
+        cudaSuccess)
+      return e;
+    kern<<<device_sms() * 8, 256, smem, st>>>(X, C, D, K, G, groups, scan_rows, scan_n, assign, bounds, d_changed,
+                                              smem_d);
   }
   return cudaGetLastError();
 }

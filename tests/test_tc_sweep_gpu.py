@@ -60,8 +60,9 @@ def sms(km):
     return torch.cuda.get_device_properties(0).multi_processor_count
 
 
-def run_pass(X, C, metric="L2", force_exact=False, assign=None):
-    """one Shard pass: (assign, prev, changed, (used_tc, rechecked, overflowed)); the pipeline status must be clean"""
+def run_pass(X, C, metric="L2", force_exact=False, assign=None, tc=True):
+    """one Shard pass: (assign, prev, changed, (used_tc, rechecked, overflowed)); the pipeline status must be clean.
+    tc: whether the shape is one the tensor-core route takes (checked unless force_exact)"""
     import torch
     from kmcuda_b200.shard import Shard
     old = os.environ.get("KMCUDA_B200_FORCE_EXACT")
@@ -85,7 +86,7 @@ def run_pass(X, C, metric="L2", force_exact=False, assign=None):
     sh.close()
     assert err == 0, "pipeline error 0x%x" % err
     if not force_exact:
-        assert info[0], "tensor-core path not taken"
+        assert info[0] == tc, "tensor-core path taken: %s, expected %s" % (info[0], tc)
     return (a.cpu().numpy().astype(np.uint32), prev.cpu().numpy().astype(np.uint32), int(ch.item()), info)
 
 
