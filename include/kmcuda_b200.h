@@ -41,6 +41,22 @@ typedef struct kmcuda_b200_shard kmcuda_b200_shard;
  * random init's walk from srand(seed) fills the rest.  Verbosity >= 1 logs one "k-means|| round" line per round. */
 #define kmcudaInitMethodKMeansParallel ((KMCUDAInitMethod)4)
 
+/* Extra KMCUDAInitMethod value accepted by kmeans_cuda(), kmcuda_b200_kmeans_weighted(), _relocate() and _minibatch():
+ * greedy k-means++, scikit-learn's k-means++ seeding (sklearn.cluster._kmeans._kmeans_plusplus).  init_params ->
+ * uint32_t trials L per round (NULL or 0 = 2 + floor(ln K), scikit-learn's default; 1 = plain d^2 k-means++; above 32
+ * is kmcudaInvalidArguments).  c0 is k-means++'s first centroid (srand(seed), rand() % N, redrawn on NaN / zero-weight
+ * rows) and d the true distance to it; the mass of a row is m = w d^2 (0 when d is not finite, on rows whose first
+ * feature is NaN, on zero-weight rows and on rows already chosen).  Each round r = 1 .. K - 1 draws L trial rows with
+ * replacement proportionally to m: trial t is the row of the smallest -ln(u) / m, u a counter hash of (seed, r, t,
+ * row), so the trials are the same on any number of GPUs.  The trial whose row lowers the potential sum(m) most (the
+ * lowest t on equal potentials, each summed in double in a fixed order) becomes centroid r and d = min(d, distance to
+ * it).  When the potential reaches 0 (fewer distinct rows than K), random init's walk from srand(seed) fills the rest
+ * with rows not chosen yet.  With every weight 1 the result is bit-identical to the unweighted call.  Verbosity >= 1
+ * logs the trial count and the final potential, >= 2 one "greedy k-means++ round" line per round.  With several GPUs
+ * the potentials are added in device order, so a pick can differ from one GPU's only where two trials' potentials lie
+ * within that rounding. */
+#define kmcudaInitMethodGreedyPlusPlus ((KMCUDAInitMethod)5)
+
 /* kmeans_cuda() with a weight per sample (scikit-learn's sample_weight).  The parameters are those of kmeans_cuda(),
  * plus `weights`: [samples_size] fp32, a host pointer when device_ptrs < 0 and device memory on device `device_ptrs`
  * otherwise (the rule for `samples`; fp32 in fp16x2 mode too).  weights == NULL is the unweighted run.

@@ -59,11 +59,14 @@ SUCCESS, INVALID_ARGUMENTS, NO_SUCH_DEVICE, MEMORY_ALLOCATION_FAILURE, RUNTIME_E
 INIT_RANDOM, INIT_PLUSPLUS, INIT_AFKMC2, INIT_IMPORT = range(4)
 INIT_KMEANS_PARALLEL = 4   # include/kmcuda_b200.h: kmcudaInitMethodKMeansParallel
 KMEANS_PARALLEL_MAX_ROUNDS = 32
+INIT_GREEDY_PLUSPLUS = 5   # include/kmcuda_b200.h: kmcudaInitMethodGreedyPlusPlus
+GREEDY_PLUSPLUS_MAX_TRIALS = 32
 METRIC_L2, METRIC_COSINE = range(2)
 
 _INIT_METHODS = {"kmeans++": INIT_PLUSPLUS, "k-means++": INIT_PLUSPLUS, "afkmc2": INIT_AFKMC2,
                  "afk-mc2": INIT_AFKMC2, "random": INIT_RANDOM, "k-means||": INIT_KMEANS_PARALLEL,
-                 "kmeans||": INIT_KMEANS_PARALLEL}
+                 "kmeans||": INIT_KMEANS_PARALLEL, "greedy-k-means++": INIT_GREEDY_PLUSPLUS,
+                 "greedy-kmeans++": INIT_GREEDY_PLUSPLUS}
 _METRICS = {"euclidean": METRIC_L2, "L2": METRIC_L2, "l2": METRIC_L2, "cos": METRIC_COSINE,
             "cosine": METRIC_COSINE, "angular": METRIC_COSINE}
 
@@ -132,6 +135,15 @@ def _kmeans_parallel_rounds(rounds):
     if not 0 <= rounds <= KMEANS_PARALLEL_MAX_ROUNDS:
         raise ValueError("k-means|| rounds must be in [0, %d], got %d" % (KMEANS_PARALLEL_MAX_ROUNDS, rounds))
     return int(rounds)
+
+
+def _greedy_plusplus_trials(trials):
+    """the trials per round of init=("greedy-k-means++", trials): an integer in [0, 32], 0 = 2 + floor(ln K)"""
+    if isinstance(trials, bool) or not isinstance(trials, (int, np.integer)):
+        raise ValueError("greedy k-means++ trials must be an integer, got %r" % (trials,))
+    if not 0 <= trials <= GREEDY_PLUSPLUS_MAX_TRIALS:
+        raise ValueError("greedy k-means++ trials must be in [0, %d], got %d" % (GREEDY_PLUSPLUS_MAX_TRIALS, trials))
+    return int(trials)
 
 
 def _count(value, name, lowest):
@@ -207,6 +219,8 @@ def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1
             afkmc2_m = ctypes.c_uint32(int(init[1]))
         if len(init) > 1 and init_method == INIT_KMEANS_PARALLEL:
             afkmc2_m = ctypes.c_uint32(_kmeans_parallel_rounds(init[1]))
+        if len(init) > 1 and init_method == INIT_GREEDY_PLUSPLUS:
+            afkmc2_m = ctypes.c_uint32(_greedy_plusplus_trials(init[1]))
     else:
         init_method = INIT_IMPORT
     metric_id = _get_metric(metric)

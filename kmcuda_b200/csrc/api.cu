@@ -91,6 +91,9 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
   if (init == kmcudaInitMethodKMeansParallel && init_params &&
       *static_cast<const uint32_t*>(init_params) > kKMeansParallelMaxRounds)
     return kmcudaInvalidArguments;
+  if (init == kmcudaInitMethodGreedyPlusPlus && init_params &&
+      *static_cast<const uint32_t*>(init_params) > kGreedyPlusPlusMaxTrials)
+    return kmcudaInvalidArguments;
   if (minibatch) {
     // one GPU, L2, a real batch; strict mode replays a Lloyd update that mini-batch steps do not have
     const char* su = getenv("KMCUDA_B200_STRICT_UPDATE");

@@ -25,6 +25,7 @@ static const float kYinyangDraftReassignments = 0.11f;  // reference kmeans.cu:2
 static const float kYinyangRefreshEpsilon = 1e-4f;      // reference kmeans.cu:29
 static const uint32_t kKMeansParallelRounds = 5;        // k-means|| rounds when init_params gives none
 static const uint32_t kKMeansParallelMaxRounds = 32;    // the round number is 8 bits of the draw hash's key
+static const uint32_t kGreedyPlusPlusMaxTrials = 32;    // greedy k-means++ trials per round (kGppMaxTrials)
 
 // Device teardown (transfer.cu).  A buffer goes back to the pool only after its stream has been synchronised
 // (kernels.h), also when a call returns early on an error while work is still queued: the owner of several devices
@@ -176,6 +177,7 @@ class Job {
   KMCUDAResult init_plusplus();
   KMCUDAResult init_afkmc2(uint32_t m, uint32_t seed);
   KMCUDAResult init_kmeans_parallel(uint32_t rounds, uint32_t seed);
+  KMCUDAResult init_greedy_plusplus(uint32_t trials, uint32_t seed);
   KMCUDAResult assign_pass(uint32_t* changed);
   KMCUDAResult update(int iter);
   KMCUDAResult relocate(int iter);

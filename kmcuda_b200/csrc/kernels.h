@@ -171,7 +171,39 @@ cudaError_t launch_kmp_weights(const uint32_t* nearest, const float* w, uint32_t
 // from each other and from the k-means|| draws (whose first-level inputs stay below 2^40)
 constexpr uint64_t kMbTagBatch = 0x6D696E6962617463ull;      // "minibatc"
 constexpr uint64_t kMbTagReassign = 0x7265617373696721ull;   // "reassig!"
+constexpr uint64_t kGppTagTrial = 0x677265656479212Bull;     // "greedy!+": the trial draws of greedy k-means++
 uint64_t mb_step_key(uint32_t seed, uint64_t step, uint64_t tag);
+
+// ---- greedy k-means++ seeding (greedy_plusplus.cu) ------------------------------------------------------------------
+constexpr uint32_t kGppMaxTrials = 32;
+// Round state on the device: the trial whose d' column the next draw folds into d (UINT32_MAX: none), the global row
+// whose d the next draw sets to 0 (UINT32_MAX: none), and stop = 1 once no row has mass left (one GPU).
+struct GppCtl {
+  uint32_t winner, chosen, stop, pad;
+};
+// the draw key of round `round`: trial t of row i draws u = ((mix(mix(key + t) ^ i) >> 11) + 0.5) 2^-53
+uint64_t gpp_round_key(uint32_t seed, uint32_t round);
+uint32_t gpp_draw_blocks(uint32_t n);    // bkey / brow hold L * gpp_draw_blocks(n) entries
+uint32_t gpp_trial_blocks(uint32_t n);   // bsum holds L * gpp_trial_blocks(n) partials
+// fold + draw: d = winner's d' column (or d), d[chosen] = 0, then keys[t] / rows[t] = the minimum (-ln u / w d^2, global
+// row) of trial t over the shard (INFINITY / UINT32_MAX when no row has mass).  single: ctl_w->stop = 1 in that case.
+// `ctl` and `ctl_w` are the same buffer (read-only in the draw kernel)
+cudaError_t launch_gpp_draw(float* dists, const float* dprime, const float* w, uint32_t n, uint32_t off, uint32_t L,
+                            const GppCtl* ctl, uint64_t rkey, double* bkey, uint32_t* brow, double* keys,
+                            uint32_t* rows, GppCtl* ctl_w, bool single, cudaStream_t st);
+// T[t][:] = X[rows[t] - off][:] (the trial rows live on this shard: one GPU)
+cudaError_t launch_gpp_gather(const float* X, uint32_t off, int D, const uint32_t* rows, uint32_t L, const GppCtl* ctl,
+                              float* T, cudaStream_t st);
+// dprime[t][i] = min(d_i, true distance of row i to T[t]) (0 on trial_rows[t], d on NaN rows), bsum[t][b] = block
+// partials of sum w d'^2
+cudaError_t launch_gpp_trial(int metric, const float* X, uint32_t n, uint32_t off, int D, const float* T, uint32_t L,
+                             const uint32_t* trial_rows, const float* dists, const float* w, const GppCtl* ctl,
+                             float* dprime, double* bsum, cudaStream_t st);
+// phis[t] = the partials of trial t folded in a fixed order; pick: the argmin goes to ctl, *row_log, *phi_log and its
+// row to crow[D] (one GPU)
+cudaError_t launch_gpp_pick(const double* bsum, uint32_t n, uint32_t L, GppCtl* ctl, const uint32_t* trial_rows,
+                            double* phis, bool pick, const float* X, uint32_t off, int D, float* crow,
+                            uint32_t* row_log, double* phi_log, cudaStream_t st);
 // rows[j] = floor(u(key, j) * N), j < b
 cudaError_t launch_mb_draw(uint32_t N, uint32_t b, uint64_t key, uint32_t* rows, cudaStream_t st);
 // bsum[mb_blocks(n)] = block partials of sum w_j * (Kahan sum of (X[rows[j]] - C[a_j])^2), a_j = result[j],

@@ -213,6 +213,10 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
       init = kmcudaInitMethodKMeansParallel;
       return true;
     }
+    if (s && (strcmp(s, "greedy-k-means++") == 0 || strcmp(s, "greedy-kmeans++") == 0)) {   // kmcuda_b200.h too
+      init = kmcudaInitMethodGreedyPlusPlus;
+      return true;
+    }
     auto it = s ? kmcuda::init_methods.find(s) : kmcuda::init_methods.end();
     if (it == kmcuda::init_methods.end()) {
       PyErr_SetString(PyExc_ValueError, "Unknown centroids initialization method. Supported values are "
@@ -235,7 +239,9 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
     if (!named_init(first)) return nullptr;
     if (PyTuple_Size(init_obj) > 1 && init == kmcudaInitMethodAFKMC2)
       afkmc2_m = static_cast<uint32_t>(PyLong_AsUnsignedLong(PyTuple_GetItem(init_obj, 1)));
-    if (PyTuple_Size(init_obj) > 1 && init == kmcudaInitMethodKMeansParallel) {   // rounds: an integer in [0, 32]
+    const bool greedy = init == kmcudaInitMethodGreedyPlusPlus;
+    if (PyTuple_Size(init_obj) > 1 && (init == kmcudaInitMethodKMeansParallel || greedy)) {
+      // k-means|| rounds or greedy k-means++ trials: an integer in [0, 32]
       PyObject* r = PyTuple_GetItem(init_obj, 1);
       long v = -1;
       if (PyLong_Check(r) && !PyBool_Check(r)) {
@@ -247,7 +253,8 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
       }
       if (v < 0 || v > 32) {
         PyErr_Clear();
-        PyErr_SetString(PyExc_ValueError, "k-means|| rounds must be an integer in [0, 32]");
+        PyErr_SetString(PyExc_ValueError, greedy ? "greedy k-means++ trials must be an integer in [0, 32]"
+                                                 : "k-means|| rounds must be an integer in [0, 32]");
         return nullptr;
       }
       afkmc2_m = static_cast<uint32_t>(v);
