@@ -115,6 +115,32 @@ KMCUDAResult kmcuda_b200_kmeans_minibatch(KMCUDAInitMethod init, const void *ini
                                           const float *weights, uint32_t batch_size, uint32_t max_steps,
                                           float *centroids, uint32_t *assignments, float *average_distance);
 
+/* k-means restarts, scikit-learn's KMeans(n_init=...): n_init seedings and runs over one ingest of the samples, keeping
+ * the run of lowest inertia.  The parameters up to `weights` are those of kmcuda_b200_kmeans_relocate(); restart r
+ * (r = 0 .. n_init - 1) is exactly what one kmcuda_b200_kmeans_relocate() call (relocate_empty_clusters != 0) or one
+ * kmcuda_b200_kmeans_weighted() call (relocate_empty_clusters == 0) runs with seed_r = seed + r * 0x9E3779B9 (mod 2^32):
+ * the seeding, then the Lloyd or Yinyang run.  The samples are ingested and the weights checked once per call.
+ * The inertia of a run is sum_i w_i e_i over all rows (w_i = 1 without weights): L2 e_i = the Kahan sum of squared
+ * differences to the row's centroid, angular e_i = the angle to it, squared; a row without a centroid or with a
+ * non-finite e_i adds 0.  Each device adds its block partials in double in a fixed order, the host adds the devices in
+ * device order.  Restart 0 is the first best; a later restart replaces it only with a strictly lower inertia (ties keep
+ * the earlier one, NaN never wins), so with several GPUs the pick can differ from one GPU's only where two inertias lie
+ * within the rounding of that sum.  The outputs are the kept restart's centroids and assignments; average_distance (if
+ * not NULL) is computed on that restart, and *inertia (if not NULL) is its inertia against the fp32 centroids (before
+ * any fp16x2 narrowing of the copy-out).  With n_init == 1 the centroids, assignments, average distance and log are
+ * bit-identical to the corresponding kmcuda_b200_kmeans_relocate() / _weighted() / kmeans_cuda() call; only *inertia
+ * is added.  kmcudaInvalidArguments: n_init == 0, or n_init > 1 with kmcudaInitMethodImport (every restart would be the
+ * same run).  Verbosity >= 1 with n_init > 1 logs each restart's own lines in turn, "restart r/n_init: seed s, inertia
+ * %.17g" after restart r, and "restarts: kept restart r, inertia %.17g" at the end. */
+KMCUDAResult kmcuda_b200_kmeans_restarts(KMCUDAInitMethod init, const void *init_params, float tolerance,
+                                         float yinyang_t, KMCUDADistanceMetric metric, uint32_t samples_size,
+                                         uint16_t features_size, uint32_t clusters_size, uint32_t seed,
+                                         uint32_t device, int32_t device_ptrs, int32_t fp16x2, int32_t verbosity,
+                                         const float *samples, const float *weights /* NULL = unweighted */,
+                                         int32_t relocate_empty_clusters, uint32_t n_init,
+                                         float *centroids, uint32_t *assignments, float *average_distance,
+                                         double *inertia /* NULL = not wanted */);
+
 /* Creates the per-shard workspace (fp16 centroid table, TMA descriptors, re-check queues, sort
  * buffers) for up to max_samples samples of features_size fp32 features and clusters_size clusters. */
 KMCUDAResult kmcuda_b200_shard_create(kmcuda_b200_shard **shard, KMCUDADistanceMetric metric,

@@ -6,7 +6,8 @@ Python surface = the reference's `libKMCUDA` module (reference src/python.cc:33-
                 average_distance=False, seed=time(), device=0, verbosity=0,   # python.cc:159-410
                 sample_weight=None,                                           # extension: per-sample weights
                 batch_size=None, max_steps=0,                                 # extension: mini-batch k-means
-                relocate_empty_clusters=False)                                # extension: scikit-learn's relocation
+                relocate_empty_clusters=False,                                # extension: scikit-learn's relocation
+                n_init=1, inertia=False)                                      # extension: restarts, inertia
                 init="k-means||" / ("k-means||", rounds)                      # extension: k-means|| seeding
     knn_cuda(k, samples, centroids, assignments, metric="L2", device=0, verbosity=0)  # python.cc:412-632
     supports_fp16                                                             # python.cc:52
@@ -46,6 +47,9 @@ _lib.kmcuda_b200_kmeans_relocate.argtypes = _lib.kmcuda_b200_kmeans_weighted.arg
 _lib.kmcuda_b200_kmeans_minibatch.restype = ctypes.c_int
 _lib.kmcuda_b200_kmeans_minibatch.argtypes = _lib.kmeans_cuda.argtypes[:3] + _lib.kmeans_cuda.argtypes[4:14] + \
     [ctypes.c_void_p, ctypes.c_uint32, ctypes.c_uint32] + _lib.kmeans_cuda.argtypes[14:]
+_lib.kmcuda_b200_kmeans_restarts.restype = ctypes.c_int
+_lib.kmcuda_b200_kmeans_restarts.argtypes = _lib.kmeans_cuda.argtypes[:14] + \
+    [ctypes.c_void_p, ctypes.c_int32, ctypes.c_uint32] + _lib.kmeans_cuda.argtypes[14:] + [ctypes.c_void_p]
 _lib.knn_cuda.restype = ctypes.c_int
 _lib.knn_cuda.argtypes = [
     ctypes.c_uint16, ctypes.c_int, ctypes.c_uint32, ctypes.c_uint16, ctypes.c_uint32, ctypes.c_uint32,
@@ -173,8 +177,8 @@ def _raise_for(result, fn):
 
 def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1, metric="L2",
                 average_distance=False, seed=None, device=0, verbosity=0, sample_weight=None, batch_size=None,
-                max_steps=0, relocate_empty_clusters=False):
-    """K-means on the GPU(s); see the module docstring.  Returns (centroids, assignments[, avg_distance]).
+                max_steps=0, relocate_empty_clusters=False, n_init=1, inertia=False):
+    """K-means on the GPU(s); see the module docstring.  Returns (centroids, assignments[, avg_distance][, inertia]).
 
     sample_weight: one non-negative weight per sample (include/kmcuda_b200.h, kmcuda_b200_kmeans_weighted), a 1-D
     array-like of length N, or an int device pointer when `samples` is the device-pointer tuple; None = unweighted.
@@ -185,13 +189,28 @@ def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1
 
     relocate_empty_clusters: True moves every cluster that ends an update without members to one of the samples
     farthest from their centroids (kmcuda_b200_kmeans_relocate, scikit-learn's KMeans rule) instead of leaving a NaN
-    centroid; not with batch_size (mini-batch has its own reassignment)."""
+    centroid; not with batch_size (mini-batch has its own reassignment).
+
+    n_init: an int >= 1, the number of restarts (kmcuda_b200_kmeans_restarts, scikit-learn's KMeans n_init): restart r
+    seeds with (seed + r * 0x9E3779B9) mod 2^32 and runs Lloyd / Yinyang as a fresh call would, on one ingest of the
+    samples; the run of lowest inertia is returned (ties keep the earlier restart).  Not with an ndarray init (every
+    restart would be the same run) nor with batch_size.
+
+    inertia: True appends the returned run's inertia, sum w * ||x - c||^2 (angular: w * angle^2) as a float, to the
+    result; not with batch_size."""
     if not isinstance(relocate_empty_clusters, (bool, np.bool_)):
         raise TypeError("\"relocate_empty_clusters\" must be a bool, got %r" % (relocate_empty_clusters,))
     relocate_empty_clusters = bool(relocate_empty_clusters)
     if relocate_empty_clusters and batch_size is not None:
         raise ValueError("\"relocate_empty_clusters\" applies to Lloyd / Yinyang runs: mini-batch k-means "
                          "(\"batch_size\") reassigns its clusters itself")
+    n_init = _count(n_init, "n_init", 1)
+    if not isinstance(inertia, (bool, np.bool_)):
+        raise TypeError("\"inertia\" must be a bool, got %r" % (inertia,))
+    inertia = bool(inertia)
+    if (n_init != 1 or inertia) and batch_size is not None:
+        raise ValueError("\"n_init\" and \"inertia\" apply to Lloyd / Yinyang runs, not to mini-batch k-means "
+                         "(\"batch_size\")")
     clusters = int(clusters)
     if batch_size is not None:
         batch_size = _count(batch_size, "batch_size", 1)
@@ -223,6 +242,8 @@ def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1
             afkmc2_m = ctypes.c_uint32(_greedy_plusplus_trials(init[1]))
     else:
         init_method = INIT_IMPORT
+    if init_method == INIT_IMPORT and n_init > 1:
+        raise ValueError("\"n_init\" > 1 needs a seeding method: with imported centroids every restart is the same run")
     metric_id = _get_metric(metric)
     if clusters < 2 or clusters >= 0xFFFFFFFF:
         raise ValueError("\"clusters\" must be greater than 1 and less than (1 << 32) - 1")
@@ -277,10 +298,14 @@ def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1
         else:
             _cuda_memcpy_h2d(device_ptrs, centroids_ptr, imp.ctypes.data, clusters * d * 4)
     avg = ctypes.c_float(0)
+    inertia_value = ctypes.c_double(0)
     common = (init_method, ctypes.byref(afkmc2_m), tolerance, yinyang_t, metric_id, n, d, clusters,
               int(seed) & 0xFFFFFFFF, int(device), device_ptrs, int(fp16x2), int(verbosity), samples_ptr)
     outputs = (centroids_ptr, assignments_ptr, ctypes.byref(avg) if average_distance else None)
-    if batch_size is not None:
+    if n_init != 1 or inertia:
+        result = _lib.kmcuda_b200_kmeans_restarts(*common, weights_ptr, int(relocate_empty_clusters), n_init, *outputs,
+                                                  ctypes.byref(inertia_value) if inertia else None)
+    elif batch_size is not None:
         if yinyang_t and verbosity > 0:
             print("mini-batch k-means: yinyang_t is ignored", flush=True)
         result = _lib.kmcuda_b200_kmeans_minibatch(*common[:3], *common[4:], weights_ptr, batch_size, max_steps,
@@ -293,9 +318,12 @@ def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1
         result = _lib.kmcuda_b200_kmeans_weighted(*common, weights_ptr, *outputs)
     del owned, keep_w
     _raise_for(result, "kmeans_cuda")
-    if device_ptrs < 0:
-        return (centroids, assignments, avg.value) if average_distance else (centroids, assignments)
-    return (centroids_ptr, assignments_ptr, avg.value) if average_distance else (centroids_ptr, assignments_ptr)
+    out = (centroids, assignments) if device_ptrs < 0 else (centroids_ptr, assignments_ptr)
+    if average_distance:
+        out += (avg.value,)
+    if inertia:
+        out += (inertia_value.value,)
+    return out
 
 
 def knn_cuda(k, samples, centroids, assignments, metric="L2", device=0, verbosity=0):

@@ -63,14 +63,15 @@ static KMCUDAResult print_memory_stats(const std::vector<int>& devs) {
 
 using namespace kmb;
 
-// kmeans_cuda, kmcuda_b200_kmeans_weighted and kmcuda_b200_kmeans_relocate (weights == nullptr: the unweighted run)
+// kmeans_cuda, kmcuda_b200_kmeans_weighted, _relocate, _minibatch and _restarts (weights == nullptr: the unweighted run)
 static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, float tolerance,
                                 float yinyang_t, KMCUDADistanceMetric metric, uint32_t samples_size,
                                 uint16_t features_size, uint32_t clusters_size, uint32_t seed,
                                 uint32_t device, int32_t device_ptrs, int32_t fp16x2, int32_t verbosity,
                                 const float* samples, const float* weights, float* centroids,
                                 uint32_t* assignments, float* average_distance, bool minibatch = false,
-                                uint32_t batch_size = 0, uint32_t max_steps = 0, bool relocate = false) {
+                                uint32_t batch_size = 0, uint32_t max_steps = 0, bool relocate = false,
+                                uint32_t n_init = 1, double* inertia = nullptr) {
   KMB_DEBUG("arguments: %d %p %.3f %.2f %d %" PRIu32 " %" PRIu16 " %" PRIu32 " %" PRIu32 " %" PRIu32
             " %d %" PRIi32 " %p %p %p %p\n", init, init_params, tolerance, yinyang_t, metric, samples_size,
             features_size, clusters_size, seed, device, fp16x2, verbosity, samples, centroids, assignments,
@@ -94,6 +95,8 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
   if (init == kmcudaInitMethodGreedyPlusPlus && init_params &&
       *static_cast<const uint32_t*>(init_params) > kGreedyPlusPlusMaxTrials)
     return kmcudaInvalidArguments;
+  // restarts: at least one run; imported centroids would make every restart the same run
+  if (n_init == 0 || (n_init > 1 && init == kmcudaInitMethodImport)) return kmcudaInvalidArguments;
   if (minibatch) {
     // one GPU, L2, a real batch; strict mode replays a Lloyd update that mini-batch steps do not have
     const char* su = getenv("KMCUDA_B200_STRICT_UPDATE");
@@ -149,10 +152,14 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
     g_prof.mark("weight check");
   }
   if (verbosity > 1) KMB_RET(print_memory_stats(dev_ids));
-  KMB_RET(job.init_centroids(init, init_params, seed, device_ptrs, fp16x2 != 0, centroids));
-  g_prof.mark("init centroids");
-  if (minibatch) KMB_RET(job.minibatch(batch_size, max_steps, tolerance, seed));
-  else KMB_RET(job.yinyang(tolerance, yy_groups_size));
+  if (minibatch) {
+    KMB_RET(job.init_centroids(init, init_params, seed, device_ptrs, fp16x2 != 0, centroids));
+    g_prof.mark("init centroids");
+    KMB_RET(job.minibatch(batch_size, max_steps, tolerance, seed));
+  } else {
+    KMB_RET(job.restarts(init, init_params, seed, n_init, device_ptrs, fp16x2 != 0, centroids, tolerance,
+                         yy_groups_size, inertia));
+  }
   if (average_distance) KMB_RET(job.average_distance(average_distance));
   g_prof.mark("average distance");
   // copy-out: centroids from the first device (identical everywhere), assignment slices from each shard
@@ -217,6 +224,18 @@ KMCUDAResult kmcuda_b200_kmeans_minibatch(KMCUDAInitMethod init, const void* ini
   return kmeans_impl(init, init_params, tolerance, 0.f, metric, samples_size, features_size, clusters_size, seed,
                      device, device_ptrs, fp16x2, verbosity, samples, weights, centroids, assignments,
                      average_distance, true, batch_size, max_steps);
+}
+
+KMCUDAResult kmcuda_b200_kmeans_restarts(KMCUDAInitMethod init, const void* init_params, float tolerance,
+                                         float yinyang_t, KMCUDADistanceMetric metric, uint32_t samples_size,
+                                         uint16_t features_size, uint32_t clusters_size, uint32_t seed,
+                                         uint32_t device, int32_t device_ptrs, int32_t fp16x2, int32_t verbosity,
+                                         const float* samples, const float* weights, int32_t relocate_empty_clusters,
+                                         uint32_t n_init, float* centroids, uint32_t* assignments,
+                                         float* average_distance, double* inertia) {
+  return kmeans_impl(init, init_params, tolerance, yinyang_t, metric, samples_size, features_size, clusters_size, seed,
+                     device, device_ptrs, fp16x2, verbosity, samples, weights, centroids, assignments,
+                     average_distance, false, 0, 0, relocate_empty_clusters != 0, n_init, inertia);
 }
 
 KMCUDAResult knn_cuda(uint16_t k, KMCUDADistanceMetric metric, uint32_t samples_size,

@@ -838,6 +838,88 @@ KMCUDAResult Job::minibatch(uint32_t batch_size, uint64_t max_steps, float toler
   return kmcudaSuccess;
 }
 
+// Restarts (DESIGN.md §4n): restart r seeds with seed + r * 0x9E3779B9 (mod 2^32) and runs exactly what a fresh call
+// with that seed runs; the samples stay ingested.  State that outlives a run in this Job is reset before each one (the
+// per-device update state is reset by lloyd()).  Restart 0 is the first best and a later one replaces it only with a
+// strictly lower inertia, so ties keep the earlier restart and NaN never wins.  The best run's centroids and
+// assignments are copied aside on the device, and back after the loop unless the last restart is the best.
+KMCUDAResult Job::restarts(KMCUDAInitMethod method, const void* init_params, uint32_t seed, uint32_t n_init,
+                           int device_ptrs, bool fp16x2, const float* user_centroids, float tolerance, uint32_t G,
+                           double* inertia_out) {
+  struct Best {
+    DevBuf<float> C;
+    DevBuf<uint32_t> assign;
+  };
+  std::vector<Best> best(n_init > 1 ? devs.size() : 0);
+  Drain drain{*this};
+  const size_t kd = static_cast<size_t>(K) * D;
+  for (size_t i = 0; i < best.size(); i++) {
+    KMB_CU(cudaSetDevice(devs[i].dev), kmcudaRuntimeError);
+    KMB_CU(best[i].C.alloc(kd), kmcudaMemoryAllocationFailure);
+    KMB_CU(best[i].assign.alloc(devs[i].len), kmcudaMemoryAllocationFailure);
+  }
+  double best_inertia = 0;
+  uint32_t best_r = 0;
+  for (uint32_t r = 0; r < n_init; r++) {
+    const uint32_t seed_r = seed + r * 0x9E3779B9u;
+    lloyd_iter_ms = 0;
+    relocated = 0;
+    KMB_RET(init_centroids(method, init_params, seed_r, device_ptrs, fp16x2, user_centroids));
+    g_prof.mark("init centroids");
+    KMB_RET(yinyang(tolerance, G));
+    if (n_init == 1 && !inertia_out) return kmcudaSuccess;
+    double e = 0;
+    KMB_RET(inertia(&e));
+    g_prof.mark("restarts: inertia");
+    if (n_init > 1) KMB_INFO("restart %" PRIu32 "/%" PRIu32 ": seed %" PRIu32 ", inertia %.17g\n", r, n_init, seed_r, e);
+    if (r > 0 && !(e < best_inertia)) continue;
+    best_inertia = e;
+    best_r = r;
+    if (r + 1 == n_init) break;   // the last restart's state is already in place
+    for (size_t i = 0; i < best.size(); i++) {
+      Dev& d = devs[i];
+      KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+      KMB_CU(cudaMemcpyAsync(best[i].C.get(), d.C.get(), sizeof(float) * kd, cudaMemcpyDeviceToDevice, d.st),
+             kmcudaMemoryCopyError);
+      KMB_CU(cudaMemcpyAsync(best[i].assign.get(), d.assign.get(), sizeof(uint32_t) * d.len, cudaMemcpyDeviceToDevice,
+                             d.st), kmcudaMemoryCopyError);
+    }
+  }
+  if (n_init > 1 && best_r + 1 != n_init) {
+    for (size_t i = 0; i < best.size(); i++) {
+      Dev& d = devs[i];
+      KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+      KMB_CU(cudaMemcpyAsync(d.C.get(), best[i].C.get(), sizeof(float) * kd, cudaMemcpyDeviceToDevice, d.st),
+             kmcudaMemoryCopyError);
+      KMB_CU(cudaMemcpyAsync(d.assign.get(), best[i].assign.get(), sizeof(uint32_t) * d.len, cudaMemcpyDeviceToDevice,
+                             d.st), kmcudaMemoryCopyError);
+    }
+  }
+  if (n_init > 1) KMB_INFO("restarts: kept restart %" PRIu32 ", inertia %.17g\n", best_r, best_inertia);
+  if (inertia_out) *inertia_out = best_inertia;
+  return kmcudaSuccess;
+}
+
+// sum of w e over every shard (launch_inertia), the device totals added in device order
+KMCUDAResult Job::inertia(double* out) {
+  std::vector<DevBuf<double>> bsum(devs.size()), total(devs.size());
+  Drain drain{*this};
+  for (size_t i = 0; i < devs.size(); i++) {
+    Dev& d = devs[i];
+    KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+    KMB_CU(bsum[i].alloc(inertia_blocks(d.len)), kmcudaMemoryAllocationFailure);
+    KMB_CU(total[i].alloc(1), kmcudaMemoryAllocationFailure);
+    KMB_CU(launch_inertia(metric, d.X, d.len, D, d.C, K, d.assign, d.w.get(), bsum[i], total[i], d.st),
+           kmcudaRuntimeError);
+  }
+  std::vector<double> parts;
+  KMB_RET(gather([&](size_t i) { return total[i].get(); }, &parts));
+  double sum = 0;
+  for (double part : parts) sum += part;
+  *out = sum;
+  return kmcudaSuccess;
+}
+
 KMCUDAResult Job::average_distance(float* out) {
   KMB_INFO("calculating the average distance...\n");
   for (auto& d : devs) {

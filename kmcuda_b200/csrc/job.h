@@ -187,6 +187,12 @@ class Job {
   KMCUDAResult minibatch(uint32_t batch_size, uint64_t max_steps, float tolerance, uint32_t seed);
   double lloyd_iter_ms = 0;   // wall time of the fastest complete Lloyd iteration of this run (assign pass + update), 0 = none yet
   KMCUDAResult group_centroids(uint32_t G, std::vector<uint32_t>* groups);
+  // n_init seedings + Lloyd / Yinyang runs, the one of lowest inertia left in C / assign (kmcuda_b200_kmeans_restarts);
+  // n_init == 1 and inertia_out == nullptr is the plain run
+  KMCUDAResult restarts(KMCUDAInitMethod method, const void* init_params, uint32_t seed, uint32_t n_init,
+                        int device_ptrs, bool fp16x2, const float* user_centroids, float tolerance, uint32_t G,
+                        double* inertia_out);
+  KMCUDAResult inertia(double* out);
   KMCUDAResult average_distance(float* out);
 };
 

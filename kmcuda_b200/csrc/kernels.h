@@ -249,6 +249,12 @@ cudaError_t launch_mb_variance(const float* X, uint32_t n, int D, double* work, 
 // (d desc, row asc); 0 when assign[i] >= K, w[i] <= 0 (w optional) or d_i is not finite
 cudaError_t launch_reloc_keys(int metric, const float* X, uint32_t n, int D, const float* C, uint32_t K,
                               const uint32_t* assign, const float* w, uint32_t off, uint64_t* keys, cudaStream_t st);
+// inertia of the shard (restarts, DESIGN.md §4n): *out = sum of w_i e_i over the rows a key of launch_reloc_keys would
+// call eligible, e = that key's d (L2) or d^2 (angular), in double; bsum holds inertia_blocks(n) block partials, folded
+// by launch_kmp_sum (a fixed order)
+uint32_t inertia_blocks(uint32_t n);
+cudaError_t launch_inertia(int metric, const float* X, uint32_t n, int D, const float* C, uint32_t K,
+                           const uint32_t* assign, const float* w, double* bsum, double* out, cudaStream_t st);
 struct RelocState {
   uint64_t prefix, thr;   // digits fixed so far; the selection threshold
   uint32_t above, done, eligible, pad;

@@ -164,13 +164,14 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
   int adflag = 0;
   float tolerance = .01f, yinyang_t = .1f;
   PyObject *samples_obj, *init_obj = Py_None, *metric_obj = Py_None, *weight_obj = Py_None, *batch_obj = Py_None;
-  PyObject *steps_obj = nullptr, *relocate_obj = Py_False;
+  PyObject *steps_obj = nullptr, *relocate_obj = Py_False, *n_init_obj = nullptr, *inertia_obj = Py_False;
   static const char* kwlist[] = {"samples", "clusters", "tolerance", "init", "yinyang_t", "metric",
                                  "average_distance", "seed", "device", "verbosity", "sample_weight", "batch_size",
-                                 "max_steps", "relocate_empty_clusters", nullptr};
-  if (!PyArg_ParseTupleAndKeywords(args, kwargs, "OI|fOfOpIIiOOOO", const_cast<char**>(kwlist), &samples_obj,
+                                 "max_steps", "relocate_empty_clusters", "n_init", "inertia", nullptr};
+  if (!PyArg_ParseTupleAndKeywords(args, kwargs, "OI|fOfOpIIiOOOOOO", const_cast<char**>(kwlist), &samples_obj,
                                    &clusters, &tolerance, &init_obj, &yinyang_t, &metric_obj, &adflag, &seed,
-                                   &device, &verbosity, &weight_obj, &batch_obj, &steps_obj, &relocate_obj))
+                                   &device, &verbosity, &weight_obj, &batch_obj, &steps_obj, &relocate_obj,
+                                   &n_init_obj, &inertia_obj))
     return nullptr;
   // relocation of empty clusters (kmcuda_b200.h, kmcuda_b200_kmeans_relocate): a bool, not with mini-batch
   if (!(PyBool_Check(relocate_obj) || PyArray_IsScalar(relocate_obj, Bool))) {
@@ -204,6 +205,19 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
   if (relocate && batch_obj != Py_None) {
     PyErr_SetString(PyExc_ValueError, "\"relocate_empty_clusters\" applies to Lloyd / Yinyang runs: mini-batch "
                                       "k-means (\"batch_size\") reassigns its clusters itself");
+    return nullptr;
+  }
+  // restarts (kmcuda_b200.h, kmcuda_b200_kmeans_restarts): n_init an integer >= 1, inertia a bool; not with mini-batch
+  uint32_t n_init = 1;
+  if (n_init_obj && !take_count(n_init_obj, "n_init", 1, &n_init)) return nullptr;
+  if (!(PyBool_Check(inertia_obj) || PyArray_IsScalar(inertia_obj, Bool))) {
+    PyErr_SetString(PyExc_TypeError, "\"inertia\" must be a bool");
+    return nullptr;
+  }
+  const bool want_inertia = PyObject_IsTrue(inertia_obj) == 1;
+  if ((n_init != 1 || want_inertia) && batch_obj != Py_None) {
+    PyErr_SetString(PyExc_ValueError, "\"n_init\" and \"inertia\" apply to Lloyd / Yinyang runs, not to mini-batch "
+                                      "k-means (\"batch_size\")");
     return nullptr;
   }
   KMCUDAInitMethod init = kmcudaInitMethodPlusPlus;
@@ -261,6 +275,11 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
     }
   } else {
     init = kmcudaInitMethodImport;
+  }
+  if (init == kmcudaInitMethodImport && n_init > 1) {
+    PyErr_SetString(PyExc_ValueError, "\"n_init\" > 1 needs a seeding method: with imported centroids every restart "
+                                      "is the same run");
+    return nullptr;
   }
   KMCUDADistanceMetric metric;
   if (!parse_metric(metric_obj, &metric)) return nullptr;
@@ -356,13 +375,19 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
     }
   }
   float average_distance = 0;
+  double inertia = 0;
   int result;
   if (batch_size && yinyang_t > 0 && verbosity > 0) {
     printf("mini-batch k-means: yinyang_t is ignored\n");
     fflush(stdout);
   }
   Py_BEGIN_ALLOW_THREADS
-  if (batch_size)
+  if (n_init != 1 || want_inertia)
+    result = kmcuda_b200_kmeans_restarts(init, &afkmc2_m, tolerance, yinyang_t, metric, n, static_cast<uint16_t>(d),
+                                         clusters, seed, device, device_ptrs, fp16x2, verbosity, samples, weights,
+                                         relocate ? 1 : 0, n_init, centroids, assignments,
+                                         adflag ? &average_distance : nullptr, want_inertia ? &inertia : nullptr);
+  else if (batch_size)
     result = kmcuda_b200_kmeans_minibatch(init, &afkmc2_m, tolerance, metric, n, static_cast<uint16_t>(d), clusters,
                                           seed, device, device_ptrs, fp16x2, verbosity, samples, weights, batch_size,
                                           max_steps, centroids, assignments, adflag ? &average_distance : nullptr);
@@ -380,6 +405,15 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
                          adflag ? &average_distance : nullptr);
   Py_END_ALLOW_THREADS
   if (result != kmcudaSuccess) return raise_for(result, "kmeans_cuda");
+  if (want_inertia) {
+    if (device_ptrs < 0) {
+      if (!adflag) return Py_BuildValue("OOd", centroids_arr.p, assignments_arr.p, inertia);
+      return Py_BuildValue("OOfd", centroids_arr.p, assignments_arr.p, average_distance, inertia);
+    }
+    const unsigned long long cp = reinterpret_cast<uintptr_t>(centroids), ap = reinterpret_cast<uintptr_t>(assignments);
+    if (!adflag) return Py_BuildValue("KKd", cp, ap, inertia);
+    return Py_BuildValue("KKfd", cp, ap, average_distance, inertia);
+  }
   if (device_ptrs < 0) {
     if (!adflag) return Py_BuildValue("OO", centroids_arr.p, assignments_arr.p);
     return Py_BuildValue("OOf", centroids_arr.p, assignments_arr.p, average_distance);
@@ -503,8 +537,8 @@ PyObject* py_knn_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
 char module_doc[] = "K-means and K-nn on NVIDIA H100 (drop-in for src-d/kmcuda's libKMCUDA).";
 char kmeans_doc[] = "kmeans_cuda(samples, clusters, tolerance=.01, init=\"k-means++\", yinyang_t=.1, metric=\"L2\", "
                     "average_distance=False, seed=time(), device=0, verbosity=0, sample_weight=None, batch_size=None, "
-                    "max_steps=0, relocate_empty_clusters=False) -> "
-                    "(centroids, assignments[, avg])";
+                    "max_steps=0, relocate_empty_clusters=False, n_init=1, inertia=False) -> "
+                    "(centroids, assignments[, avg][, inertia])";
 char knn_doc[] = "knn_cuda(k, samples, centroids, assignments, metric=\"L2\", device=0, verbosity=0) -> neighbors";
 
 PyMethodDef module_functions[] = {

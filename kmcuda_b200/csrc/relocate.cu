@@ -8,6 +8,8 @@
 //            that at most cap keys reach, cub::DeviceSelect takes those, cub::DeviceRadixSort orders them
 //   apply    in walk order: sums[donor] -= w x, counts[donor] -= 1, W[donor] -= w; sums[e] = w x, counts[e] = 1,
 //            W[e] = w; after the normalisation the angular centroid of e is overwritten with x / ||x||
+// The restarts' inertia pass (Job::restarts, DESIGN.md §4n) sums w e over the rows the keys pass would find eligible,
+// with the same staged row distance.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_select.cuh>
 
@@ -51,6 +53,44 @@ reloc_keys_kernel(const float* __restrict__ X, uint32_t n, int D, const float* _
       key = (static_cast<uint64_t>(ob) << 32) | static_cast<uint32_t>(~(off + i));
     }
     keys[i] = key;
+  }
+}
+
+// Inertia of a run (restarts, DESIGN.md §4n): the rows of reloc_keys_kernel with the same distance d, e = d (L2: the
+// Kahan sum of squared differences) or d^2 (angular: the angle); rows that would get key 0 there contribute 0.
+// bsum[block] = sum of w e over the block's rows, lanes and warps added in a fixed order.
+template <bool VEC4, int METRIC>
+__global__ void __launch_bounds__(kStagedRows)
+inertia_kernel(const float* __restrict__ X, uint32_t n, int D, const float* __restrict__ C, uint32_t K,
+               const uint32_t* __restrict__ assign, const float* __restrict__ w, double* __restrict__ bsum) {
+  __shared__ uint32_t s_row[kStagedRows];
+  __shared__ float tile[kStagedRows * 33];
+  __shared__ double s_part[kStagedRows / 32];
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const uint32_t row0 = blockIdx.x * kStagedRows, i = row0 + t;
+  uint32_t a = K;
+  float wi = 0.f;
+  if (i < n) {
+    a = min(assign[i], K);
+    wi = w ? w[i] : 1.f;
+  }
+  const bool live = a < K && wi > 0.f;
+  const float* c = C + static_cast<size_t>(live ? a : 0) * D;
+  s_row[t] = i < n ? i : 0u;
+  __syncthreads();
+  const float sum = staged_own_sum<VEC4, METRIC>(X, s_row, row0, n, D, c, live, tile);
+  double m = 0.0;
+  if (live) {
+    const float d = METRIC == 1 ? acos_clamped(sum) : sum;
+    if (isfinite(d)) m = static_cast<double>(wi) * (METRIC == 1 ? static_cast<double>(d) * d : static_cast<double>(d));
+  }
+  for (int o = 16; o > 0; o >>= 1) m += __shfl_down_sync(0xffffffffu, m, o);
+  if (lane == 0) s_part[warp] = m;
+  __syncthreads();
+  if (t == 0) {
+    double s = 0.0;
+    for (int q = 0; q < kStagedRows / 32; q++) s += s_part[q];
+    bsum[blockIdx.x] = s;
   }
 }
 
@@ -183,6 +223,24 @@ cudaError_t launch_reloc_keys(int metric, const float* X, uint32_t n, int D, con
     else reloc_keys_kernel<false, 0><<<grid, kStagedRows, 0, st>>>(X, n, D, C, K, assign, w, off, keys);
   }
   return cudaGetLastError();
+}
+
+uint32_t inertia_blocks(uint32_t n) { return std::max(1u, cdiv(n, kStagedRows)); }
+
+cudaError_t launch_inertia(int metric, const float* X, uint32_t n, int D, const float* C, uint32_t K,
+                           const uint32_t* assign, const float* w, double* bsum, double* out, cudaStream_t st) {
+  if (n == 0) return cudaMemsetAsync(out, 0, sizeof(double), st);
+  const unsigned grid = cdiv(n, kStagedRows);
+  const bool v4 = D % 4 == 0;
+  if (metric == 1) {
+    if (v4) inertia_kernel<true, 1><<<grid, kStagedRows, 0, st>>>(X, n, D, C, K, assign, w, bsum);
+    else inertia_kernel<false, 1><<<grid, kStagedRows, 0, st>>>(X, n, D, C, K, assign, w, bsum);
+  } else {
+    if (v4) inertia_kernel<true, 0><<<grid, kStagedRows, 0, st>>>(X, n, D, C, K, assign, w, bsum);
+    else inertia_kernel<false, 0><<<grid, kStagedRows, 0, st>>>(X, n, D, C, K, assign, w, bsum);
+  }
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? launch_kmp_sum(bsum, grid, out, st) : e;
 }
 
 uint32_t reloc_cap(uint32_t T) { return 2 * T + 4096; }
