@@ -83,26 +83,41 @@ __device__ __forceinline__ float distance_exact(const float* __restrict__ a,
   return finalize_distance<METRIC>(k.sum);
 }
 
-// Staged pass body of the per-row kernels that need each row's exact distance to its own centroid (mini-batch inertia,
-// relocation keys): kStagedRows rows per CTA, one thread per row, 32-feature slices of the rows staged through padded
-// shared memory (coalesced loads), the own centroid `c` read as float4 when VEC4 (D % 4 == 0).  s_row[r] is the
-// sample of CTA row r (rows row0 + r >= n are padding); tile holds kStagedRows * 33 floats.  Returns the Kahan sum of
-// (x - c)^2 (METRIC 0) or of x * c (METRIC 1) in the reference's order; meaningful only where `live`.
+// The staged pass of the per-row kernels (k-means|| update, greedy k-means++ trials, mini-batch inertia, relocation
+// keys, restart inertia): kStagedRows rows per CTA, one thread per row, 32-feature slices of the rows staged through
+// padded shared memory (coalesced loads), then every thread advances the sequential Kahan chain of its own row.
 constexpr int kStagedRows = 128;
 
-template <bool VEC4, int METRIC>
-__device__ __forceinline__ float staged_own_sum(const float* __restrict__ X, const uint32_t* s_row, uint32_t row0,
+// the sample rows row0, row0 + 1, ... of a CTA, indexed as s_row[] is
+struct RowRange {
+  uint32_t row0;
+  __device__ __forceinline__ uint32_t operator[](int r) const { return row0 + r; }
+};
+
+// tile[r * 33 + f] = feature f0 + f of sample rows[r] for the fl features of the slice, 0 past them and on the padding
+// rows (row0 + r >= n); rows is s_row[] (shared memory) or a RowRange; tile holds kStagedRows * 33 floats
+template <class Rows>
+__device__ __forceinline__ void stage_slice(const float* __restrict__ X, const Rows& rows, uint32_t row0, uint32_t n,
+                                            int D, int f0, int fl, float* tile) {
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+#pragma unroll 8
+  for (int rr = 0; rr < 32; rr++) {   // warp w stages rows w, w + 4, ...: one coalesced 128-byte segment per row
+    const int r = warp + 4 * rr;
+    tile[r * 33 + lane] = (row0 + r < n && lane < fl) ? X[static_cast<size_t>(rows[r]) * D + f0 + lane] : 0.f;
+  }
+}
+
+// The staged pass against each row's own centroid `c`, read as float4 when VEC4 (D % 4 == 0).  Returns the Kahan sum
+// of (x - c)^2 (METRIC 0) or of x * c (METRIC 1) in the reference's order; meaningful only where `live`.
+template <bool VEC4, int METRIC, class Rows>
+__device__ __forceinline__ float staged_own_sum(const float* __restrict__ X, const Rows& rows, uint32_t row0,
                                                 uint32_t n, int D, const float* __restrict__ c, bool live,
                                                 float* tile) {
-  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int t = threadIdx.x;
   Kahan k;
   for (int f0 = 0; f0 < D; f0 += 32) {
     const int fl = min(32, D - f0);
-#pragma unroll 8
-    for (int rr = 0; rr < 32; rr++) {
-      const int r = warp + 4 * rr;
-      tile[r * 33 + lane] = (row0 + r < n && lane < fl) ? X[static_cast<size_t>(s_row[r]) * D + f0 + lane] : 0.f;
-    }
+    stage_slice(X, rows, row0, n, D, f0, fl, tile);
     __syncthreads();
     if (live) {
       const float* xs = tile + t * 33;

@@ -10,39 +10,24 @@
 //   gather    the L trial rows out of X
 //   trial     the hot pass: one read of X, every row's true distance e_t to every trial row (exact.cuh's Kahan chain,
 //             bit for bit), d'_t = e_t < d ? e_t : d (0 on the trial row itself), and the per-block partials of
-//             phi_t = sum w d'_t^2 in kmp_update_kernel's order
-//   pick      one CTA: phi_t folded as kmp_sum_kernel folds, argmin t (lowest t on equal values), and the winner row
-//             appended to C
+//             phi_t = sum w d'_t^2 (block_sum)
+//   pick      one CTA: phi_t folded in a fixed order (chunk_sum, fold_chunks), argmin t (lowest t on equal values), and
+//             the winner row appended to C
 // On one GPU every step stays on the device (GppCtl carries the winner from the pick to the next draw); with several
 // GPUs the host merges the keys and the potentials between the steps.
 #include <algorithm>
 
 #include "exact.cuh"
+#include "fixed_order.cuh"
 #include "kernels.h"
 
 namespace kmb {
 
 namespace {
 
-constexpr int kGppRows = 128;          // rows per CTA of the trial pass (= threads)
+constexpr int kGppRows = kStagedRows;  // rows per CTA of the trial pass (= threads)
 constexpr int kGppDrawThreads = 256;   // rows per tile of the draw pass
 constexpr int kGppFoldGroup = 4;       // trials whose chunk sums the pick kernel holds in shared memory at once
-
-inline unsigned cdiv(size_t a, size_t b) { return static_cast<unsigned>((a + b - 1) / b); }
-
-__host__ __device__ __forceinline__ uint64_t gpp_mix(uint64_t z) {
-  z += 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
-
-// w d^2 in double; rows with a non-finite distance carry none (kmp_mass)
-__device__ __forceinline__ double gpp_mass(float d, float w) {
-  if (!isfinite(d)) return 0.0;
-  const double dd = static_cast<double>(d);
-  return static_cast<double>(w) * (dd * dd);
-}
 
 __device__ __forceinline__ bool key_less(double ka, uint32_t ra, double kb, uint32_t rb) {
   return ka < kb || (ka == kb && ra < rb);
@@ -83,16 +68,14 @@ gpp_draw_kernel(float* __restrict__ dists, const float* __restrict__ dprime, con
       float d = winner < L ? dprime[static_cast<size_t>(winner) * n + i] : dists[i];
       if (off + i == chosen) d = 0.f;
       dists[i] = d;
-      m = gpp_mass(d, w ? w[i] : 1.f);
+      m = d2_mass(d, w ? w[i] : 1.f);
     }
     if (!__any_sync(0xffffffffu, m > 0.0)) continue;
     for (uint32_t t = 0; t < L; t++) {
       double k = INFINITY;
       uint32_t r = UINT32_MAX;
       if (m > 0.0) {
-        const uint64_t h = gpp_mix(gpp_mix(rkey + t) ^ static_cast<uint64_t>(off + i));
-        const double u = (static_cast<double>(h >> 11) + 0.5) * (1.0 / 9007199254740992.0);   // (0, 1)
-        k = -log(u) / m;
+        k = -log(unit_oo(splitmix64(splitmix64(rkey + t) ^ static_cast<uint64_t>(off + i)))) / m;
         r = off + i;
       }
       warp_min_key(k, r);
@@ -165,18 +148,13 @@ gpp_trial_kernel(const float* __restrict__ X, uint32_t n, uint32_t off, int D, c
   __shared__ __align__(16) float s_t[LC * 32];
   __shared__ double s_part[kGppRows / 32];
   if (ctl->stop) return;
-  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int t = threadIdx.x;
   const uint32_t row0 = blockIdx.x * kGppRows, i = row0 + t;
   const bool live = i < n;
   Kahan k[LC];
   for (int f0 = 0; f0 < D; f0 += 32) {
     const int fl = min(32, D - f0);
-#pragma unroll 8
-    for (int rr = 0; rr < 32; rr++) {   // warp w stages rows w, w + 4, ...: one coalesced 128-byte segment per row
-      const int r = warp + 4 * rr;
-      const uint32_t row = row0 + r;
-      tile[r * 33 + lane] = (row < n && lane < fl) ? X[static_cast<size_t>(row) * D + f0 + lane] : 0.f;
-    }
+    stage_slice(X, RowRange{row0}, row0, n, D, f0, fl, tile);
     for (uint32_t e = t; e < L * 32; e += kGppRows) {
       const uint32_t q = e >> 5, f = e & 31;
       s_t[e] = static_cast<int>(f) < fl ? T[static_cast<size_t>(q) * D + f0 + f] : 0.f;
@@ -235,16 +213,10 @@ gpp_trial_kernel(const float* __restrict__ X, uint32_t n, uint32_t off, int D, c
           if (e < d) dp = e;
         }
         dprime[static_cast<size_t>(q) * n + i] = dp;
-        m = gpp_mass(dp, wi);
+        m = d2_mass(dp, wi);
       }
-      for (int o = 16; o > 0; o >>= 1) m += __shfl_down_sync(0xffffffffu, m, o);
-      if (lane == 0) s_part[warp] = m;
-      __syncthreads();
-      if (t == 0) {
-        double s = 0.0;
-        for (int p = 0; p < kGppRows / 32; p++) s += s_part[p];
-        bsum[static_cast<size_t>(q) * nb + blockIdx.x] = s;
-      }
+      const double s = block_sum<kGppRows>(m, s_part);
+      if (t == 0) bsum[static_cast<size_t>(q) * nb + blockIdx.x] = s;
       __syncthreads();
     }
   }
@@ -267,9 +239,9 @@ void gpp_trial_dispatch(const float* X, uint32_t n, uint32_t off, int D, const f
     gpp_trial_kernel<METRIC, 32><<<grid, kGppRows, 0, st>>>(X, n, off, D, T, L, trial_rows, dists, w, ctl, dprime, bsum);
 }
 
-// One CTA: phis[t] = trial t's block partials folded as kmp_sum_kernel folds them (a contiguous chunk per thread, then
-// the 1024 chunks in order).  pick: thread 0 takes the argmin t (lowest t on equal values), records it in ctl and the
-// round log, and the CTA copies the winner row into crow.
+// One CTA: phis[t] = trial t's block partials folded in a fixed order (chunk_sum, fold_chunks).  pick: thread 0 takes
+// the argmin t (lowest t on equal values), records it in ctl and the round log, and the CTA copies the winner row into
+// crow.
 __global__ void __launch_bounds__(1024)
 gpp_pick_kernel(const double* __restrict__ bsum, uint32_t nb, uint32_t L, GppCtl* __restrict__ ctl,
                 const uint32_t* __restrict__ trial_rows, double* __restrict__ phis, bool pick,
@@ -278,20 +250,11 @@ gpp_pick_kernel(const double* __restrict__ bsum, uint32_t nb, uint32_t L, GppCtl
   __shared__ double s_chunk[kGppFoldGroup][1024];
   __shared__ uint32_t s_chosen;
   if (ctl->stop) return;
-  const uint32_t per = (nb + 1023) / 1024;
-  const uint32_t lo = min(nb, threadIdx.x * per), hi = min(nb, lo + per);
   for (uint32_t t0 = 0; t0 < L; t0 += kGppFoldGroup) {
-    for (uint32_t g = 0; g < kGppFoldGroup && t0 + g < L; g++) {
-      double acc = 0.0;
-      for (uint32_t b = lo; b < hi; b++) acc += bsum[static_cast<size_t>(t0 + g) * nb + b];
-      s_chunk[g][threadIdx.x] = acc;
-    }
+    for (uint32_t g = 0; g < kGppFoldGroup && t0 + g < L; g++)
+      s_chunk[g][threadIdx.x] = chunk_sum(bsum + static_cast<size_t>(t0 + g) * nb, nb);
     __syncthreads();
-    if (threadIdx.x < kGppFoldGroup && t0 + threadIdx.x < L) {
-      double s = 0.0;
-      for (int q = 0; q < 1024; q++) s += s_chunk[threadIdx.x][q];
-      phis[t0 + threadIdx.x] = s;
-    }
+    if (threadIdx.x < kGppFoldGroup && t0 + threadIdx.x < L) phis[t0 + threadIdx.x] = fold_chunks(s_chunk[threadIdx.x]);
     __syncthreads();
   }
   if (!pick) return;

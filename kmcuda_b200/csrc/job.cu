@@ -783,7 +783,7 @@ KMCUDAResult Job::minibatch(uint32_t batch_size, uint64_t max_steps, float toler
     KMB_CU(launch_mb_draw(N, b, mb_step_key(seed, s, kMbTagBatch), rows, d.st), kmcudaRuntimeError);
     KMB_RET(bs.assign_rows(b, d.X, N, rows, cur, row_result, result, d.st));
     KMB_CU(launch_mb_inertia(d.X, rows, b, D, cur, K, result, d.w.get(), keys, bsum, d.st), kmcudaRuntimeError);
-    KMB_CU(launch_kmp_sum(bsum, nb, stats.get(), d.st), kmcudaRuntimeError);
+    KMB_CU(launch_fixed_sum(bsum, nb, stats.get(), d.st), kmcudaRuntimeError);
     // unweighted: the member counts are the weight totals (a weight of 1 per entry; all-ones weights give the same bits)
     KMB_RET(bs.partial_sums_rows(b, d.X, rows, keys, S, counts, d.st, d.w.get(), weighted ? Wb.get() : nullptr));
     KMB_CU(launch_mb_blend(cur, wcur, S, weighted ? Wb.get() : nullptr, counts, K, D, nxt, wnxt, d.st),

@@ -12,6 +12,8 @@
 
 namespace kmb {
 
+inline unsigned cdiv(size_t a, size_t b) { return static_cast<unsigned>((a + b - 1) / b); }
+
 // Device-memory cache (shard.cu).  kmeans_cuda / knn_cuda allocate their whole workspace at entry like the reference
 // (wrappers.h:16-21); GB-sized cudaMalloc / cudaFree pairs can cost a call more than its kernels, so freed blocks
 // are kept per device and handed to the next call.  Blocks are
@@ -149,8 +151,6 @@ uint32_t kmp_blocks(uint32_t n);
 cudaError_t launch_kmp_update(int metric, const float* X, uint32_t n, int D, const float* cand, uint32_t ncand,
                               const uint32_t* assign, uint32_t base, float* dists, uint32_t* nearest, const float* w,
                               double* bsum, cudaStream_t st);
-// *out = the block partials added in a fixed order
-cudaError_t launch_kmp_sum(const double* bsum, uint32_t nb, double* out, cudaStream_t st);
 // the draw of round `round`: flags[i] = u(seed, round, off + i) < ell * w_i d_i^2 / phi; idx[0 .. *d_count) = the
 // drawn local row ids, ascending.  tmp: kmp_select_bytes(n) bytes
 size_t kmp_select_bytes(uint32_t n);
@@ -251,7 +251,7 @@ cudaError_t launch_reloc_keys(int metric, const float* X, uint32_t n, int D, con
                               const uint32_t* assign, const float* w, uint32_t off, uint64_t* keys, cudaStream_t st);
 // inertia of the shard (restarts, DESIGN.md §4n): *out = sum of w_i e_i over the rows a key of launch_reloc_keys would
 // call eligible, e = that key's d (L2) or d^2 (angular), in double; bsum holds inertia_blocks(n) block partials, folded
-// by launch_kmp_sum (a fixed order)
+// by launch_fixed_sum
 uint32_t inertia_blocks(uint32_t n);
 cudaError_t launch_inertia(int metric, const float* X, uint32_t n, int D, const float* C, uint32_t K,
                            const uint32_t* assign, const float* w, double* bsum, double* out, cudaStream_t st);
@@ -290,6 +290,8 @@ cudaError_t launch_reloc_cos_overwrite(float* C, int D, const float* xs, const u
 cudaError_t launch_half_to_float(const void* src, float* dst, size_t n, cudaStream_t st);
 cudaError_t launch_float_to_half(const float* src, void* dst, size_t n, cudaStream_t st);
 cudaError_t launch_fill_u32(uint32_t* p, uint32_t v, size_t n, cudaStream_t st);
+// *out = bsum[0] + ... + bsum[nb - 1], added in an order that depends only on nb (fixed_order.cuh)
+cudaError_t launch_fixed_sum(const double* bsum, uint32_t nb, double* out, cudaStream_t st);
 
 // ---- k-NN ------------------------------------------------------------------------------------------
 // inverse assignments: inv[] = sample ids sorted by (cluster, id), off[K+1] = CSR offsets

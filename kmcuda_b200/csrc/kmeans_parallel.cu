@@ -19,29 +19,14 @@
 #include <algorithm>
 
 #include "exact.cuh"
+#include "fixed_order.cuh"
 #include "kernels.h"
 
 namespace kmb {
 
 namespace {
 
-constexpr int kKmpRows = 128;   // rows per CTA of the update kernel (= threads)
-
-inline unsigned cdiv(size_t a, size_t b) { return static_cast<unsigned>((a + b - 1) / b); }
-
-__device__ __forceinline__ uint64_t kmp_mix(uint64_t z) {
-  z += 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
-
-// the draw's mass w_i d_i^2; rows with a non-finite distance carry none
-__device__ __forceinline__ double kmp_mass(float d, float w) {
-  if (!isfinite(d)) return 0.0;
-  const double dd = static_cast<double>(d);
-  return static_cast<double>(w) * (dd * dd);
-}
+constexpr int kKmpRows = kStagedRows;   // rows per CTA of the update kernel (= threads)
 
 // FIRST: the distance to c0 (cand, one row) starts every row's running minimum, nearest = 0.  Otherwise: the true
 // distance e to the round's winner cand[assign[i]] replaces d_i when e < d_i, nearest_i = base + assign[i].
@@ -53,56 +38,24 @@ kmp_update_kernel(const float* __restrict__ X, uint32_t n, int D, const float* _
                   uint32_t* __restrict__ nearest, const float* __restrict__ w, double* __restrict__ bsum) {
   __shared__ float tile[kKmpRows * 33];
   __shared__ double s_part[kKmpRows / 32];
-  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-  const uint32_t row0 = blockIdx.x * kKmpRows, i = row0 + t;
+  const uint32_t row0 = blockIdx.x * kKmpRows, i = row0 + threadIdx.x;
   uint32_t a = 0;
   if (!FIRST && i < n) a = assign[i];
   const bool live = i < n && (FIRST || a < ncand);
   const float* c = cand + static_cast<size_t>(live ? a : 0) * D;
-  Kahan k;
-  for (int f0 = 0; f0 < D; f0 += 32) {
-    const int fl = min(32, D - f0);
-#pragma unroll 8
-    for (int rr = 0; rr < 32; rr++) {   // warp w stages rows w, w + 4, ...: one coalesced 128-byte segment per row
-      const int r = warp + 4 * rr;
-      const uint32_t row = row0 + r;
-      tile[r * 33 + lane] = (row < n && lane < fl) ? X[static_cast<size_t>(row) * D + f0 + lane] : 0.f;
-    }
-    __syncthreads();
-    if (live) {
-      const float* xs = tile + t * 33;
-      if (VEC4 && fl == 32) {
-#pragma unroll
-        for (int q = 0; q < 8; q++) {
-          const float4 cv = __ldg(reinterpret_cast<const float4*>(c + f0) + q);
-          if (METRIC == 1) {
-            k.mac(xs[4 * q], cv.x); k.mac(xs[4 * q + 1], cv.y); k.mac(xs[4 * q + 2], cv.z); k.mac(xs[4 * q + 3], cv.w);
-          } else {
-            k.sqdiff(xs[4 * q], cv.x); k.sqdiff(xs[4 * q + 1], cv.y);
-            k.sqdiff(xs[4 * q + 2], cv.z); k.sqdiff(xs[4 * q + 3], cv.w);
-          }
-        }
-      } else {
-        for (int f = 0; f < fl; f++) {
-          if (METRIC == 1) k.mac(xs[f], __ldg(c + f0 + f));
-          else k.sqdiff(xs[f], __ldg(c + f0 + f));
-        }
-      }
-    }
-    __syncthreads();
-  }
+  const float sum = staged_own_sum<VEC4, METRIC>(X, RowRange{row0}, row0, n, D, c, live, tile);
   double m = 0.0;
   if (i < n) {
     const bool nan_row = !(X[static_cast<size_t>(i) * D] == X[static_cast<size_t>(i) * D]);
     float d;
     if (FIRST) {
-      d = nan_row ? 0.f : finalize_distance<METRIC>(k.sum);
+      d = nan_row ? 0.f : finalize_distance<METRIC>(sum);
       dists[i] = d;
       nearest[i] = 0;
     } else {
       d = dists[i];
       if (live && !nan_row) {
-        const float e = finalize_distance<METRIC>(k.sum);
+        const float e = finalize_distance<METRIC>(sum);
         if (e < d) {
           d = e;
           dists[i] = e;
@@ -110,41 +63,18 @@ kmp_update_kernel(const float* __restrict__ X, uint32_t n, int D, const float* _
         }
       }
     }
-    m = kmp_mass(d, w ? w[i] : 1.f);
+    m = d2_mass(d, w ? w[i] : 1.f);
   }
-  for (int o = 16; o > 0; o >>= 1) m += __shfl_down_sync(0xffffffffu, m, o);
-  if (lane == 0) s_part[warp] = m;
-  __syncthreads();
-  if (t == 0) {
-    double s = 0.0;
-    for (int q = 0; q < kKmpRows / 32; q++) s += s_part[q];
-    bsum[blockIdx.x] = s;
-  }
-}
-
-// *out = bsum[0] + ... + bsum[nb - 1] in a fixed order (contiguous chunk per thread, then the chunks in order)
-__global__ void __launch_bounds__(1024)
-kmp_sum_kernel(const double* __restrict__ bsum, uint32_t nb, double* __restrict__ out) {
-  __shared__ double s_chunk[1024];
-  const uint32_t per = (nb + 1023) / 1024;
-  const uint32_t lo = min(nb, threadIdx.x * per), hi = min(nb, lo + per);
-  double acc = 0.0;
-  for (uint32_t b = lo; b < hi; b++) acc += bsum[b];
-  s_chunk[threadIdx.x] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double s = 0.0;
-    for (int q = 0; q < 1024; q++) s += s_chunk[q];
-    *out = s;
-  }
+  const double s = block_sum<kKmpRows>(m, s_part);
+  if (threadIdx.x == 0) bsum[blockIdx.x] = s;
 }
 
 __global__ void kmp_flag_kernel(const float* __restrict__ dists, const float* __restrict__ w, uint32_t n, uint32_t off,
                                 uint64_t key, double ell, double phi, uint8_t* __restrict__ flags) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const double u = static_cast<double>(kmp_mix(key ^ static_cast<uint64_t>(off + i)) >> 11) * (1.0 / 9007199254740992.0);
-  const double m = kmp_mass(dists[i], w ? w[i] : 1.f);
+  const double u = unit_co(splitmix64(key ^ static_cast<uint64_t>(off + i)));
+  const double m = d2_mass(dists[i], w ? w[i] : 1.f);
   flags[i] = u < (ell * m) / phi;
 }
 
@@ -233,11 +163,6 @@ cudaError_t launch_kmp_update(int metric, const float* X, uint32_t n, int D, con
   return cudaGetLastError();
 }
 
-cudaError_t launch_kmp_sum(const double* bsum, uint32_t nb, double* out, cudaStream_t st) {
-  kmp_sum_kernel<<<1, 1024, 0, st>>>(bsum, nb, out);
-  return cudaGetLastError();
-}
-
 size_t kmp_select_bytes(uint32_t n) {
   size_t bytes = 0;
   thrust::counting_iterator<uint32_t> it(0);
@@ -250,13 +175,7 @@ cudaError_t launch_kmp_draw(const float* dists, const float* w, uint32_t n, uint
                             double ell, double phi, uint8_t* flags, uint32_t* idx, uint32_t* d_count, void* tmp,
                             size_t tmp_bytes, cudaStream_t st) {
   if (n == 0) return cudaMemsetAsync(d_count, 0, sizeof(uint32_t), st);
-  const uint64_t key = [&] {   // mix((seed << 8) | round), computed once on the host
-    uint64_t z = (static_cast<uint64_t>(seed) << 8) | round;
-    z += 0x9E3779B97F4A7C15ull;
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    return z ^ (z >> 31);
-  }();
+  const uint64_t key = splitmix64((static_cast<uint64_t>(seed) << 8) | round);
   kmp_flag_kernel<<<cdiv(n, 256), 256, 0, st>>>(dists, w, n, off, key, ell, phi, flags);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;

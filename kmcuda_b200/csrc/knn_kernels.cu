@@ -10,8 +10,6 @@
 
 namespace kmb {
 
-static inline unsigned cdivk(size_t a, size_t b) { return static_cast<unsigned>((a + b - 1) / b); }
-
 // distance accumulated over feature chunks: fresh Kahan sum per chunk, chunks added with a plain
 // fp32 add, finalize at the end (knn.cu:36-47 with 16-feature chunks, knn.cu:79-100 with 24)
 template <int METRIC, int CHUNK>
@@ -52,9 +50,9 @@ cudaError_t launch_knn_radii(int metric, const float* X, const float* C, uint32_
   cudaMemsetAsync(radii, 0, sizeof(float) * K, st);
   if (n == 0) return cudaGetLastError();
   if (metric == 1)
-    knn_radii_kernel<1><<<cdivk(n, 256), 256, 0, st>>>(X, C, n, D, K, assign, reinterpret_cast<uint32_t*>(radii));
+    knn_radii_kernel<1><<<cdiv(n, 256), 256, 0, st>>>(X, C, n, D, K, assign, reinterpret_cast<uint32_t*>(radii));
   else
-    knn_radii_kernel<0><<<cdivk(n, 256), 256, 0, st>>>(X, C, n, D, K, assign, reinterpret_cast<uint32_t*>(radii));
+    knn_radii_kernel<0><<<cdiv(n, 256), 256, 0, st>>>(X, C, n, D, K, assign, reinterpret_cast<uint32_t*>(radii));
   return cudaGetLastError();
 }
 
@@ -71,8 +69,8 @@ __global__ void knn_cdist_kernel(const float* __restrict__ C, uint32_t K, int D,
 cudaError_t launch_knn_centroid_distances(int metric, const float* C, uint32_t K, int D, float* cd,
                                           cudaStream_t st) {
   size_t n = static_cast<size_t>(K) * K;
-  if (metric == 1) knn_cdist_kernel<1><<<cdivk(n, 128), 128, 0, st>>>(C, K, D, cd);
-  else knn_cdist_kernel<0><<<cdivk(n, 128), 128, 0, st>>>(C, K, D, cd);
+  if (metric == 1) knn_cdist_kernel<1><<<cdiv(n, 128), 128, 0, st>>>(C, K, D, cd);
+  else knn_cdist_kernel<0><<<cdiv(n, 128), 128, 0, st>>>(C, K, D, cd);
   return cudaGetLastError();
 }
 
@@ -204,7 +202,7 @@ cudaError_t launch_knn_search(int metric, int k, const float* X, const float* C,
   if (q_length == 0) return cudaSuccess;
   const int smem_d = D <= kKnnMaxSmemD ? D : 0;
   const size_t smem = static_cast<size_t>(kKnnWarps) * smem_d * sizeof(float);
-  const unsigned grid = rows ? device_sms() * 8u : static_cast<unsigned>(std::min<size_t>(cdivk(q_length, kKnnWarps), device_sms() * 64u));
+  const unsigned grid = rows ? device_sms() * 8u : static_cast<unsigned>(std::min<size_t>(cdiv(q_length, kKnnWarps), device_sms() * 64u));
   cudaError_t e;
   if (metric == 1) {
     if ((e = cudaFuncSetAttribute(knn_warp_search_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -224,7 +222,7 @@ cudaError_t launch_knn_search(int metric, int k, const float* X, const float* C,
 
 // empty clusters have no radius (NaN, knn.cu:56); run once after launch_knn_radii + the inverse assignment
 cudaError_t launch_knn_radii_fix(const uint32_t* inv_off, uint32_t K, float* radii, cudaStream_t st) {
-  knn_radii_fix_kernel<<<cdivk(K, 128), 128, 0, st>>>(inv_off, K, radii);
+  knn_radii_fix_kernel<<<cdiv(K, 128), 128, 0, st>>>(inv_off, K, radii);
   return cudaGetLastError();
 }
 
@@ -237,7 +235,7 @@ __global__ void knn_tail_rows_kernel(const uint32_t* __restrict__ inv, uint32_t 
 cudaError_t launch_knn_tail_rows(const uint32_t* inv, uint32_t nv, uint32_t n, uint32_t* rows, uint32_t* d_nrows,
                                  cudaStream_t st) {
   if (nv >= n) return cudaSuccess;
-  knn_tail_rows_kernel<<<cdivk(n - nv, 256), 256, 0, st>>>(inv, nv, n, rows, d_nrows);
+  knn_tail_rows_kernel<<<cdiv(n - nv, 256), 256, 0, st>>>(inv, nv, n, rows, d_nrows);
   return cudaGetLastError();
 }
 

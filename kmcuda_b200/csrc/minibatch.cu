@@ -4,7 +4,7 @@
 //              SplitMix64 counter hash with its own domain tag, so the draws depend on (seed, s, j) only
 //   assign     Shard::assign_rows: the exact argmin of every entry, the tensor-core pass reading X[row_j] itself
 //   inertia    sum_j w_j ||X[row_j] - c_{a_j}||^2 (the reference's L2 Kahan sum before its square root), block partials
-//              in double added in a fixed order (launch_kmp_sum)
+//              in double added in a fixed order (launch_fixed_sum)
 //   sums       the existing deterministic member sums (launch_partial_sums) with the entries' rows as the sorted values
 //   blend      c <- (c W_c + S_c) / (W_c + W_b,c), W_c += W_b,c for every centroid with W_b,c > 0
 //   reassign   (when the host says so) the centroids with W_c < 0.01 max W, at most floor(b / 2) of the smallest, become
@@ -16,6 +16,7 @@
 #include <cmath>
 
 #include "exact.cuh"
+#include "fixed_order.cuh"
 #include "kernels.h"
 
 namespace kmb {
@@ -24,28 +25,15 @@ namespace {
 
 constexpr int kMbRows = kStagedRows;   // rows per CTA of the inertia kernel (= threads)
 
-inline unsigned cdiv(size_t a, size_t b) { return static_cast<unsigned>((a + b - 1) / b); }
-
-__host__ __device__ __forceinline__ uint64_t mb_mix(uint64_t z) {
-  z += 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
-
-__device__ __forceinline__ double mb_unit(uint64_t h) {   // [0, 1)
-  return static_cast<double>(h >> 11) * (1.0 / 9007199254740992.0);
-}
-
 __global__ void mb_draw_kernel(uint32_t N, uint32_t b, uint64_t key, uint32_t* __restrict__ rows) {
   const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= b) return;
-  rows[j] = min(static_cast<uint32_t>(mb_unit(mb_mix(key ^ j)) * N), N - 1);
+  rows[j] = min(static_cast<uint32_t>(unit_co(splitmix64(key ^ j)) * N), N - 1);
 }
 
-// Exact squared L2 distance of every entry to its centroid, staged as kmp_update_kernel stages its rows.  Entries whose
-// winner is not a centroid (K for a NaN row, kUntouched when every score is NaN) carry no inertia and are given the key
-// K, so the member sums skip them.
+// Exact squared L2 distance of every entry to its centroid (staged_own_sum).  Entries whose winner is not a centroid
+// (K for a NaN row, kUntouched when every score is NaN) carry no inertia and are given the key K, so the member sums
+// skip them.
 template <bool VEC4>
 __global__ void __launch_bounds__(kMbRows)
 mb_inertia_kernel(const float* __restrict__ X, const uint32_t* __restrict__ rows, uint32_t n, int D,
@@ -54,7 +42,7 @@ mb_inertia_kernel(const float* __restrict__ X, const uint32_t* __restrict__ rows
   __shared__ uint32_t s_row[kMbRows];
   __shared__ float tile[kMbRows * 33];
   __shared__ double s_part[kMbRows / 32];
-  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int t = threadIdx.x;
   const uint32_t row0 = blockIdx.x * kMbRows, i = row0 + t;
   uint32_t a = K;
   if (i < n) a = min(result[i], K);
@@ -68,14 +56,8 @@ mb_inertia_kernel(const float* __restrict__ X, const uint32_t* __restrict__ rows
     keys[i] = a;
     if (live) m = static_cast<double>(w ? w[s_row[t]] : 1.f) * static_cast<double>(sum);
   }
-  for (int o = 16; o > 0; o >>= 1) m += __shfl_down_sync(0xffffffffu, m, o);
-  if (lane == 0) s_part[warp] = m;
-  __syncthreads();
-  if (t == 0) {
-    double s = 0.0;
-    for (int q = 0; q < kMbRows / 32; q++) s += s_part[q];
-    bsum[blockIdx.x] = s;
-  }
+  const double s = block_sum<kMbRows>(m, s_part);
+  if (t == 0) bsum[blockIdx.x] = s;
 }
 
 // c_new = (c W + S) / (W + W_b) where W_b > 0, else c; W_new = W + W_b
@@ -99,8 +81,7 @@ __global__ void mb_reassign_keys_kernel(uint32_t b, uint64_t key, const float* _
   const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= b) return;
   const float w = wrow ? wrow[rows[j]] : 1.f;
-  const double u = (static_cast<double>(mb_mix(key ^ j) >> 11) + 0.5) * (1.0 / 9007199254740992.0);   // (0, 1)
-  ekey[j] = w > 0.f ? -log(u) / static_cast<double>(w) : INFINITY;
+  ekey[j] = w > 0.f ? -log(unit_oo(splitmix64(key ^ j))) / static_cast<double>(w) : INFINITY;
   pos[j] = j;
   const unsigned act = __activemask();
   const unsigned live = __ballot_sync(act, w > 0.f);
@@ -159,28 +140,21 @@ mb_shift_kernel(const float* __restrict__ Cold, const float* __restrict__ Cnew, 
   if (threadIdx.x == 0) dsq[c] = ((s_part[0] + s_part[1]) + s_part[2]) + s_part[3];
 }
 
-// out[0] = sum of dsq[K] (contiguous chunk per thread, chunks in order), out[1] = #{W_c == 0}
+// out[0] = sum of dsq[K] (chunk_sum, fold_chunks), out[1] = #{W_c == 0}
 __global__ void __launch_bounds__(1024)
 mb_stats_kernel(const double* __restrict__ dsq, const double* __restrict__ W, uint32_t K, double* __restrict__ out) {
   __shared__ double s_chunk[1024];
   __shared__ uint32_t s_zero;
   if (threadIdx.x == 0) s_zero = 0;
   __syncthreads();
-  const uint32_t per = (K + 1023) / 1024;
-  const uint32_t lo = min(K, threadIdx.x * per), hi = min(K, lo + per);
-  double acc = 0.0;
-  uint32_t z = 0;
-  for (uint32_t c = lo; c < hi; c++) {
-    acc += dsq[c];
-    z += W[c] == 0.0;
-  }
-  s_chunk[threadIdx.x] = acc;
+  s_chunk[threadIdx.x] = chunk_sum(dsq, K);
+  uint32_t lo, hi, z = 0;
+  chunk_range(K, lo, hi);
+  for (uint32_t c = lo; c < hi; c++) z += W[c] == 0.0;
   if (z) atomicAdd(&s_zero, z);
   __syncthreads();
   if (threadIdx.x == 0) {
-    double s = 0.0;
-    for (int q = 0; q < 1024; q++) s += s_chunk[q];
-    out[0] = s;
+    out[0] = fold_chunks(s_chunk);
     out[1] = static_cast<double>(s_zero);
   }
 }
@@ -215,7 +189,7 @@ __global__ void mb_colfold_kernel(const double* __restrict__ partial, int nb, in
 
 }  // namespace
 
-uint64_t mb_step_key(uint32_t seed, uint64_t step, uint64_t tag) { return mb_mix(mb_mix(tag ^ seed) + step); }
+uint64_t mb_step_key(uint32_t seed, uint64_t step, uint64_t tag) { return splitmix64(splitmix64(tag ^ seed) + step); }
 
 cudaError_t launch_mb_draw(uint32_t N, uint32_t b, uint64_t key, uint32_t* rows, cudaStream_t st) {
   if (b == 0) return cudaSuccess;

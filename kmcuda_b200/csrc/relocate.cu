@@ -16,13 +16,39 @@
 #include <algorithm>
 
 #include "exact.cuh"
+#include "fixed_order.cuh"
 #include "shard.h"
 
 namespace kmb {
 
 namespace {
 
-inline unsigned cdiv(size_t a, size_t b) { return static_cast<unsigned>((a + b - 1) / b); }
+// The rule both the relocation keys and the inertia apply to shard row i of the CTA (kStagedRows threads): eligible
+// when assign[i] < K, w_i > 0 (w optional) and its distance d to its own centroid is finite; d = the L2 Kahan sum of
+// squared differences (before the square root) or the angle (METRIC 1).  wi = w_i (0 past the shard), d is set only
+// where eligible.
+template <bool VEC4, int METRIC>
+__device__ __forceinline__ bool eligible_own_distance(const float* __restrict__ X, uint32_t n, int D,
+                                                      const float* __restrict__ C, uint32_t K,
+                                                      const uint32_t* __restrict__ assign, const float* __restrict__ w,
+                                                      uint32_t* s_row, float* tile, float& d, float& wi) {
+  const int t = threadIdx.x;
+  const uint32_t row0 = blockIdx.x * kStagedRows, i = row0 + t;
+  uint32_t a = K;
+  wi = 0.f;
+  if (i < n) {
+    a = min(assign[i], K);
+    wi = w ? w[i] : 1.f;
+  }
+  const bool live = a < K && wi > 0.f;
+  const float* c = C + static_cast<size_t>(live ? a : 0) * D;
+  s_row[t] = i < n ? i : 0u;
+  __syncthreads();
+  const float sum = staged_own_sum<VEC4, METRIC>(X, s_row, row0, n, D, c, live, tile);
+  if (!live) return false;
+  d = METRIC == 1 ? acos_clamped(sum) : sum;
+  return isfinite(d);
+}
 
 template <bool VEC4, int METRIC>
 __global__ void __launch_bounds__(kStagedRows)
@@ -31,23 +57,12 @@ reloc_keys_kernel(const float* __restrict__ X, uint32_t n, int D, const float* _
                   uint64_t* __restrict__ keys) {
   __shared__ uint32_t s_row[kStagedRows];
   __shared__ float tile[kStagedRows * 33];
-  const int t = threadIdx.x;
-  const uint32_t row0 = blockIdx.x * kStagedRows, i = row0 + t;
-  uint32_t a = K;
-  float wi = 0.f;
+  const uint32_t i = blockIdx.x * kStagedRows + threadIdx.x;
+  float d, wi;
+  const bool eligible = eligible_own_distance<VEC4, METRIC>(X, n, D, C, K, assign, w, s_row, tile, d, wi);
   if (i < n) {
-    a = min(assign[i], K);
-    wi = w ? w[i] : 1.f;
-  }
-  const bool live = a < K && wi > 0.f;
-  const float* c = C + static_cast<size_t>(live ? a : 0) * D;
-  s_row[t] = i < n ? i : 0u;
-  __syncthreads();
-  const float sum = staged_own_sum<VEC4, METRIC>(X, s_row, row0, n, D, c, live, tile);
-  if (i < n) {
-    const float d = METRIC == 1 ? acos_clamped(sum) : sum;
     uint64_t key = 0;
-    if (live && isfinite(d)) {
+    if (eligible) {
       const uint32_t b = __float_as_uint(d);
       const uint32_t ob = (b & 0x80000000u) ? ~b : (b | 0x80000000u);
       key = (static_cast<uint64_t>(ob) << 32) | static_cast<uint32_t>(~(off + i));
@@ -56,9 +71,8 @@ reloc_keys_kernel(const float* __restrict__ X, uint32_t n, int D, const float* _
   }
 }
 
-// Inertia of a run (restarts, DESIGN.md §4n): the rows of reloc_keys_kernel with the same distance d, e = d (L2: the
-// Kahan sum of squared differences) or d^2 (angular: the angle); rows that would get key 0 there contribute 0.
-// bsum[block] = sum of w e over the block's rows, lanes and warps added in a fixed order.
+// Inertia of a run (restarts, DESIGN.md §4n): sum of w e over the block's eligible rows, e = d (L2: the Kahan sum of
+// squared differences) or d^2 (angular: the angle), into bsum[block] (block_sum).
 template <bool VEC4, int METRIC>
 __global__ void __launch_bounds__(kStagedRows)
 inertia_kernel(const float* __restrict__ X, uint32_t n, int D, const float* __restrict__ C, uint32_t K,
@@ -66,32 +80,12 @@ inertia_kernel(const float* __restrict__ X, uint32_t n, int D, const float* __re
   __shared__ uint32_t s_row[kStagedRows];
   __shared__ float tile[kStagedRows * 33];
   __shared__ double s_part[kStagedRows / 32];
-  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-  const uint32_t row0 = blockIdx.x * kStagedRows, i = row0 + t;
-  uint32_t a = K;
-  float wi = 0.f;
-  if (i < n) {
-    a = min(assign[i], K);
-    wi = w ? w[i] : 1.f;
-  }
-  const bool live = a < K && wi > 0.f;
-  const float* c = C + static_cast<size_t>(live ? a : 0) * D;
-  s_row[t] = i < n ? i : 0u;
-  __syncthreads();
-  const float sum = staged_own_sum<VEC4, METRIC>(X, s_row, row0, n, D, c, live, tile);
+  float d, wi;
   double m = 0.0;
-  if (live) {
-    const float d = METRIC == 1 ? acos_clamped(sum) : sum;
-    if (isfinite(d)) m = static_cast<double>(wi) * (METRIC == 1 ? static_cast<double>(d) * d : static_cast<double>(d));
-  }
-  for (int o = 16; o > 0; o >>= 1) m += __shfl_down_sync(0xffffffffu, m, o);
-  if (lane == 0) s_part[warp] = m;
-  __syncthreads();
-  if (t == 0) {
-    double s = 0.0;
-    for (int q = 0; q < kStagedRows / 32; q++) s += s_part[q];
-    bsum[blockIdx.x] = s;
-  }
+  if (eligible_own_distance<VEC4, METRIC>(X, n, D, C, K, assign, w, s_row, tile, d, wi))
+    m = static_cast<double>(wi) * (METRIC == 1 ? static_cast<double>(d) * d : static_cast<double>(d));
+  const double s = block_sum<kStagedRows>(m, s_part);
+  if (threadIdx.x == 0) bsum[blockIdx.x] = s;
 }
 
 // one radix-select pass: histogram of the 8-bit digit at `shift` over the eligible keys whose higher digits equal the
@@ -240,7 +234,7 @@ cudaError_t launch_inertia(int metric, const float* X, uint32_t n, int D, const 
     else inertia_kernel<false, 0><<<grid, kStagedRows, 0, st>>>(X, n, D, C, K, assign, w, bsum);
   }
   cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? launch_kmp_sum(bsum, grid, out, st) : e;
+  return e == cudaSuccess ? launch_fixed_sum(bsum, grid, out, st) : e;
 }
 
 uint32_t reloc_cap(uint32_t T) { return 2 * T + 4096; }

@@ -346,7 +346,7 @@ KMCUDAResult Job::init_kmeans_parallel(uint32_t rounds, uint32_t seed) {
            kmcudaMemoryCopyError);
     KMB_CU(launch_kmp_update(metric, d.X, d.len, D, w.table, 1, nullptr, 0, d.dists, w.nearest, d.w.get(), w.bsum, d.st),
            kmcudaRuntimeError);
-    KMB_CU(launch_kmp_sum(w.bsum, w.nb, w.phi, d.st), kmcudaRuntimeError);
+    KMB_CU(launch_fixed_sum(w.bsum, w.nb, w.phi, d.st), kmcudaRuntimeError);
   }
   const double ell = 2.0 * K;
   for (uint32_t r = 1; r <= rounds; r++) {
@@ -420,7 +420,7 @@ KMCUDAResult Job::init_kmeans_parallel(uint32_t rounds, uint32_t seed) {
       KMB_RET(pass[s]->assign(d.len, d.X, w.table, d.assign, d.prev, d.d_changed, d.st));
       KMB_CU(launch_kmp_update(metric, d.X, d.len, D, w.table, fresh, d.assign, base, d.dists, w.nearest, d.w.get(),
                                w.bsum, d.st), kmcudaRuntimeError);
-      KMB_CU(launch_kmp_sum(w.bsum, w.nb, w.phi, d.st), kmcudaRuntimeError);
+      KMB_CU(launch_fixed_sum(w.bsum, w.nb, w.phi, d.st), kmcudaRuntimeError);
     }
     KMB_RET(sync_all());
     for (auto& p : pass) KMB_RET(p->check_pipeline());

@@ -10,6 +10,7 @@
 #include <algorithm>
 
 #include "exact.cuh"
+#include "fixed_order.cuh"
 #include "kernels.h"
 
 namespace kmb {
@@ -23,8 +24,6 @@ unsigned device_sms() {
   }
   return static_cast<unsigned>(n);
 }
-
-static inline unsigned cdiv(size_t a, size_t b) { return static_cast<unsigned>((a + b - 1) / b); }
 
 // row lists up to this length are handled one CTA per row (exact_rows_few_kernel)
 constexpr uint32_t kFewRows = 8192;
@@ -1060,15 +1059,8 @@ pp_update_kernel(const float* __restrict__ X, uint32_t n, int D, const float* __
     else dist = prev;
     if (WEIGHTED) dist *= w[i];
   }
-  double v = (dist == dist) ? static_cast<double>(dist) : 0.0;
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-  if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = v;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0.0;
-    for (int k = 0; k < kPpBlock / 32; k++) t += s_part[k];
-    bsum[blockIdx.x] = t;            // deterministic (fixed order), unlike an atomic total
-  }
+  const double t = block_sum<kPpBlock>((dist == dist) ? static_cast<double>(dist) : 0.0, s_part);
+  if (threadIdx.x == 0) bsum[blockIdx.x] = t;   // deterministic (fixed order), unlike an atomic total
 }
 
 // prefix P(t) = sum of the first t distances, from the scanned block sums + the tail of one block
@@ -1090,11 +1082,7 @@ pp_pick_kernel(const float* __restrict__ X, uint32_t n, int D, const float* __re
   __shared__ double s_total;
   __shared__ uint32_t s_j;
   // exclusive scan of the block sums into bpre[0 .. nb] (bpre[nb] = total): each thread owns a contiguous chunk
-  const uint32_t per = (nb + 1023) / 1024;
-  const uint32_t lo = min(nb, threadIdx.x * per), hi = min(nb, lo + per);
-  double acc = 0.0;
-  for (uint32_t b = lo; b < hi; b++) acc += bsum[b];
-  s_chunk[threadIdx.x] = acc;
+  s_chunk[threadIdx.x] = chunk_sum(bsum, nb);
   __syncthreads();
   if (threadIdx.x == 0) {
     double run = 0.0;
@@ -1106,6 +1094,8 @@ pp_pick_kernel(const float* __restrict__ X, uint32_t n, int D, const float* __re
     s_total = run;
   }
   __syncthreads();
+  uint32_t lo, hi;
+  chunk_range(nb, lo, hi);
   double run = s_chunk[threadIdx.x];
   for (uint32_t b = lo; b < hi; b++) {
     bpre[b] = run;
@@ -1229,6 +1219,20 @@ cudaError_t launch_afkmc2_min_dist(int metric, const float* X, const float* C, i
     afkmc2_min_dist_kernel<1><<<grid, 128, 0, st>>>(X, C, D, k, rows, m, reinterpret_cast<uint32_t*>(min_dists));
   else
     afkmc2_min_dist_kernel<0><<<grid, 128, 0, st>>>(X, C, D, k, rows, m, reinterpret_cast<uint32_t*>(min_dists));
+  return cudaGetLastError();
+}
+
+// *out = bsum[0] + ... + bsum[nb - 1] in a fixed order (chunk_sum, fold_chunks)
+__global__ void __launch_bounds__(1024)
+fixed_sum_kernel(const double* __restrict__ bsum, uint32_t nb, double* __restrict__ out) {
+  __shared__ double s_chunk[1024];
+  s_chunk[threadIdx.x] = chunk_sum(bsum, nb);
+  __syncthreads();
+  if (threadIdx.x == 0) *out = fold_chunks(s_chunk);
+}
+
+cudaError_t launch_fixed_sum(const double* bsum, uint32_t nb, double* out, cudaStream_t st) {
+  fixed_sum_kernel<<<1, 1024, 0, st>>>(bsum, nb, out);
   return cudaGetLastError();
 }
 
