@@ -64,8 +64,10 @@ typedef struct kmcuda_b200_shard kmcuda_b200_shard;
  * with KMCUDA_B200_STRICT_UPDATE=1.  The assignment step is unchanged; the centroid update is sum(w x) / sum(w) (L2)
  * or the angular recurrence with weight totals for counts; a cluster whose weight total is 0 is treated as the
  * reference treats an empty cluster (L2: NaN centroid, never chosen again; angular: the same recurrence);
- * k-means++ draws proportionally to w * d, AFK-MC2 uses q = w / 2W + w d^2 / (2 sum w d^2), random init skips rows
- * of weight 0, and average_distance is sum(w d) / sum(w).  With every weight 1 the result is bit-identical to
+ * k-means++ draws proportionally to w * d, AFK-MC2 uses q = w / 2W + w d^2 / (2 sum w d^2) (q = 0, never drawn, on
+ * rows of weight 0 and on rows whose distance d to the first centroid is not finite: every row with a NaN feature,
+ * which also adds nothing to sum w d^2), random init skips rows of weight 0, and average_distance is
+ * sum(w d) / sum(w).  With every weight 1 the result is bit-identical to
  * kmeans_cuda(). */
 KMCUDAResult kmcuda_b200_kmeans_weighted(KMCUDAInitMethod init, const void *init_params, float tolerance,
                                          float yinyang_t, KMCUDADistanceMetric metric, uint32_t samples_size,

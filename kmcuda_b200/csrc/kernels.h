@@ -135,9 +135,11 @@ cudaError_t launch_average_distance(int metric, const float* X, const float* C, 
                                     const uint32_t* assign, double* d_sum, cudaStream_t st, const float* w = nullptr);
 cudaError_t launch_afkmc2_min_dist(int metric, const float* X, const float* C, int D, uint32_t k,
                                    const uint32_t* rows, uint32_t m, float* min_dists, cudaStream_t st);
-// w (optional): dists[] stays the plain minimum distance, *d_sum accumulates w_i * d_i
+// w (optional): dists[] stays the plain minimum distance, *d_sum accumulates w_i * d_i; rows whose first feature is NaN
+// get the distance nan_row_dist (AFK-MC2 passes NaN to tell them from rows at distance 0)
 cudaError_t launch_plusplus_step(int metric, const float* X, uint32_t n, int D, const float* centroid,
-                                 int first, float* dists, double* d_sum, cudaStream_t st, const float* w = nullptr);
+                                 int first, float* dists, double* d_sum, cudaStream_t st, const float* w = nullptr,
+                                 float nan_row_dist = 0.f);
 // device-resident k-means++ round (simt_kernels.cu): bsum / bpre hold ceil(n / 256) + 1 doubles, chosen [K];
 // w (optional): the draw is proportional to w_i * d_i and never picks a zero-weight row
 cudaError_t launch_plusplus_round(int metric, const float* X, uint32_t n, int D, float* C, uint32_t i, double choice,

@@ -194,6 +194,9 @@ KMCUDAResult Job::init_plusplus() {
 // the candidates' nearest-centroid distances) runs on the shards that own the samples.
 //
 // Weighted: q = w / (2 W) + w d^2 / (2 sum w d^2) and p = w * (squared distance), so zero-weight rows are never drawn.
+// Rows whose distance to c0 is not finite (a NaN feature, the first one included) have q = 0 and add nothing to
+// sum w d^2: they are never drawn either.  Drawn, such a row would have no finite distance to any centroid, p = +inf,
+// and the chain would always take it.
 KMCUDAResult Job::init_afkmc2(uint32_t m, uint32_t seed) {
   std::vector<float> hostC(static_cast<size_t>(K) * D);
   std::vector<float> host_dists(N);
@@ -205,7 +208,8 @@ KMCUDAResult Job::init_afkmc2(uint32_t m, uint32_t seed) {
     KMB_CU(d.dists.alloc(std::max<size_t>(d.len, 2 * static_cast<size_t>(m))), kmcudaMemoryAllocationFailure);
     KMB_CU(cudaMemcpyAsync(d.C.get(), hostC.data(), sizeof(float) * D, cudaMemcpyHostToDevice, d.st), kmcudaMemoryCopyError);
     KMB_CU(cudaMemsetAsync(d.d_dsum.get(), 0, sizeof(double), d.st), kmcudaRuntimeError);
-    KMB_CU(launch_plusplus_step(metric, d.X, d.len, D, d.C.get(), 1, d.dists, d.d_dsum, d.st), kmcudaRuntimeError);
+    KMB_CU(launch_plusplus_step(metric, d.X, d.len, D, d.C.get(), 1, d.dists, d.d_dsum, d.st, nullptr, NAN),
+           kmcudaRuntimeError);
     KMB_CU(cudaMemcpyAsync(host_dists.data() + d.off, d.dists.get(), sizeof(float) * d.len, cudaMemcpyDeviceToHost, d.st),
            kmcudaMemoryCopyError);
   }
@@ -218,14 +222,14 @@ KMCUDAResult Job::init_afkmc2(uint32_t m, uint32_t seed) {
     double dsum = 0;
     for (uint32_t i = 0; i < N; i++) {
       const double d2 = static_cast<double>(host_dists[i]) * host_dists[i];
-      if (d2 == d2) dsum += weighted ? host_w[i] * d2 : d2;
+      if (std::isfinite(d2)) dsum += weighted ? host_w[i] * d2 : d2;
     }
     double acc = 0;
     for (uint32_t i = 0; i < N; i++) {
-      double d2 = static_cast<double>(host_dists[i]) * host_dists[i];
-      if (!(d2 == d2)) d2 = 0;
+      const double d2 = static_cast<double>(host_dists[i]) * host_dists[i];
       const double wi = weighted ? host_w[i] : 1.0;
-      const double qi = wi / (2.0 * W) + (dsum > 0 ? wi * d2 / (2.0 * dsum) : wi / (2.0 * W));
+      const double qi = !std::isfinite(d2) ? 0.0
+                        : wi / (2.0 * W) + (dsum > 0 ? wi * d2 / (2.0 * dsum) : wi / (2.0 * W));
       q[i] = static_cast<float>(qi);
       acc += qi;
       cdf[i] = acc;

@@ -946,16 +946,18 @@ cudaError_t launch_average_distance(int metric, const float* X, const float* C, 
   return cudaGetLastError();
 }
 
-// WEIGHTED: dists[] keeps the plain minimum distance d_i (the next round compares against it); d_sum adds w_i * d_i
+// WEIGHTED: dists[] keeps the plain minimum distance d_i (the next round compares against it); d_sum adds w_i * d_i.
+// A row whose first feature is NaN gets the distance nan_row_dist (k-means++: 0, the reference's rule)
 template <int METRIC, bool WEIGHTED>
 __global__ void plusplus_kernel(const float* __restrict__ X, uint32_t n, int D,
                                 const float* __restrict__ centroid, int first,
-                                float* __restrict__ dists, double* __restrict__ d_sum, const float* __restrict__ w) {
+                                float* __restrict__ dists, double* __restrict__ d_sum, const float* __restrict__ w,
+                                float nan_row_dist) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   float dist = 0.f;
   if (i < n) {
     const float* x = X + static_cast<size_t>(i) * D;
-    if (x[0] == x[0]) dist = distance_exact<METRIC>(x, centroid, D);
+    dist = x[0] == x[0] ? distance_exact<METRIC>(x, centroid, D) : nan_row_dist;
     float prev;
     if (first || dist < (prev = dists[i])) dists[i] = dist;
     else dist = prev;
@@ -966,16 +968,19 @@ __global__ void plusplus_kernel(const float* __restrict__ X, uint32_t n, int D,
 }
 
 cudaError_t launch_plusplus_step(int metric, const float* X, uint32_t n, int D, const float* centroid,
-                                 int first, float* dists, double* d_sum, cudaStream_t st, const float* w) {
+                                 int first, float* dists, double* d_sum, cudaStream_t st, const float* w,
+                                 float nan_row_dist) {
   if (n == 0) return cudaSuccess;
   const unsigned grid = cdiv(n, 256);
   if (w) {
-    if (metric == 1) plusplus_kernel<1, true><<<grid, 256, 0, st>>>(X, n, D, centroid, first, dists, d_sum, w);
-    else plusplus_kernel<0, true><<<grid, 256, 0, st>>>(X, n, D, centroid, first, dists, d_sum, w);
+    if (metric == 1)
+      plusplus_kernel<1, true><<<grid, 256, 0, st>>>(X, n, D, centroid, first, dists, d_sum, w, nan_row_dist);
+    else plusplus_kernel<0, true><<<grid, 256, 0, st>>>(X, n, D, centroid, first, dists, d_sum, w, nan_row_dist);
     return cudaGetLastError();
   }
-  if (metric == 1) plusplus_kernel<1, false><<<grid, 256, 0, st>>>(X, n, D, centroid, first, dists, d_sum, nullptr);
-  else plusplus_kernel<0, false><<<grid, 256, 0, st>>>(X, n, D, centroid, first, dists, d_sum, nullptr);
+  if (metric == 1)
+    plusplus_kernel<1, false><<<grid, 256, 0, st>>>(X, n, D, centroid, first, dists, d_sum, nullptr, nan_row_dist);
+  else plusplus_kernel<0, false><<<grid, 256, 0, st>>>(X, n, D, centroid, first, dists, d_sum, nullptr, nan_row_dist);
   return cudaGetLastError();
 }
 
