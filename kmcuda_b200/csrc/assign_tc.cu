@@ -45,10 +45,12 @@
 
 #include <cstdio>
 #include <algorithm>
+#include <array>
 #include <cstring>
 #include <map>
 #include <mutex>
 #include <tuple>
+#include <utility>
 #include <vector>
 
 #include <cub/cub.cuh>
@@ -83,9 +85,6 @@ constexpr int LIST_ARRAYS = 4;
 #ifndef KMB_KO
 #define KMB_KO 0
 #endif
-#ifndef KMB_PREP_FUSED
-#define KMB_PREP_FUSED 1   // 1: centroid preparation as one launch (tc_prep_fused_kernel), 0: the chain of small kernels
-#endif
 // Four warpgroups: 0 = emitters + B producer, 1 = converters, 2 and 3 = consumers.
 constexpr int FIRST_EMIT_WARP = 0;      // 3 emitter warps (merge + global emission)
 constexpr int WARP_B_PRODUCER = 3;      // TMA producer: the last warp of warpgroup 0
@@ -119,7 +118,7 @@ struct Stats {       // written by the centroid prep kernels, read by the main k
   uint32_t csq_max_bits;
   uint32_t force_exact; // cosine only: a centroid with an infinite element / norm can still win -> no filtering
   float yabs;           // k-NN: max over samples of s * (|y| + |c(y)|): bounds the rounding of the centring y - c
-  float mun;            // s * ||mu|| (upper bound): mu = centring vector of the assignment filter (0 when not centred)
+  float mun;            // s * ||mu|| (upper bound): mu = centring vector of the assignment filter (0: cosine, k-NN)
   float knn_extra;      // k-NN, angular metric served through the L2 pass: s^2 * max |1 - ||y||^2| (see tc_knn_search)
 };
 
@@ -200,49 +199,51 @@ enum {
 };
 static_assert(BAR_COUNT <= 63, "barrier array too small");   // slot 63 is the CTA's "a wait has given up" flag
 
+// Every field defaults to 0 / nullptr (one device: knn_nparts = 1); a pass sets the fields its MODE reads.
 struct Params {
-  uint32_t n;
-  int D;
-  uint32_t K;
-  int nkb;                   // K-blocks of 64 features
-  int nt;                    // n-tiles of 128 centroids
-  uint32_t ntiles;           // sample tiles
-  const __half* aug_blob;    // [nt][AUG_B_BYTES] in the shared-memory byte layout
-  const Stats* stats;
-  uint32_t* result;          // [n]
-  uint32_t* pair_row;        // re-check queue: (row, candidate) pairs
-  uint32_t* pair_cand;
-  uint32_t max_pairs;
-  uint32_t* rowq;            // [3*i]: row, first pair, pair count
-  uint32_t* ovf_rows;        // rows for the full exact pass
-  uint32_t* counters;        // CNT_*
-  int metric;                // 0 = L2 (score x.c - ||c||^2/2), 1 = cosine (score x.c; larger dot = smaller angle)
-  const float* neg_mu_s;     // [nkb*64] -mu*s (zero padded), nullptr = no centring: MODE 0/1 multiply (x - mu) with the
-                             // table of (c - mu); scores shift by a per-row constant, so the ranking is unchanged while
-                             // the fp16 rounding error (proportional to |x - mu| |c - mu|) shrinks
+  uint32_t n = 0;
+  int D = 0;
+  uint32_t K = 0;
+  int nkb = 0;                   // K-blocks of 64 features
+  int nt = 0;                    // n-tiles of 128 centroids
+  uint32_t ntiles = 0;           // sample tiles
+  const __half* aug_blob = nullptr;   // [nt][AUG_B_BYTES] in the shared-memory byte layout
+  const Stats* stats = nullptr;
+  uint32_t* result = nullptr;    // [n]
+  uint32_t* pair_row = nullptr;  // re-check queue: (row, candidate) pairs
+  uint32_t* pair_cand = nullptr;
+  uint32_t max_pairs = 0;
+  uint32_t* rowq = nullptr;      // [3*i]: row, first pair, pair count
+  uint32_t* ovf_rows = nullptr;  // rows for the full exact pass
+  uint32_t* counters = nullptr;  // CNT_*
+  int metric = 0;                // 0 = L2 (score x.c - ||c||^2/2), 1 = cosine (score x.c; larger dot = smaller angle)
+  const float* neg_mu_s = nullptr;   // [nkb*64] -mu*s (zero padded), nullptr = no centring: MODE 0/1 multiply
+                                     // (x - mu) with the table of (c - mu); scores shift by a per-row constant, so the
+                                     // ranking is unchanged while the fp16 rounding error (proportional to
+                                     // |x - mu| |c - mu|) shrinks
   // MODE 0 with assign != nullptr: the bookkeeping of the assignment pass is fused (reference kmeans.cu:356-363):
   // prev[row] = assign[row]; assign[row] = winner; *d_changed += (winner != old); rows that go to the re-check /
   // exact queues are finished by those kernels
-  uint32_t* assign;
-  uint32_t* prev;
-  uint32_t* d_changed;
+  uint32_t* assign = nullptr;
+  uint32_t* prev = nullptr;
+  uint32_t* d_changed = nullptr;
   // MODE 3 (Yinyang bounds refresh, reference kmeans_yy_init kmeans.cu:431-485): the table is the GROUP-SORTED
   // centroid list, every group padded to whole 4-column quads (yy_qgroup[(n-tile * 2 + half) * 16 + quad] = group of
   // that quad, UINT32_MAX past the end).  The epilogue folds the quad maxima into per-group maxima and turns each
   // into a LOWER bound of the distance to the nearest centroid of that group, d >= sqrt(|x^|^2 - 2 (max + E)) / s,
   // merged into bounds[row][1 + g] with an atomic minimum; the sample's own group and its upper bound are exact
   // (yy_own_group_kernel).  Valid bounds are all Yinyang needs: the assignments stay those of Lloyd's algorithm.
-  const uint32_t* yy_qgroup;
-  const uint32_t* yy_groups;     // [K] centroid -> group
-  const uint32_t* yy_assign;     // [n]
-  float* yy_bounds;              // [n][G + 1]
-  uint32_t G;
+  const uint32_t* yy_qgroup = nullptr;
+  const uint32_t* yy_groups = nullptr;   // [K] centroid -> group
+  const uint32_t* yy_assign = nullptr;   // [n]
+  float* yy_bounds = nullptr;            // [n][G + 1]
+  uint32_t G = 0;
   // MODE 1 (Yinyang local step): the samples are the rows listed in rows[0 .. *d_nrows), read straight from
   // global memory by the converter warps; every column within the margin of the row's SECOND best score is a
   // candidate and every candidate goes to the pair queue (the caller needs exact best and second-best distances)
-  const float* X;
-  const uint32_t* rows;
-  const uint32_t* d_nrows;
+  const float* X = nullptr;
+  const uint32_t* rows = nullptr;
+  const uint32_t* d_nrows = nullptr;
   // MODE 2 (k-NN candidate pass): queries AND candidates are the samples in the cluster-aligned table order: cluster
   // c owns the blocks [blk_first[c], blk_first[c+1]) of 128 table rows (zero-padded), rows[] maps a table row to the
   // original sample (UINT32_MAX = padding), so query tile t IS block t.  A tile is multiplied with a list of
@@ -254,26 +255,25 @@ struct Params {
   // kk-th largest 4-column-group maximum (kk = k + 1, self included) is recorded as (max, mask, chunk id, margin).
   // 64-row tiles (NKB 9..16): query tile t is half t & 1 of block t >> 1; the per-tile arrays below stay per block and
   // are read at t >> 1, so the kernel runs 2 * (blocks) tiles and skips a second half without live rows.
-  const uint32_t* d_ntiles;
-  const uint32_t* tile_nrows;
-  const uint32_t* blk_cluster;
-  const float* C;                // centroids [K][D] (fp32)
-  const uint2* knn_ranges;
-  const uint32_t* knn_roff;
-  const uint32_t* knn_rcount;
-  const uint32_t* knn_nblk;      // blocks per tile (sum over its segments)
-  int kk;
-  int knn_first_pass;            // 1: the per-row state starts empty; the tile has TWO segments, both its own cluster:
+  const uint32_t* d_ntiles = nullptr;
+  const uint32_t* tile_nrows = nullptr;
+  const uint32_t* blk_cluster = nullptr;
+  const float* C = nullptr;                // centroids [K][D] (fp32)
+  const uint2* knn_ranges = nullptr;
+  const uint32_t* knn_roff = nullptr;
+  const uint32_t* knn_rcount = nullptr;
+  const uint32_t* knn_nblk = nullptr;      // blocks per tile (sum over its segments)
+  int kk = 0;
+  int knn_first_pass = 0;        // 1: the per-row state starts empty; the tile has TWO segments, both its own cluster:
                                  //    the first sweep only builds the top-kk threshold, the second one only records
-  uint32_t knn_stride;           // = parts * (table rows): stride of the [kk][stride] top-kk state (2 parts per row, 4 at
-                                 //   NKB 9..16)
-  float* knn_topk;               // [kk][stride] descending group maxima (g-space) of part (table row * parts + part)
-  uint32_t* knn_cnt;             // [stride] entries used
-  uint32_t* knn_flags;           // [stride]
-  float* knn_dub;                // [stride] upper bound of the exact distance to the kk-th nearest candidate seen so far
-  uint4* knn_entries;            // [stride][KNN_CAP]: (group max bits (g-space), mask, chunk id, margin bits)
-  uint32_t knn_part, knn_nparts; // query-tile shard of this device (0, 1 = everything)
-  float* dbg_scores;         // optional [ntiles*128][nt*128] dump of the approximate scores
+  uint32_t knn_stride = 0;       // = parts * (table rows): stride of the [kk][stride] top-kk state (2 parts per row,
+                                 //   4 at NKB 9..16)
+  float* knn_topk = nullptr;     // [kk][stride] descending group maxima (g-space) of part (table row * parts + part)
+  uint32_t* knn_cnt = nullptr;   // [stride] entries used
+  uint32_t* knn_flags = nullptr; // [stride]
+  float* knn_dub = nullptr;      // [stride] upper bound of the exact distance to the kk-th nearest candidate so far
+  uint4* knn_entries = nullptr;  // [stride][KNN_CAP]: (group max bits (g-space), mask, chunk id, margin bits)
+  uint32_t knn_part = 0, knn_nparts = 1;   // query-tile shard of this device (0, 1 = everything)
 };
 
 // ---------------------------------------------------------------------------------------------------
@@ -290,101 +290,45 @@ __global__ void tc_prep_stats_kernel(const float* __restrict__ csq, uint32_t K, 
   if ((threadIdx.x & 31) == 0) atomicMax(&st->csq_max_bits, best);
 }
 
-// cosine: upper bound of ||c||^2 per centroid (one warp per row)
-// (k-NN: the "centroids" are the samples in cluster-sorted order, row r = C[gather[r]], and the value feeds the bias
-// term, so no safety factor is applied)
-__global__ void tc_prep_norms_kernel(const float* __restrict__ C, uint32_t K, int D, float* __restrict__ out,
-                                     const uint32_t* __restrict__ gather, float factor) {
-  const uint32_t row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (row >= K) return;
-  const float* src = C + static_cast<size_t>(gather ? gather[row] : row) * D;
-  float a = 0.f;
-  for (int f = lane; f < D; f += 32) {
-    float v = src[f];
-    a = fmaf(v, v, a);
-  }
-  for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
-  if (lane == 0) out[row] = a * factor;
-}
-
-// centring vector of the L2 filter: column sums of the valid centroids (rows whose ||c||^2 is finite).  ANY vector
-// is a correct choice of mu (scores shift by a per-row constant); the mean minimises the operand norms.
-__global__ void tc_prep_mean_kernel(const float* __restrict__ C, const float* __restrict__ csq, uint32_t K, int D,
-                                    double* __restrict__ musum, uint32_t* __restrict__ nvalid) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  const uint32_t r0 = blockIdx.y * 64u, r1 = min(K, r0 + 64u);
-  double a = 0.0;
-  uint32_t nv = 0;
-  // 8 rows per step, loads first: the 64 rows of a CTA were one chain of dependent global loads before (36 us per pass)
-  for (uint32_t rb = r0; rb < r1; rb += 8) {
-    float v[8], q[8];
-#pragma unroll
-    for (int j = 0; j < 8; j++) {
-      const uint32_t r = min(rb + j, r1 - 1);
-      q[j] = csq[r];
-      v[j] = f < D ? C[static_cast<size_t>(r) * D + f] : 0.f;
-    }
-#pragma unroll
-    for (int j = 0; j < 8; j++) {
-      if (rb + j >= r1 || !(q[j] == q[j] && q[j] < 3.0e38f)) continue;
-      nv++;
-      a += static_cast<double>(v[j]);
-    }
-  }
-  if (f < D && nv) atomicAdd(&musum[f], a);
-  if (blockIdx.x == 0 && threadIdx.x == 0 && nv) atomicAdd(nvalid, nv);
-}
-__global__ void tc_prep_mu_kernel(const double* __restrict__ musum, const uint32_t* __restrict__ nvalid, int D,
-                                  float* __restrict__ mu) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= D) return;
-  const uint32_t nv = *nvalid;
-  const float m = nv ? static_cast<float>(musum[f] / nv) : 0.f;
-  mu[f] = (fabsf(m) < 3.0e38f) ? m : 0.f;
-}
-// ||c - mu||^2 per centroid (one warp per row, double accumulation: the value becomes the bias term)
-__global__ void tc_prep_cnorm_kernel(const float* __restrict__ C, const float* __restrict__ csq,
-                                     const float* __restrict__ mu, uint32_t K, int D, float* __restrict__ out) {
-  const uint32_t row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (row >= K) return;
-  const float* src = C + static_cast<size_t>(row) * D;
-  double a = 0.0;
-  for (int f = lane; f < D; f += 32) {
-    const float v = src[f] - mu[f];      // the fp32 difference IS the table operand (before scaling)
-    a += static_cast<double>(v) * v;
-  }
-  for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
-  if (lane == 0) {
-    const float q = csq[row];
-    out[row] = (q == q && q < 3.0e38f) ? static_cast<float>(a) : q;   // dead centroids stay dead
-  }
-}
-
-__global__ void tc_prep_scale_kernel(Stats* __restrict__ st, const float* __restrict__ mu, int D, int Dp,
-                                     float* __restrict__ neg_mu_s) {   // one warp
-  const int lane = threadIdx.x;
-  float cmax = __fsqrt_ru(__uint_as_float(st->csq_max_bits));
+// s = 2^k with s * cmax in [32, 64); 1 when cmax is 0 or not finite
+__device__ __forceinline__ float prep_scale(float cmax) {
   float s = 1.f;
   if (cmax > 0.f && cmax < 3.0e38f) {
     int e;
     frexpf(cmax, &e);          // cmax = m * 2^e, m in [0.5, 1)
     s = ldexpf(1.f, 6 - e);    // s*cmax in [32, 64)
   }
-  float m2 = 0.f;
-  if (neg_mu_s)
-    for (int f = lane; f < Dp; f += 32) {
-      const float m = (mu && f < D) ? mu[f] : 0.f;
-      neg_mu_s[f] = -m * s;      // exact (power of two) unless it overflows, which the norm below reports
-      m2 = fmaf(m * s, m * s, m2);
-    }
-  for (int o = 16; o > 0; o >>= 1) m2 += __shfl_xor_sync(0xffffffffu, m2, o);
-  if (lane == 0) {
-    st->scale = s;
-    st->cmax = cmax * s * 1.001f;
-    st->dcmax = 0.f;
-    st->mun = __fsqrt_ru(m2) * 1.002f;   // (1.002: the lane-partial sums are added in a different order than a serial loop)
+  return s;
+}
+
+// k-NN (one thread): scale and norm bound of the table from tc_prep_stats_kernel's maximum; the caller zeroes the
+// Stats, and the table kernel raises dcmax from there
+__global__ void tc_prep_scale_kernel(Stats* __restrict__ st) {
+  const float cmax = __fsqrt_ru(__uint_as_float(st->csq_max_bits));
+  const float s = prep_scale(cmax);
+  st->scale = s;
+  st->cmax = cmax * s * 1.001f;
+}
+
+// bias of table row `row`: h as three fp16 terms, or -65504 for a padding / invalid row, in the row's slot of the
+// K = 16 no-swizzle block (core matrix = 8 rows x 16 bytes contiguous, 8-row groups 128 bytes apart, second K half
+// TN*16 bytes further)
+__device__ __forceinline__ void write_bias_row(__half* __restrict__ aug_blob, uint32_t row, bool valid, float h) {
+  __half b[3];
+  if (valid) {
+    b[0] = __float2half_rn(h);
+    const float r1 = h - __half2float(b[0]);
+    b[1] = __float2half_rn(r1);
+    b[2] = __float2half_rn(r1 - __half2float(b[1]));
+  } else {
+    b[0] = __float2half_rn(-65504.f);
+    b[1] = b[2] = __float2half_rn(0.f);
+  }
+  const uint32_t t = row / TN, r = row % TN;
+  __half* blob = aug_blob + static_cast<size_t>(t) * (AUG_B_BYTES / 2);
+  for (int k = 0; k < 16; k++) {
+    const int j = k >> 3, e = k & 7;
+    blob[(j * (TN * 16) + (r >> 3) * 128 + (r & 7) * 16) / 2 + e] = k < 3 ? b[k] : __float2half_rn(0.f);
   }
 }
 
@@ -439,61 +383,28 @@ __device__ __forceinline__ void prep_table_row(uint32_t row, int lane, float s, 
   for (int o = 16; o > 0; o >>= 1) d2 += __shfl_xor_sync(0xffffffffu, d2, o);
   if (lane == 0) {
     if (finite) atomicMax(reinterpret_cast<uint32_t*>(&st->dcmax), __float_as_uint(__fsqrt_ru(d2) * 1.0001f));
-    // bias: three fp16 terms of -(s^2 ||c - mu||^2 / 2); invalid / padded centroids get -65504
-    __half b[3];
-    if (finite) {
-      float h = metric == 1 ? 0.f : -0.5f * ((s * __ldcg(csq + qrow)) * s);   // s = 2^k: exact; this order cannot overflow for tiny data
-      b[0] = __float2half_rn(h);
-      float r1 = h - __half2float(b[0]);
-      b[1] = __float2half_rn(r1);
-      float r2 = r1 - __half2float(b[1]);
-      b[2] = __float2half_rn(r2);
-    } else {
-      b[0] = __float2half_rn(-65504.f);
-      b[1] = b[2] = __float2half_rn(0.f);
-    }
-    // shared-memory layout of the K=16 no-swizzle block: core matrix = 8 rows x 16 bytes contiguous,
-    // 8-row groups 128 bytes apart, second K half TN*16 bytes further
-    const uint32_t t = row / TN, r = row % TN;
-    __half* blob = aug_blob + static_cast<size_t>(t) * (AUG_B_BYTES / 2);
-    for (int k = 0; k < 16; k++) {
-      int j = k >> 3, e = k & 7;
-      const uint32_t off = j * (TN * 16) + (r >> 3) * 128 + (r & 7) * 16;
-      blob[off / 2 + e] = k < 3 ? b[k] : __float2half_rn(0.f);
-    }
+    // bias: -(s^2 ||c - mu||^2 / 2) (L2; s = 2^k: exact; this order cannot overflow for tiny data), 0 (cosine)
+    write_bias_row(aug_blob, row, finite, (finite && metric != 1) ? -0.5f * ((s * __ldcg(csq + qrow)) * s) : 0.f);
   }
-}
-
-// one warp per centroid row (including the zero padding rows up to nt*256)
-__global__ void tc_prep_table_kernel(int metric, const float* __restrict__ C, const float* __restrict__ csq,
-                                     uint32_t K, int D, int nkb, int nt, __half* __restrict__ table,
-                                     __half* __restrict__ aug_blob, Stats* __restrict__ st,
-                                     const uint32_t* __restrict__ gather, const float* __restrict__ mu,
-                                     int by_source) {
-  const uint32_t row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (row >= static_cast<uint32_t>(nt) * TN) return;
-  prep_table_row(row, lane, st->scale, metric, C, csq, K, D, nkb, table, aug_blob, st, gather, mu, by_source);
 }
 
 // ---------------------------------------------------------------------------------------------------
 // The whole centroid preparation of one pass as ONE launch (Lloyd / Yinyang tables; the k-NN tables have their own
-// chain).  The chain above is ten stream operations (three memsets, ||c||^2, mean, mu, centred norms, maximum, scale,
-// table) of 3-12 us each on a 1 MB centroid matrix: ~0.05 ms of dependent launches per pass, 1 % of the step of an
-// 8M-row shard and 8 % of the step of a 1M-row shard (8 GPUs).  Here the same arithmetic (the device bodies are shared
-// with the chain, which stays as the KMB_PREP_FUSED=0 build) runs as four phases of one small grid separated by a
-// sense-reversing grid barrier; every CTA is resident (grid <= number of SMs, 256 threads, 38 KB static shared memory),
-// so the barrier cannot deadlock.  Values produced by other CTAs in an earlier phase are read with ld.global.cg.
+// kernels).  As separate kernels it would be ten stream operations (three memsets, ||c||^2, mean, mu, centred norms,
+// maximum, scale, table) of 3-12 us each on a 1 MB centroid matrix: ~0.05 ms of dependent launches per pass, 1 % of the
+// step of an 8M-row shard and 8 % of the step of a 1M-row shard (8 GPUs).  Here they run as four phases of one small
+// grid separated by a sense-reversing grid barrier; every CTA is resident (grid <= number of SMs, 256 threads, 38 KB
+// static shared memory), so the barrier cannot deadlock.  Values produced by other CTAs in an earlier phase are read
+// with ld.global.cg.
 // ---------------------------------------------------------------------------------------------------
 struct PrepArgs {
-  int metric, centred, D, nkb, by_source;
+  int metric, D, nkb, by_source;
   uint32_t K, rows_pad;
   const float* C;
   float* csq;            // reference-order ||c||^2 (L2) / 1 (cosine); written here when compute_csq
   int compute_csq;
-  float* cnorm2;         // L2 centred: ||c - mu||^2; cosine: upper bound of ||c||^2
+  float* cnorm2;         // L2: ||c - mu||^2; cosine: upper bound of ||c||^2
   double* musum;         // [D] + valid-row count
-  float* mu;             // [D]
   float* neg_mu_s;       // [nkb * KB]
   Stats* stats;
   uint32_t* counters;    // CNT_N words, zeroed here
@@ -535,7 +446,7 @@ tc_prep_fused_kernel(const PrepArgs a) {
   // ---- phase 0: zero the pass counters / statistics / column sums; ||c||^2 in the reference's order
   if (gt < CNT_N) a.counters[gt] = 0u;
   if (gt < sizeof(Stats) / 4) reinterpret_cast<uint32_t*>(a.stats)[gt] = 0u;
-  if (a.centred)
+  if (a.metric == 0)
     for (uint32_t i = gt; i < static_cast<uint32_t>(D) + 1u; i += nthr) a.musum[i] = 0.0;
   if (a.compute_csq) {
     float* tile = s_tile[warp];
@@ -577,7 +488,7 @@ tc_prep_fused_kernel(const PrepArgs a) {
 
   const float* nsq = a.csq;
   if (a.metric == 1) {
-    // ---- cosine: upper bound of ||c||^2 per centroid + its maximum (tc_prep_norms_kernel, tc_prep_stats_kernel)
+    // ---- cosine: upper bound of ||c||^2 per centroid + its maximum
     uint32_t best = 0;
     for (uint32_t row = gw; row < K; row += nw) {
       const float* src = a.C + static_cast<size_t>(row) * D;
@@ -594,8 +505,10 @@ tc_prep_fused_kernel(const PrepArgs a) {
     if (lane == 0 && best) atomicMax(&a.stats->csq_max_bits, best);
     nsq = a.cnorm2;
     prep_grid_barrier(a.barrier, gridDim.x);
-  } else if (a.centred) {
-    // ---- phase 1: column sums of the valid centroids (as tc_prep_mean_kernel: 128 features per half CTA)
+  } else {
+    // ---- L2, phase 1: the centring vector mu of the filter (see Params::neg_mu_s) is the mean of the valid centroids
+    // (rows whose ||c||^2 is finite).  ANY vector is a correct choice of mu (scores shift by a per-row constant); the
+    // mean minimises the operand norms.  Column sums, 128 features per half CTA
     {
       const int fb = (D + 127) / 128;
       const uint32_t nvb = static_cast<uint32_t>(fb) * ((K + 15u) / 16u);   // 16 rows per half CTA: two load groups deep
@@ -632,7 +545,6 @@ tc_prep_fused_kernel(const PrepArgs a) {
         const float m = nv ? static_cast<float>(__ldcg(a.musum + f) / nv) : 0.f;
         const float mm = (fabsf(m) < 3.0e38f) ? m : 0.f;
         s_mu[f] = mm;
-        if (blockIdx.x == 0) a.mu[f] = mm;
       }
       __syncthreads();
       uint32_t best = 0;
@@ -653,28 +565,13 @@ tc_prep_fused_kernel(const PrepArgs a) {
     }
     nsq = a.cnorm2;
     prep_grid_barrier(a.barrier, gridDim.x);
-  } else {
-    // ---- uncentred L2 (A/B switch): maximum of ||c||^2
-    uint32_t best = 0;
-    for (uint32_t c = gt; c < K; c += nthr) {
-      const float v = __ldcg(a.csq + c);
-      if (v == v && v < 3.0e38f) best = max(best, __float_as_uint(fmaxf(v, 0.f)));
-    }
-    for (int o = 16; o > 0; o >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, o));
-    if (lane == 0 && best) atomicMax(&a.stats->csq_max_bits, best);
-    prep_grid_barrier(a.barrier, gridDim.x);
   }
 
   // ---- phase 3: scale (every CTA derives it; CTA 0 publishes Stats and -mu*s), then the fp16 table + bias blocks
-  const bool have_mu = a.metric == 0 && a.centred;
+  const bool have_mu = a.metric == 0;
   if (warp == 0) {
-    float cmax = __fsqrt_ru(__uint_as_float(__ldcg(&a.stats->csq_max_bits)));
-    float s = 1.f;
-    if (cmax > 0.f && cmax < 3.0e38f) {
-      int e;
-      frexpf(cmax, &e);
-      s = ldexpf(1.f, 6 - e);
-    }
+    const float cmax = __fsqrt_ru(__uint_as_float(__ldcg(&a.stats->csq_max_bits)));
+    const float s = prep_scale(cmax);
     if (lane == 0) s_scale = s;
     if (blockIdx.x == 0) {
       const int Dp = a.nkb * KB;
@@ -688,6 +585,7 @@ tc_prep_fused_kernel(const PrepArgs a) {
       if (lane == 0) {
         a.stats->scale = s;
         a.stats->cmax = cmax * s * 1.001f;
+        // (1.002: the lane-partial sums are added in a different order than a serial loop)
         a.stats->mun = __fsqrt_ru(m2) * 1.002f;
       }
     }
@@ -955,14 +853,9 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   constexpr int nkb = NKB;
   // The error bound needs |x~| (the fp16-rounded operand row) and the rounding residual |a - x~|; the converters MEASURE
-  // both.  KMB_ANALYTIC_RESIDUAL=1 (A/B build) bounds them from |a|^2 alone in the streaming modes 0 and 3 -- round-to-
-  // nearest into fp16 moves a normal value by at most 2^-11 |a_i|, a subnormal one by at most 2^-25 -- which takes the
-  // back-conversion and the residual sums out of the converter's inner loop; the margin widens, so it is off.
-#if defined(KMB_ANALYTIC_RESIDUAL) && KMB_ANALYTIC_RESIDUAL
-  constexpr bool MEASURED_RESIDUAL = (MODE == 1 || MODE == 2);
-#else
+  // both.  (row_margin keeps the analytic bound from |a|^2 alone behind this constant: dropping that dead branch too
+  // changes ptxas's instruction schedule of tc_assign_kernel<1..8, 1>.)
   constexpr bool MEASURED_RESIDUAL = true;
-#endif
   [[maybe_unused]] const int nt = p.nt;
   const uint32_t n_eff = MODE == 1 ? min(*p.d_nrows, p.n) : p.n;
   constexpr uint32_t KNN_TPB = T64 ? 2u : 1u;   // MODE 2: query tiles per 128-row table block
@@ -1249,19 +1142,13 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
               ptx::unpack2(a01, a0, a1);
               ptx::unpack2(a23, a2_, a3);
               __half2 h0 = __floats2half2_rn(a0, a1), h1 = __floats2half2_rn(a2_, a3);
-              if (MEASURED_RESIDUAL) {
-                const float2 b0 = __half22float2(h0), b1 = __half22float2(h1);
-                const uint64_t b01 = ptx::pack2(b0.x, b0.y), b23 = ptx::pack2(b1.x, b1.y);
-                nx2 = ptx::ffma2(b01, b01, nx2);
-                nx2 = ptx::ffma2(b23, b23, nx2);
-                const uint64_t d01 = ptx::fsub2(a01, b01), d23 = ptx::fsub2(a23, b23);
-                nd2 = ptx::ffma2(d01, d01, nd2);
-                nd2 = ptx::ffma2(d23, d23, nd2);
-              } else {
-                // |a|^2 before the rounding: the epilogue bounds the rounded norm and the residual from it
-                nx2 = ptx::ffma2(a01, a01, nx2);
-                nx2 = ptx::ffma2(a23, a23, nx2);
-              }
+              const float2 b0 = __half22float2(h0), b1 = __half22float2(h1);
+              const uint64_t b01 = ptx::pack2(b0.x, b0.y), b23 = ptx::pack2(b1.x, b1.y);
+              nx2 = ptx::ffma2(b01, b01, nx2);
+              nx2 = ptx::ffma2(b23, b23, nx2);
+              const uint64_t d01 = ptx::fsub2(a01, b01), d23 = ptx::fsub2(a23, b23);
+              nd2 = ptx::ffma2(d01, d01, nd2);
+              nd2 = ptx::ffma2(d23, d23, nd2);
               if (MODE == 2) {   // compensated: this sum is subtracted from scores of the same magnitude
                 const float q4 = fmaf(a0, a0, fmaf(a1, a1, fmaf(a2_, a2_, a3 * a3)));
                 const float y = q4 - a2c, t = a2 + y;
@@ -1310,7 +1197,7 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
             }
             if (!T64 || hsel == 0) {
               norms[row] = nxl + nxh;
-              if (MEASURED_RESIDUAL) norms[TM + row] = ndl + ndh;
+              norms[TM + row] = ndl + ndh;
             }
             if (MODE == 2 && (!T64 || hsel == 0)) {
               norms[2 * TM + row] = a2;
@@ -1583,17 +1470,6 @@ tc_assign_body(const CUtensorMap& tmap_b, const Params& p) {
           // Lloyd / Yinyang candidate epilogue on the fragment as it lands: mask bit b = 2j + e of row hh (R0 / R1) is
           // acc[j*4 + hh*2 + e], column 8j + 2t + e of the n-tile.  Any fixed column order would do: the running row
           // maximum and the "within margin" bits do not depend on it, and the emitter decodes bits into columns.
-#ifdef KMB_DEBUG_SCORES   // bring-up builds only: 64 stores per n-tile bloat the hot loop's instruction footprint
-          if (MODE == 0 && !T64 && p.dbg_scores)
-            for (int hh = 0; hh < 2; hh++) {
-              const uint64_t grow = static_cast<uint64_t>(tile) * TM + qrow + 8 * hh;
-              float* dst = p.dbg_scores + grow * (static_cast<uint64_t>(nt) * TN) + n * TN + 2 * (lane & 3);
-              for (int j = 0; j < 16; j++) {
-                dst[8 * j] = acc[j * 4 + hh * 2];
-                dst[8 * j + 1] = acc[j * 4 + hh * 2 + 1];
-              }
-            }
-#endif
           if (it.seg_last()) si++;
 #if KMB_KO == 7
           if (MODE == 0) {   // timing build: the accumulators are loaded, the ALU work on them is skipped
@@ -2051,9 +1927,7 @@ struct TcPlan {
   tc::Stats* stats = nullptr;
   float* cnorm2 = nullptr;         // cosine: ||c||^2 (the reference's 'csqr' is the constant 1 there); L2: ||c - mu||^2
   double* musum = nullptr;         // [D] column sums of the valid centroids, followed by the valid-row count
-  float* mu = nullptr;             // [D] centring vector (L2), see Params::neg_mu_s
-  float* neg_mu_s = nullptr;       // [nkb*64]
-  bool centred = false;
+  float* neg_mu_s = nullptr;       // [nkb*64] centring term (L2), see Params::neg_mu_s
   bool inject_error = false;       // test hook (KMCUDA_B200_INJECT_PIPELINE_ERROR=1): report a timed-out barrier
   // Yinyang bounds refresh (MODE 3): group-sorted table layout, built once per run by tc_yy_layout()
   int nt3 = 0;
@@ -2073,7 +1947,6 @@ struct TcPlan {
   CUtensorMap tmap;     // fp16 centroid table
   int num_sms = 132;
   size_t smem_bytes = 0;
-  float* dbg_scores = nullptr;
   // CUDA-event pairs around the main kernel of the most recent passes (bench.py roofline)
   static constexpr int kEvRing = 64;
   cudaEvent_t ev0[kEvRing] = {}, ev1[kEvRing] = {};
@@ -2099,69 +1972,62 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// MODE 0, MODE 2 and the row list at NKB 9..16 (64-row tiles)
-template <bool ROWS, int MODE, int NKB>
-static void tc_launch_t64_one(unsigned grid, size_t smem, cudaStream_t st, const CUtensorMap& tb, const tc::Params& prm) {
-  if constexpr (ROWS) tc::tc_assign_rows_kernel<NKB><<<grid, tc::N_THREADS, smem, st>>>(tb, prm);
-  else tc::tc_assign_kernel<NKB, MODE><<<grid, tc::N_THREADS, smem, st>>>(tb, prm);
-}
-template <bool ROWS, int MODE = 0>
-static void tc_launch_t64(int nkb, unsigned grid, size_t smem, cudaStream_t st, const CUtensorMap& tb,
-                          const tc::Params& prm) {
-  switch (nkb) {
-    case 9: tc_launch_t64_one<ROWS, MODE, 9>(grid, smem, st, tb, prm); break;
-    case 10: tc_launch_t64_one<ROWS, MODE, 10>(grid, smem, st, tb, prm); break;
-    case 11: tc_launch_t64_one<ROWS, MODE, 11>(grid, smem, st, tb, prm); break;
-    case 12: tc_launch_t64_one<ROWS, MODE, 12>(grid, smem, st, tb, prm); break;
-    case 13: tc_launch_t64_one<ROWS, MODE, 13>(grid, smem, st, tb, prm); break;
-    case 14: tc_launch_t64_one<ROWS, MODE, 14>(grid, smem, st, tb, prm); break;
-    case 15: tc_launch_t64_one<ROWS, MODE, 15>(grid, smem, st, tb, prm); break;
-    default: tc_launch_t64_one<ROWS, MODE, 16>(grid, smem, st, tb, prm); break;
-  }
+// fp16 table [rows][nkb*64] as the B operand: boxes of 64 features x 128 rows, 128-byte swizzle
+static cudaError_t encode_table_map(CUtensorMap* map, const __half* table, size_t rows, int nkb) {
+  using namespace tc;
+  EncodeTiledFn enc = get_encode_fn();
+  if (!enc) return cudaErrorNotSupported;
+  cuuint64_t gdim[2] = {static_cast<cuuint64_t>(nkb * KB), static_cast<cuuint64_t>(rows)};
+  cuuint64_t gstride[1] = {static_cast<cuuint64_t>(nkb * KB) * sizeof(__half)};
+  cuuint32_t box[2] = {KB, TN};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult cr = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<__half*>(table), gdim, gstride, box, estr,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return cr == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
 }
 
+// The main kernels, tc_kernels[nkb - 1][MODE]: tc_assign_kernel<nkb, MODE> for MODE 0..3, then at [4] the row list
+// (tc_assign_rows_kernel<nkb>, MODE 0), for nkb 1..16
+typedef void (*TcKernel)(CUtensorMap, tc::Params);
+typedef std::array<TcKernel, 5> TcKernels;
+template <class F, int... I>
+static std::array<TcKernels, sizeof...(I)> table_over_nkb(F row, std::integer_sequence<int, I...>) {
+  return {row(std::integral_constant<int, I + 1>{})...};
+}
+static const auto tc_kernels = table_over_nkb([](auto nkb) {
+  return TcKernels{tc::tc_assign_kernel<decltype(nkb)::value, 0>, tc::tc_assign_kernel<decltype(nkb)::value, 1>,
+                   tc::tc_assign_kernel<decltype(nkb)::value, 2>, tc::tc_assign_kernel<decltype(nkb)::value, 3>,
+                   tc::tc_assign_rows_kernel<decltype(nkb)::value>};
+}, std::make_integer_sequence<int, tc::MAX_TILE64_NKB>{});
+
+// nkb lies in 1..16 for every plan (tc_supported) and k-NN call (tc_knn_supported)
+static void tc_launch(int mode, bool rows, int nkb, unsigned grid, size_t smem, cudaStream_t st, const CUtensorMap& tb,
+                      const tc::Params& prm) {
+  tc_kernels[nkb - 1][rows ? 4 : mode]<<<grid, tc::N_THREADS, smem, st>>>(tb, prm);
+}
+// every kernel a plan of this nkb may launch (MODE 0..3 and the row list) may use `bytes` of dynamic shared memory
+static cudaError_t tc_set_smem_attr(int bytes, int nkb) {
+  if (nkb < 1 || nkb > tc::MAX_TILE64_NKB) return cudaErrorInvalidValue;
+  for (int k = 0; k < 5; k++) {
+    const cudaError_t e =
+        cudaFuncSetAttribute(tc_kernels[nkb - 1][k], cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
+}
+
+// exact re-check of the queued (row, candidate) pairs in the metric of the run: MODE 0 Lloyd ranking score, MODE 1 true
+// distance (see recheck_pairs_kernel)
 template <int MODE>
-static void tc_launch_mode(int nkb, unsigned grid, size_t smem, cudaStream_t st, const CUtensorMap& tb,
-                           const tc::Params& prm) {
-  using namespace tc;
-  switch (nkb) {
-    case 1: tc_assign_kernel<1, MODE><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
-    case 2: tc_assign_kernel<2, MODE><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
-    case 3: tc_assign_kernel<3, MODE><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
-    case 4: tc_assign_kernel<4, MODE><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
-    case 5: tc_assign_kernel<5, MODE><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
-    case 6: tc_assign_kernel<6, MODE><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
-    case 7: tc_assign_kernel<7, MODE><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
-    default: tc_assign_kernel<8, MODE><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
-  }
+static void launch_recheck_pairs(int metric, unsigned grid, cudaStream_t st, const float* X, const float* C,
+                                 const float* csq, int D, const uint32_t* pair_row, const uint32_t* pair_cand,
+                                 const uint32_t* d_npairs, uint32_t max_pairs, uint32_t n, uint32_t K,
+                                 float* pair_score) {
+  (metric == 1 ? recheck_pairs_kernel<1, MODE> : recheck_pairs_kernel<0, MODE>)<<<grid, 128, 0, st>>>(
+      X, C, csq, D, pair_row, pair_cand, d_npairs, max_pairs, n, K, pair_score);
 }
-static void tc_launch_rows(int nkb, unsigned grid, size_t smem, cudaStream_t st, const CUtensorMap& tb,
-                           const tc::Params& prm) {
-  using namespace tc;
-  if (tile64(nkb)) return tc_launch_t64<true>(nkb, grid, smem, st, tb, prm);
-  switch (nkb) {
-    case 1: tc_assign_rows_kernel<1><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
-    case 2: tc_assign_rows_kernel<2><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
-    case 3: tc_assign_rows_kernel<3><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
-    case 4: tc_assign_rows_kernel<4><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
-    case 5: tc_assign_rows_kernel<5><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
-    case 6: tc_assign_rows_kernel<6><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
-    case 7: tc_assign_rows_kernel<7><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
-    default: tc_assign_rows_kernel<8><<<grid, N_THREADS, smem, st>>>(tb, prm); break;
-  }
-}
-static void tc_launch_main(int mode, int nkb, unsigned grid, size_t smem, cudaStream_t st, const CUtensorMap& tb,
-                           const tc::Params& prm) {
-  if (tc::tile64(nkb)) {
-    if (mode == 3) tc_launch_t64<false, 3>(nkb, grid, smem, st, tb, prm);
-    else if (mode == 2) tc_launch_t64<false, 2>(nkb, grid, smem, st, tb, prm);
-    else if (mode == 1) tc_launch_t64<false, 1>(nkb, grid, smem, st, tb, prm);
-    else tc_launch_t64<false, 0>(nkb, grid, smem, st, tb, prm);
-  } else if (mode == 3) tc_launch_mode<3>(nkb, grid, smem, st, tb, prm);
-  else if (mode == 2) tc_launch_mode<2>(nkb, grid, smem, st, tb, prm);
-  else if (mode == 1) tc_launch_mode<1>(nkb, grid, smem, st, tb, prm);
-  else tc_launch_mode<0>(nkb, grid, smem, st, tb, prm);
-}
+
 // (the pinned allocation below is milliseconds: a plan is created by every kmeans_cuda call, so freed blocks are
 // kept per process)
 static std::mutex g_pinned_mu;
@@ -2188,51 +2054,6 @@ static void pinned_counters_free(uint32_t* p) {
   g_pinned_free.push_back(p);
 }
 
-template <int NKB>
-static cudaError_t tc_set_smem_attr_one(int bytes) {
-  cudaError_t e = cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(tc::tc_assign_rows_kernel<NKB>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e != cudaSuccess) return e;
-  return cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-}
-template <int NKB>
-static cudaError_t tc_set_smem_attr_t64(int bytes) {
-  cudaError_t e = cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(tc::tc_assign_kernel<NKB, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e != cudaSuccess) return e;
-  return cudaFuncSetAttribute(tc::tc_assign_rows_kernel<NKB>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-}
-static cudaError_t tc_set_smem_attr(int bytes, int nkb) {   // only the instantiation this shape launches
-  switch (nkb) {
-    case 9: return tc_set_smem_attr_t64<9>(bytes);
-    case 10: return tc_set_smem_attr_t64<10>(bytes);
-    case 11: return tc_set_smem_attr_t64<11>(bytes);
-    case 12: return tc_set_smem_attr_t64<12>(bytes);
-    case 13: return tc_set_smem_attr_t64<13>(bytes);
-    case 14: return tc_set_smem_attr_t64<14>(bytes);
-    case 15: return tc_set_smem_attr_t64<15>(bytes);
-    case 16: return tc_set_smem_attr_t64<16>(bytes);
-    case 1: return tc_set_smem_attr_one<1>(bytes);
-    case 2: return tc_set_smem_attr_one<2>(bytes);
-    case 3: return tc_set_smem_attr_one<3>(bytes);
-    case 4: return tc_set_smem_attr_one<4>(bytes);
-    case 5: return tc_set_smem_attr_one<5>(bytes);
-    case 6: return tc_set_smem_attr_one<6>(bytes);
-    case 7: return tc_set_smem_attr_one<7>(bytes);
-    default: return tc_set_smem_attr_one<8>(bytes);
-  }
-}
-
 // every mode up to D = 1024 (512 < D <= 1024 on 64-row tiles; k-NN keeps its own checks in tc_knn_supported)
 bool tc_supported(int metric, uint32_t n, int D, uint32_t K) {
   if (D < 4 || D % 4 != 0 || D > tc::MAX_TILE64_NKB * tc::KB) return false;   // TMA row pitch must be 16-byte aligned
@@ -2248,7 +2069,6 @@ void tc_plan_destroy(TcPlan* p) {
   pool_free(p->stats);
   pool_free(p->cnorm2);
   pool_free(p->musum);
-  pool_free(p->mu);
   pool_free(p->neg_mu_s);
   pool_free(p->table3);
   pool_free(p->aug_blob3);
@@ -2263,7 +2083,6 @@ void tc_plan_destroy(TcPlan* p) {
   pool_free(p->ovf_rows);
   pool_free(p->counters);
   pool_free(p->prep_barrier);
-  pool_free(p->dbg_scores);
   pinned_counters_free(p->h_counters);
   for (int i = 0; i < TcPlan::kEvRing; i++) {
     if (p->ev0[i]) cudaEventDestroy(p->ev0[i]);
@@ -2292,11 +2111,8 @@ cudaError_t tc_plan_create(TcPlan** out, int metric, uint32_t max_n, int D, uint
   TC_TRY(pool_alloc(reinterpret_cast<void**>(&p->stats), sizeof(Stats)));
   TC_TRY(pool_alloc(reinterpret_cast<void**>(&p->cnorm2), sizeof(float) * K));
   TC_TRY(pool_alloc(reinterpret_cast<void**>(&p->musum), sizeof(double) * (D + 1)));
-  TC_TRY(pool_alloc(reinterpret_cast<void**>(&p->mu), sizeof(float) * D));
   TC_TRY(pool_alloc(reinterpret_cast<void**>(&p->neg_mu_s), sizeof(float) * mu_features(p->nkb)));
   {
-    const char* nc = getenv("KMCUDA_B200_NO_CENTER");   // A/B switch: uncentred operands (the round-1 filter)
-    p->centred = metric == 0 && !(nc && nc[0] == '1');
     const char* ie = getenv("KMCUDA_B200_INJECT_PIPELINE_ERROR");
     p->inject_error = ie && ie[0] == '1';
   }
@@ -2312,22 +2128,7 @@ cudaError_t tc_plan_create(TcPlan** out, int metric, uint32_t max_n, int D, uint
   p->h_counters = pinned_counters_alloc();
   if (!p->h_counters) { tc_plan_destroy(p); return cudaErrorMemoryAllocation; }
   memset(p->h_counters, 0, sizeof(uint32_t) * CNT_N);
-  const char* dbg = getenv("KMCUDA_B200_DUMP_SCORES");
-  if (dbg && dbg[0] == '1') {
-    size_t tiles = (static_cast<size_t>(max_n) + TM - 1) / TM;
-    TC_TRY(pool_alloc(reinterpret_cast<void**>(&p->dbg_scores), tiles * TM * rows_pad * sizeof(float)));
-  }
-  // tensor map over the fp16 centroid table [rows_pad][nkb*64], box 64 x 256, 128-byte swizzle
-  EncodeTiledFn enc = get_encode_fn();
-  if (!enc) { tc_plan_destroy(p); return cudaErrorNotSupported; }
-  cuuint64_t gdim[2] = {static_cast<cuuint64_t>(p->nkb * KB), static_cast<cuuint64_t>(rows_pad)};
-  cuuint64_t gstride[1] = {static_cast<cuuint64_t>(p->nkb * KB) * sizeof(__half)};
-  cuuint32_t box[2] = {KB, TN};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult cr = enc(&p->tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, p->table, gdim, gstride, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) { tc_plan_destroy(p); return cudaErrorInvalidValue; }
+  TC_TRY(encode_table_map(&p->tmap, p->table, rows_pad, p->nkb));
   for (int i = 0; i < TcPlan::kEvRing; i++) {
     TC_TRY(cudaEventCreate(&p->ev0[i]));
     TC_TRY(cudaEventCreate(&p->ev1[i]));
@@ -2343,74 +2144,37 @@ cudaError_t tc_plan_create(TcPlan** out, int metric, uint32_t max_n, int D, uint
 static cudaError_t tc_prepare(TcPlan* p, const float* C, const float* csq, uint32_t n, tc::Params* out,
                               cudaStream_t st, bool yy_layout = false, bool compute_csq = false) {
   using namespace tc;
-  cudaError_t e;
-#if KMB_PREP_FUSED
-  {
-    PrepArgs a;
-    a.metric = p->metric;
-    a.centred = p->centred ? 1 : 0;
-    a.D = p->D;
-    a.nkb = p->nkb;
-    a.by_source = yy_layout ? 1 : 0;
-    a.K = p->K;
-    a.rows_pad = static_cast<uint32_t>(yy_layout ? p->nt3 : p->nt) * TN;
-    a.C = C;
-    a.csq = const_cast<float*>(csq);
-    a.compute_csq = compute_csq ? 1 : 0;
-    a.cnorm2 = p->cnorm2;
-    a.musum = p->musum;
-    a.mu = p->mu;
-    a.neg_mu_s = p->neg_mu_s;
-    a.stats = p->stats;
-    a.counters = p->counters;
-    a.table = yy_layout ? p->table3 : p->table;
-    a.aug_blob = yy_layout ? p->aug_blob3 : p->aug_blob;
-    a.gather = yy_layout ? p->yy_perm : nullptr;
-    a.barrier = p->prep_barrier;
-    // one table row per warp up to the number of SMs (every CTA must be resident for the grid barrier)
-    const unsigned grid = std::min<unsigned>(static_cast<unsigned>(p->num_sms), std::max(1u, (a.rows_pad + 7u) / 8u));
-    tc_prep_fused_kernel<<<grid, 256, 0, st>>>(a);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  }
-#else
-  if (compute_csq && (e = kmb::launch_csqr(p->metric, C, p->K, p->D, const_cast<float*>(csq), st)) != cudaSuccess) return e;
-  if ((e = cudaMemsetAsync(p->counters, 0, sizeof(uint32_t) * CNT_N, st)) != cudaSuccess) return e;
-  if ((e = cudaMemsetAsync(p->stats, 0, sizeof(Stats), st)) != cudaSuccess) return e;
-  const float* nsq = csq;
-  const float* mu = nullptr;
-  if (p->metric == 1) {
-    tc_prep_norms_kernel<<<(p->K * 32 + 255) / 256, 256, 0, st>>>(C, p->K, p->D, p->cnorm2, nullptr, 1.0001f);
-    nsq = p->cnorm2;
-  } else if (p->centred) {
-    // L2: both operands are centred on the mean of the valid centroids (see Params::neg_mu_s)
-    if ((e = cudaMemsetAsync(p->musum, 0, sizeof(double) * (p->D + 1), st)) != cudaSuccess) return e;
-    uint32_t* nvalid = reinterpret_cast<uint32_t*>(p->musum + p->D);
-    tc_prep_mean_kernel<<<dim3((p->D + 127) / 128, (p->K + 63) / 64), 128, 0, st>>>(C, csq, p->K, p->D, p->musum, nvalid);
-    tc_prep_mu_kernel<<<(p->D + 127) / 128, 128, 0, st>>>(p->musum, nvalid, p->D, p->mu);
-    tc_prep_cnorm_kernel<<<(p->K * 32 + 255) / 256, 256, 0, st>>>(C, csq, p->mu, p->K, p->D, p->cnorm2);
-    nsq = p->cnorm2;
-    mu = p->mu;
-  }
-  tc_prep_stats_kernel<<<8, 256, 0, st>>>(nsq, p->K, p->stats);
-  tc_prep_scale_kernel<<<1, 32, 0, st>>>(p->stats, mu, p->D, p->nkb * KB, p->neg_mu_s);
-  const uint32_t rows_pad = static_cast<uint32_t>(p->nt) * TN;
-  if (!yy_layout)
-    tc_prep_table_kernel<<<(rows_pad * 32 + 255) / 256, 256, 0, st>>>(p->metric, C, nsq, p->K, p->D, p->nkb, p->nt, p->table,
-                                                                      p->aug_blob, p->stats, nullptr, mu, 0);
-  else
-    tc_prep_table_kernel<<<(static_cast<uint32_t>(p->nt3) * TN * 32 + 255) / 256, 256, 0, st>>>(
-        p->metric, C, nsq, p->K, p->D, p->nkb, p->nt3, p->table3, p->aug_blob3, p->stats, p->yy_perm, mu, 1);
-#endif
+  PrepArgs a;
+  a.metric = p->metric;
+  a.D = p->D;
+  a.nkb = p->nkb;
+  a.by_source = yy_layout ? 1 : 0;
+  a.K = p->K;
+  a.rows_pad = static_cast<uint32_t>(yy_layout ? p->nt3 : p->nt) * TN;
+  a.C = C;
+  a.csq = const_cast<float*>(csq);
+  a.compute_csq = compute_csq ? 1 : 0;
+  a.cnorm2 = p->cnorm2;
+  a.musum = p->musum;
+  a.neg_mu_s = p->neg_mu_s;
+  a.stats = p->stats;
+  a.counters = p->counters;
+  a.table = yy_layout ? p->table3 : p->table;
+  a.aug_blob = yy_layout ? p->aug_blob3 : p->aug_blob;
+  a.gather = yy_layout ? p->yy_perm : nullptr;
+  a.barrier = p->prep_barrier;
+  // one table row per warp up to the number of SMs (every CTA must be resident for the grid barrier)
+  const unsigned grid = std::min<unsigned>(static_cast<unsigned>(p->num_sms), std::max(1u, (a.rows_pad + 7u) / 8u));
+  tc_prep_fused_kernel<<<grid, 256, 0, st>>>(a);
   Params prm;
   prm.n = n;
   prm.D = p->D;
   prm.K = p->K;
   prm.nkb = p->nkb;
-  prm.nt = p->nt;
+  prm.nt = yy_layout ? p->nt3 : p->nt;
   prm.ntiles = (n + tile_rows(p->nkb) - 1) / tile_rows(p->nkb);
-  prm.aug_blob = p->aug_blob;
+  prm.aug_blob = yy_layout ? p->aug_blob3 : p->aug_blob;
   prm.stats = p->stats;
-  prm.result = nullptr;
   prm.pair_row = p->pair_row;
   prm.pair_cand = p->pair_cand;
   prm.max_pairs = p->max_pairs;
@@ -2419,30 +2183,6 @@ static cudaError_t tc_prepare(TcPlan* p, const float* C, const float* csq, uint3
   prm.counters = p->counters;
   prm.metric = p->metric;
   prm.neg_mu_s = p->neg_mu_s;
-  prm.assign = prm.prev = prm.d_changed = nullptr;
-  prm.yy_qgroup = prm.yy_groups = prm.yy_assign = nullptr;
-  prm.yy_bounds = nullptr;
-  prm.G = 0;
-  if (yy_layout) {
-    prm.nt = p->nt3;
-    prm.aug_blob = p->aug_blob3;
-  }
-  prm.X = nullptr;
-  prm.rows = nullptr;
-  prm.d_nrows = nullptr;
-  prm.d_ntiles = nullptr;
-  prm.tile_nrows = prm.blk_cluster = prm.knn_roff = prm.knn_rcount = prm.knn_nblk = nullptr;
-  prm.C = nullptr;
-  prm.knn_ranges = nullptr;
-  prm.kk = 0;
-  prm.knn_first_pass = 0;
-  prm.knn_stride = 0;
-  prm.knn_topk = prm.knn_dub = nullptr;
-  prm.knn_cnt = prm.knn_flags = nullptr;
-  prm.knn_entries = nullptr;
-  prm.knn_part = 0;
-  prm.knn_nparts = 1;
-  prm.dbg_scores = p->dbg_scores;
   *out = prm;
   return cudaGetLastError();
 }
@@ -2471,19 +2211,14 @@ cudaError_t tc_assign(TcPlan* p, const float* X, const float* C, const float* cs
     p->graph_slot = -1;
     cudaEventRecord(p->ev0[slot], st);
   }
-  tc_launch_main(0, p->nkb, grid, p->smem_bytes, st, p->tmap, prm);
+  tc_launch(0, false, p->nkb, grid, p->smem_bytes, st, p->tmap, prm);
   if (p->capturing) cudaEventRecordWithFlags(p->ev1[slot], st, cudaEventRecordExternal);
   else cudaEventRecord(p->ev1[slot], st);
   p->passes++;
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
   // exact re-check of the multi-candidate rows, then the rows that need the full exact pass
-  const unsigned rgrid = p->num_sms * 4;
-  if (p->metric == 1)
-    recheck_pairs_kernel<1, 0><<<rgrid, 128, 0, st>>>(X, C, csq, p->D, p->pair_row, p->pair_cand,
-                                                      p->counters + CNT_PAIRS, p->max_pairs, n, p->K, p->pair_score);
-  else
-    recheck_pairs_kernel<0, 0><<<rgrid, 128, 0, st>>>(X, C, csq, p->D, p->pair_row, p->pair_cand,
-                                                      p->counters + CNT_PAIRS, p->max_pairs, n, p->K, p->pair_score);
+  launch_recheck_pairs<0>(p->metric, p->num_sms * 4, st, X, C, csq, p->D, p->pair_row, p->pair_cand,
+                          p->counters + CNT_PAIRS, p->max_pairs, n, p->K, p->pair_score);
   recheck_reduce_kernel<<<p->num_sms * 2, 256, 0, st>>>(p->rowq, p->counters + CNT_ROWQ, p->pair_cand,
                                                         p->pair_score, result, assign, prev, d_changed);
   if ((e = launch_assign_exact(p->metric, X, C, csq, n, p->D, p->K, p->ovf_rows, p->counters + CNT_OVF, result,
@@ -2518,17 +2253,12 @@ cudaError_t tc_assign_rows(TcPlan* p, const float* X, uint32_t nX, const uint32_
   const int slot = static_cast<int>(p->passes % TcPlan::kEvRing);
   p->graph_slot = -1;
   cudaEventRecord(p->ev0[slot], st);
-  tc_launch_rows(p->nkb, grid, p->smem_bytes, st, p->tmap, prm);
+  tc_launch(0, true, p->nkb, grid, p->smem_bytes, st, p->tmap, prm);
   cudaEventRecord(p->ev1[slot], st);
   p->passes++;
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  const unsigned rgrid = p->num_sms * 4;
-  if (p->metric == 1)
-    recheck_pairs_kernel<1, 0><<<rgrid, 128, 0, st>>>(X, C, csq, p->D, p->pair_row, p->pair_cand,
-                                                      p->counters + CNT_PAIRS, p->max_pairs, nX, p->K, p->pair_score);
-  else
-    recheck_pairs_kernel<0, 0><<<rgrid, 128, 0, st>>>(X, C, csq, p->D, p->pair_row, p->pair_cand,
-                                                      p->counters + CNT_PAIRS, p->max_pairs, nX, p->K, p->pair_score);
+  launch_recheck_pairs<0>(p->metric, p->num_sms * 4, st, X, C, csq, p->D, p->pair_row, p->pair_cand,
+                          p->counters + CNT_PAIRS, p->max_pairs, nX, p->K, p->pair_score);
   recheck_reduce_kernel<<<p->num_sms * 2, 256, 0, st>>>(p->rowq, p->counters + CNT_ROWQ, p->pair_cand,
                                                         p->pair_score, result, nullptr, nullptr, nullptr);
   if ((e = launch_assign_exact(p->metric, X, C, csq, n, p->D, p->K, p->ovf_rows, p->counters + CNT_OVF, row_result,
@@ -2547,7 +2277,6 @@ cudaError_t tc_assign_rows(TcPlan* p, const float* X, uint32_t nX, const uint32_
 cudaError_t tc_yy_candidates(TcPlan* p, const float* X, const float* C, const float* csq, uint32_t n,
                              const uint32_t* rows, const uint32_t* d_nrows, cudaStream_t st) {
   using namespace tc;
-  if (!tc_yy_supported(p)) return cudaErrorNotSupported;
   if (n > p->max_n) return cudaErrorInvalidValue;
   if ((reinterpret_cast<uintptr_t>(X) & 15) || (reinterpret_cast<uintptr_t>(C) & 15)) return cudaErrorMisalignedAddress;
   cudaError_t e;
@@ -2557,7 +2286,7 @@ cudaError_t tc_yy_candidates(TcPlan* p, const float* X, const float* C, const fl
   prm.rows = rows;
   prm.d_nrows = d_nrows;
   const unsigned grid = min(static_cast<uint32_t>(p->num_sms), prm.ntiles);
-  tc_launch_main(1, p->nkb, grid, p->smem_bytes, st, p->tmap, prm);
+  tc_launch(1, false, p->nkb, grid, p->smem_bytes, st, p->tmap, prm);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
   if ((e = tc_exact_distances(p, X, C, n, p->pair_row, p->pair_cand, p->counters + CNT_PAIRS, p->max_pairs,
                               p->pair_score, st)) != cudaSuccess)
@@ -2569,13 +2298,8 @@ cudaError_t tc_yy_candidates(TcPlan* p, const float* X, const float* C, const fl
 cudaError_t tc_exact_distances(TcPlan* p, const float* X, const float* C, uint32_t n, const uint32_t* pair_row,
                                const uint32_t* pair_cand, const uint32_t* d_npairs, uint32_t max_pairs,
                                float* pair_score, cudaStream_t st) {
-  const unsigned rgrid = p->num_sms * 4;
-  if (p->metric == 1)
-    recheck_pairs_kernel<1, 1><<<rgrid, 128, 0, st>>>(X, C, nullptr, p->D, pair_row, pair_cand, d_npairs, max_pairs,
-                                                      n, p->K, pair_score);
-  else
-    recheck_pairs_kernel<0, 1><<<rgrid, 128, 0, st>>>(X, C, nullptr, p->D, pair_row, pair_cand, d_npairs, max_pairs,
-                                                      n, p->K, pair_score);
+  launch_recheck_pairs<1>(p->metric, p->num_sms * 4, st, X, C, nullptr, p->D, pair_row, pair_cand, d_npairs, max_pairs,
+                          n, p->K, pair_score);
   return cudaGetLastError();
 }
 
@@ -2692,7 +2416,6 @@ void tc_yy_layout_host(const uint32_t* host_groups, uint32_t K, uint32_t G, std:
 
 cudaError_t tc_yy_layout(TcPlan* p, const uint32_t* host_groups, uint32_t G) {
   using namespace tc;
-  if (!tc_yy_supported(p)) return cudaErrorNotSupported;
   std::vector<uint32_t> perm, qgroup, goff, gmem;
   int nt3 = 0;
   tc_yy_layout_host(host_groups, p->K, G, &perm, &qgroup, &goff, &gmem, &nt3);
@@ -2705,16 +2428,7 @@ cudaError_t tc_yy_layout(TcPlan* p, const uint32_t* host_groups, uint32_t G) {
     if ((e = pool_alloc(reinterpret_cast<void**>(&p->aug_blob3), static_cast<size_t>(nt3) * AUG_B_BYTES)) != cudaSuccess) return e;
     if ((e = pool_alloc(reinterpret_cast<void**>(&p->yy_perm), rows_pad * sizeof(uint32_t))) != cudaSuccess) return e;
     if ((e = pool_alloc(reinterpret_cast<void**>(&p->yy_qgroup), rows_pad / 4 * sizeof(uint32_t))) != cudaSuccess) return e;
-    EncodeTiledFn enc = get_encode_fn();
-    if (!enc) return cudaErrorNotSupported;
-    cuuint64_t gdim[2] = {static_cast<cuuint64_t>(p->nkb * KB), static_cast<cuuint64_t>(rows_pad)};
-    cuuint64_t gstride[1] = {static_cast<cuuint64_t>(p->nkb * KB) * sizeof(__half)};
-    cuuint32_t box[2] = {KB, TN};
-    cuuint32_t estr[2] = {1, 1};
-    if (enc(&p->tmap3, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, p->table3, gdim, gstride, box, estr,
-            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return cudaErrorInvalidValue;
+    if ((e = encode_table_map(&p->tmap3, p->table3, rows_pad, p->nkb)) != cudaSuccess) return e;
     p->nt3 = nt3;
   }
   if (G != p->G3 || !p->yy_goff) {
@@ -2733,8 +2447,6 @@ cudaError_t tc_yy_layout(TcPlan* p, const uint32_t* host_groups, uint32_t G) {
 }
 
 bool tc_yy_layout_ready(TcPlan* p, uint32_t G) { return p && p->table3 && p->G3 == G; }
-// the Yinyang local step (MODE 1) and bounds refresh (MODE 3) run on every plan (NKB 9..16 on 64-row tiles)
-bool tc_yy_supported(TcPlan* p) { return p != nullptr; }
 
 // One bounds refresh: bounds[row] = {ub exact, lb[g] valid lower bounds} (see Params, MODE 3).  Rows the filter
 // cannot bound are left on the overflow list (tc_queues) for the caller's exact row refresh.
@@ -2756,7 +2468,7 @@ cudaError_t tc_yy_refresh(TcPlan* p, const float* X, const float* C, const float
   prm.G = G;
   prm.X = X;
   const unsigned grid = min(static_cast<uint32_t>(p->num_sms), prm.ntiles);
-  tc_launch_main(3, p->nkb, grid, p->smem_bytes, st, p->tmap3, prm);
+  tc_launch(3, false, p->nkb, grid, p->smem_bytes, st, p->tmap3, prm);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
   // own group + upper bound, exactly: chunks of rows whose pairs fit the queue (yy_max_gsize members per row at most)
   const uint32_t per_row = max(1u, p->yy_max_gsize);
@@ -2807,18 +2519,6 @@ int tc_kernel_times(TcPlan* p, float* ms_out, int max_out) {
     ms_out[i] = ms;
   }
   return n;
-}
-const float* tc_debug_scores(TcPlan* p, size_t* row_stride) {
-  *row_stride = static_cast<size_t>(p->nt) * tc::TN;
-  return p->dbg_scores;
-}
-void tc_debug_stats(TcPlan* p, float* out4) {
-  tc::Stats st;
-  cudaMemcpy(&st, p->stats, sizeof(st), cudaMemcpyDeviceToHost);
-  out4[0] = st.scale;
-  out4[1] = st.cmax;
-  out4[2] = st.dcmax;
-  out4[3] = __builtin_bit_cast(float, st.csq_max_bits);
 }
 
 // ===================================================================================================
@@ -2956,23 +2656,7 @@ __global__ void prep_table_kernel(const float* __restrict__ X, const float* __re
   for (int o = 16; o > 0; o >>= 1) d2 += __shfl_xor_sync(0xffffffffu, d2, o);
   if (lane == 0) {
     if (finite) atomicMax(reinterpret_cast<uint32_t*>(&st->dcmax), __float_as_uint(__fsqrt_ru(d2) * 1.0001f));
-    __half b[3];
-    if (finite) {
-      const float hh = -0.5f * ((s * ysq[row]) * s);
-      b[0] = __float2half_rn(hh);
-      const float r1 = hh - __half2float(b[0]);
-      b[1] = __float2half_rn(r1);
-      b[2] = __float2half_rn(r1 - __half2float(b[1]));
-    } else {
-      b[0] = __float2half_rn(-65504.f);
-      b[1] = b[2] = __float2half_rn(0.f);
-    }
-    const uint32_t t = row / TN, r = row % TN;
-    __half* blob = aug_blob + static_cast<size_t>(t) * (AUG_B_BYTES / 2);
-    for (int k = 0; k < 16; k++) {
-      const int j = k >> 3, e = k & 7;
-      blob[(j * (TN * 16) + (r >> 3) * 128 + (r & 7) * 16) / 2 + e] = k < 3 ? b[k] : __float2half_rn(0.f);
-    }
+    write_bias_row(aug_blob, row, finite, finite ? -0.5f * ((s * ysq[row]) * s) : 0.f);
   }
 }
 
@@ -3231,8 +2915,6 @@ cudaError_t tc_knn_search(int metric, int k, const float* X, const float* C, uin
   using namespace tc;
   cudaError_t e = cudaSuccess;
   *h_error = 0;
-  EncodeTiledFn enc = get_encode_fn();
-  if (!enc) return cudaErrorNotSupported;
   int dev = 0, num_sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
@@ -3313,52 +2995,36 @@ cudaError_t tc_knn_search(int metric, int k, const float* X, const float* C, uin
   // fp16 table of the centred samples + bias blobs + statistics
   knn::prep_norms_kernel<<<(rows_max / 8) + 1, 256, 0, st>>>(X, C, D, tab2orig, blk_cluster, d_ntiles, ysq, yabs, metric);
   tc_prep_stats_kernel<<<8, 256, 0, st>>>(ysq, rows_max, stats);
-  tc_prep_scale_kernel<<<1, 32, 0, st>>>(stats, nullptr, 0, 0, nullptr);
+  tc_prep_scale_kernel<<<1, 1, 0, st>>>(stats);
   knn::prep_table_kernel<<<(rows_max / 8) + 1, 256, 0, st>>>(X, C, D, nkb, tab2orig, blk_cluster, d_ntiles, ysq, table,
                                                              blobs, stats, yabs, metric, d_err);
   KNN_TRY(cudaGetLastError());
-  {
-    cuuint64_t gdim[2] = {static_cast<cuuint64_t>(nkb * KB), static_cast<cuuint64_t>(rows_max)};
-    cuuint64_t gstride[1] = {static_cast<cuuint64_t>(nkb * KB) * sizeof(__half)};
-    cuuint32_t box[2] = {KB, TN};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult cr = enc(&tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, table, gdim, gstride, box, estr,
-                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) { e = cudaErrorInvalidValue; goto done; }
-  }
-  prm.n = N; prm.D = D; prm.K = K; prm.nkb = nkb; prm.nt = 0; prm.ntiles = 0;
-  prm.aug_blob = blobs; prm.stats = stats; prm.result = nullptr; prm.pair_row = nullptr; prm.pair_cand = nullptr;
-  prm.max_pairs = 0; prm.rowq = nullptr; prm.ovf_rows = nullptr; prm.counters = counters; prm.metric = 0;
-  prm.X = X; prm.rows = tab2orig; prm.d_nrows = nullptr; prm.d_ntiles = d_ntiles; prm.tile_nrows = t_nrows;
+  KNN_TRY(encode_table_map(&tmap, table, rows_max, nkb));
+  // (Params::metric stays 0: both metrics take the L2 candidate pass, the angular one on unit-length samples)
+  prm.n = N; prm.D = D; prm.K = K; prm.nkb = nkb;
+  prm.aug_blob = blobs; prm.stats = stats; prm.counters = counters;
+  prm.X = X; prm.rows = tab2orig; prm.d_ntiles = d_ntiles; prm.tile_nrows = t_nrows;
   prm.blk_cluster = blk_cluster; prm.C = C;
   prm.knn_ranges = ranges1; prm.knn_roff = roff1; prm.knn_rcount = rcount1; prm.knn_nblk = nblk1;
   prm.kk = kk; prm.knn_first_pass = 1; prm.knn_stride = stride; prm.knn_topk = topk;
   prm.knn_cnt = kcnt; prm.knn_flags = kflags; prm.knn_dub = dub; prm.knn_entries = entries;
-  prm.dbg_scores = nullptr;
-  prm.neg_mu_s = nullptr; prm.assign = prm.prev = prm.d_changed = nullptr;
-  prm.yy_qgroup = prm.yy_groups = prm.yy_assign = nullptr; prm.yy_bounds = nullptr; prm.G = 0;
   prm.knn_part = part; prm.knn_nparts = nparts ? nparts : 1;
-  tc_launch_main(2, nkb, grid, smem_bytes, st, tmap, prm);
+  tc_launch(2, false, nkb, grid, smem_bytes, st, tmap, prm);
   KNN_TRY(cudaGetLastError());
   (t64 ? knn::range_build_kernel<4> : knn::range_build_kernel<2>)<<<num_sms * 4, 256, 0, st>>>(d_ntiles, t_nrows, blk_cluster, blk_first, off, K, cd, radii, ysq,
                                                        dub, pool, pool_cap, pool_used, roff2, rcount2, nblk2, d_err,
                                                        d_pairs, part, prm.knn_nparts);
   KNN_TRY(cudaGetLastError());
   prm.knn_ranges = pool; prm.knn_roff = roff2; prm.knn_rcount = rcount2; prm.knn_nblk = nblk2; prm.knn_first_pass = 0;
-  tc_launch_main(2, nkb, grid, smem_bytes, st, tmap, prm);
+  tc_launch(2, false, nkb, grid, smem_bytes, st, tmap, prm);
   KNN_TRY(cudaGetLastError());
   (t64 ? knn::expand_kernel<4> : knn::expand_kernel<2>)<<<num_sms * 8, 256, 0, st>>>(d_ntiles, kk, stride, topk, kcnt, kflags, entries, tab2orig, pair_cap,
                                                   pair_row, pair_cand, rowq, fb_rows, counters, pool_used + 2, part,
                                                   prm.knn_nparts);
   KNN_TRY(cudaGetLastError());
   // the exact distance of every candidate pair in the CALLER's metric (angular: acos of the Kahan dot product)
-  if (metric == 1)
-    recheck_pairs_kernel<1, 1><<<num_sms * 4, 128, 0, st>>>(X, X, nullptr, D, pair_row, pair_cand, counters + CNT_PAIRS,
-                                                            pair_cap, N, N, pair_score);
-  else
-    recheck_pairs_kernel<0, 1><<<num_sms * 4, 128, 0, st>>>(X, X, nullptr, D, pair_row, pair_cand, counters + CNT_PAIRS,
-                                                            pair_cap, N, N, pair_score);
+  launch_recheck_pairs<1>(metric, num_sms * 4, st, X, X, nullptr, D, pair_row, pair_cand, counters + CNT_PAIRS,
+                          pair_cap, N, N, pair_score);
   knn::select_kernel<<<num_sms * 8, 256, 0, st>>>(k, rowq, counters, pair_cand, pair_score, 0u, neighbors);
   KNN_TRY(cudaGetLastError());
   KNN_TRY(cudaMemcpyAsync(h_cnt, counters, sizeof(uint32_t) * CNT_N, cudaMemcpyDeviceToHost, st));

@@ -679,9 +679,9 @@ KMCUDAResult Job::yinyang(float tolerance, uint32_t G) {
       uint32_t yc[4] = {0, 0, 0, 0}, rq = 0, ov = 0;
       cudaSetDevice(devs[0].dev);
       cudaMemcpy(yc, s0->yy_counters.get(), sizeof(yc), cudaMemcpyDeviceToHost);
-      if (s0->yy_tc()) tc_last_stats(s0->tc, &rq, &ov);
+      if (s0->tc) tc_last_stats(s0->tc, &rq, &ov);
       fprintf(stderr, "[kmcuda_b200 timing]   yy step (dev 0): tightened %u, passed %u, candidate rows %u, pairs %u, "
-              "reference-order scan rows %u\n", yc[0], yc[1], rq, s0->yy_tc() ? tc_last_pairs(s0->tc) : 0u, ov);
+              "reference-order scan rows %u\n", yc[0], yc[1], rq, s0->tc ? tc_last_pairs(s0->tc) : 0u, ov);
     }
   }
 }

@@ -344,9 +344,8 @@ struct TcQueues {
   const uint32_t* ovf_rows;   // rows the filter could not bound
   const uint32_t* d_novf;
 };
-// the plan also serves the Yinyang local step and bounds refresh (MODE 1 / 3), at every D it supports (512 < D <= 1024
-// on 64-row tiles)
-bool tc_yy_supported(TcPlan* plan);
+// every plan also serves the Yinyang local step and bounds refresh (MODE 1 / 3), at every D it supports
+// (512 < D <= 1024 on 64-row tiles)
 cudaError_t tc_yy_candidates(TcPlan* plan, const float* X, const float* C, const float* csq, uint32_t n,
                              const uint32_t* rows, const uint32_t* d_nrows, cudaStream_t st);
 cudaError_t tc_exact_distances(TcPlan* plan, const float* X, const float* C, uint32_t n, const uint32_t* pair_row,
@@ -386,8 +385,5 @@ uint32_t tc_last_error(TcPlan* plan);
 uint32_t tc_last_pairs(TcPlan* plan);
 void tc_set_capture(TcPlan* plan, bool on);   // the next tc_assign is recorded into a CUDA graph (stream capture)
 int tc_kernel_times(TcPlan* plan, float* ms_out, int max_out);
-// diagnostics (KMCUDA_B200_DUMP_SCORES=1): approximate scores [tiles*128][nt*256], prep statistics
-const float* tc_debug_scores(TcPlan* plan, size_t* row_stride);
-void tc_debug_stats(TcPlan* plan, float* out4);
 
 }  // namespace kmb

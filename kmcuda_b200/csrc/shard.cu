@@ -190,7 +190,7 @@ KMCUDAResult Shard::reset_update_state(cudaStream_t st) {
 KMCUDAResult Shard::yy_prepare(const uint32_t* host_groups, cudaStream_t st) {
   KMB_CU(launch_yy_group_sizes(groups, K, G, yy_gsize, st), kmcudaRuntimeError);
   const char* er = getenv("KMCUDA_B200_YY_EXACT_REFRESH");   // A/B and parity tests: exact SIMT refresh
-  if (yy_tc() && !force_exact && !(er && er[0] == '1'))
+  if (tc && !force_exact && !(er && er[0] == '1'))
     KMB_CU(tc_yy_layout(tc, host_groups, G), kmcudaMemoryAllocationFailure);
   return kmcudaSuccess;
 }
@@ -202,7 +202,7 @@ KMCUDAResult Shard::yy_refresh(uint32_t n, const float* X, const float* C, const
                                cudaStream_t st) {
   if (n > max_n) return kmcudaInvalidArguments;
   if (n == 0) return kmcudaSuccess;
-  if (yy_tc() && tc_yy_layout_ready(tc, G)) {
+  if (tc_yy_layout_ready(tc, G)) {
     KMB_CU(launch_csqr(metric, C, K, D, csq, st), kmcudaRuntimeError);
     KMB_CU(tc_yy_refresh(tc, X, C, csq, n, assignments, groups, G, bounds, st), kmcudaRuntimeError);
     TcQueues q;
@@ -220,9 +220,9 @@ KMCUDAResult Shard::yy_step(uint32_t n, const float* X, const float* C, uint32_t
                             uint32_t* d_changed, cudaStream_t st) {
   if (n > max_n) return kmcudaInvalidArguments;
   KMB_CU(launch_yy_drifts(metric, C, oldC, K, D, G, groups, drift, maxdrift, st), kmcudaRuntimeError);
-  if (yy_tc()) KMB_CU(launch_csqr(metric, C, K, D, csq, st), kmcudaRuntimeError);
+  if (tc) KMB_CU(launch_csqr(metric, C, K, D, csq, st), kmcudaRuntimeError);
   YyWorkspace ws{yy_minlb, yy_tight_rows, yy_tight_cand, yy_tight_score, passed, yy_gsize, yy_counters};
-  KMB_CU(launch_yy_step(metric, yy_tc(), X, C, csq, n, D, K, G, groups, drift, maxdrift, assignments, prev, bounds, ws,
+  KMB_CU(launch_yy_step(metric, tc, X, C, csq, n, D, K, G, groups, drift, maxdrift, assignments, prev, bounds, ws,
                         d_changed, force_exact, st), kmcudaRuntimeError);
   return kmcudaSuccess;
 }
@@ -444,15 +444,6 @@ uint32_t kmcuda_b200_debug_last_error(kmcuda_b200_shard* shard) {
   if (!shard || !shard->impl->tc) return 0;
   return kmb::tc_last_error(shard->impl->tc);
 }
-// copies rows x cols of the dumped approximate scores (KMCUDA_B200_DUMP_SCORES=1) to host memory
-int32_t kmcuda_b200_debug_scores(kmcuda_b200_shard* shard, float* host_out, uint32_t rows, uint32_t cols) {
-  if (!shard || !shard->impl->tc) return -1;
-  size_t stride = 0;
-  const float* src = kmb::tc_debug_scores(shard->impl->tc, &stride);
-  if (!src || cols > stride) return -2;
-  return cudaMemcpy2D(host_out, cols * sizeof(float), src, stride * sizeof(float), cols * sizeof(float), rows,
-                      cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -3;
-}
 // device time (ms) of the tensor-core kernel in the most recent passes (CUDA events on the launching
 // stream), oldest first; returns how many were written.  Call after synchronising the stream.
 int32_t kmcuda_b200_kernel_times(kmcuda_b200_shard* shard, float* ms_out, int32_t max_out) {
@@ -471,7 +462,7 @@ int32_t kmcuda_b200_debug_yy_bounds(kmcuda_b200_shard* shard, uint32_t n, const 
   if (cudaMemcpy(s->groups.get(), host_groups, sizeof(uint32_t) * s->K, cudaMemcpyHostToDevice) != cudaSuccess) return -4;
   cudaStream_t st = nullptr;
   if (use_tc) {
-    if (!s->yy_tc()) return -5;
+    if (!s->tc) return -5;
     if (kmb::tc_yy_layout(s->tc, host_groups, G) != cudaSuccess) return -6;
     if (s->yy_refresh(n, samples, centroids, assignments, st) != kmcudaSuccess) return -7;
   } else {
@@ -493,11 +484,6 @@ int32_t kmcuda_b200_debug_assign_rows(kmcuda_b200_shard* shard, uint32_t n, cons
   if (!shard || !samples || !rows || !centroids || !row_scratch || !result) return -1;
   return shard->impl->assign_rows(n, samples, samples_size, rows, centroids, row_scratch, result,
                                   static_cast<cudaStream_t>(stream)) == kmcudaSuccess ? 0 : -2;
-}
-int32_t kmcuda_b200_debug_stats(kmcuda_b200_shard* shard, float* out4) {
-  if (!shard || !shard->impl->tc) return -1;
-  kmb::tc_debug_stats(shard->impl->tc, out4);
-  return 0;
 }
 
 // host layout of the Yinyang refresh table (assign_tc.cu::tc_yy_layout_host) for tests: perm_out [cap], qgroup_out

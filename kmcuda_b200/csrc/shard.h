@@ -170,9 +170,7 @@ class Shard {
   DevBuf<float> ws_partial_w;   // weighted update only, allocated on first use
   DevBuf<float> prev_sums;   // cosine update: member sums of the previous iteration
   DevBuf<char> ws_cub;
-  TcPlan* tc = nullptr;
-  // the plan of the Yinyang local step and bounds refresh: nullptr (exact kernels) when the plan does not serve them
-  TcPlan* yy_tc() const { return tc_yy_supported(tc) ? tc : nullptr; }
+  TcPlan* tc = nullptr;   // the tensor-core passes (Lloyd, Yinyang, mini-batch); nullptr: the exact kernels
 
   // Yinyang state (per shard)
   uint32_t G = 0;

@@ -43,20 +43,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t addr, uint32_t parity, ui
       : "memory");
   return done != 0;
 }
-#ifndef KMB_WAIT_HINT_NS
-#define KMB_WAIT_HINT_NS 2000   // 0 = A/B build: plain polling without a suspend hint
-#endif
-__device__ __forceinline__ bool mbar_try_wait_nohint(uint32_t addr, uint32_t parity) {
-  uint32_t done;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(done)
-      : "r"(addr), "r"(parity)
-      : "memory");
-  return done != 0;
-}
+constexpr uint32_t WAIT_HINT_NS = 2000;   // suspend-time hint of the first probe of every wait
 // Remainder of every wait: a tight polling loop (a hinted try_wait returns on every update of the barrier, not only
 // when the phase flips, so the error word and the clock are checked only every 1024 probes).  Inlined: under setmaxnreg,
 // ptxas cannot allocate a call made while wgmma accumulators are in flight.
@@ -78,11 +65,7 @@ __device__ __forceinline__ void mbar_wait_slow(uint32_t addr, uint32_t parity, u
         "{\n\t.reg .pred p, q;\n\t.reg .b32 c;\n\t"
         "mov.u32 c, 0;\n"
         "KMB_WAIT_LOOP_%=:\n\t"
-#if KMB_WAIT_HINT_NS > 0
         "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-#else
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-#endif
         "@p bra KMB_WAIT_DONE_%=;\n\t"
         "add.u32 c, c, 1;\n\t"
         "setp.lt.u32 q, c, 1024;\n\t"
@@ -104,11 +87,7 @@ __device__ __forceinline__ void mbar_wait_slow(uint32_t addr, uint32_t parity, u
 }
 // The inline part: one probe (with the suspend hint it may sleep up to the hint while the phase has not flipped).
 __device__ __forceinline__ void mbar_wait(uint32_t addr, uint32_t parity, uint32_t* err, uint32_t site, uint32_t flag_u32) {
-#if KMB_WAIT_HINT_NS > 0
-  if (!mbar_try_wait(addr, parity, KMB_WAIT_HINT_NS)) mbar_wait_slow(addr, parity, err, site, flag_u32);
-#else
-  if (!mbar_try_wait_nohint(addr, parity)) mbar_wait_slow(addr, parity, err, site, flag_u32);
-#endif
+  if (!mbar_try_wait(addr, parity, WAIT_HINT_NS)) mbar_wait_slow(addr, parity, err, site, flag_u32);
 }
 
 // ---------------------------------------------------------------------------- fp32 pairs

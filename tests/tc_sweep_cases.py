@@ -178,7 +178,7 @@ def list_case(kind, D, metric="L2", seed=0):
 
 def margins(X, C, metric="L2"):
     """per-row margin (2 E 1.001, score units) and scale s of the MODE 0 filter (centred for L2; the converters measure
-    |x~| and the rounding residual, as the kernel does unless built with KMB_ANALYTIC_RESIDUAL=1)"""
+    |x~| and the rounding residual, as the kernel does)"""
     _, E, s, _ = _filter_model(X, C, centred=(metric == "L2"), residual="measured")
     return (2.0 * E * 1.001 + 1e-30).astype(np.float32), s
 
