@@ -143,6 +143,38 @@ KMCUDAResult kmcuda_b200_kmeans_restarts(KMCUDAInitMethod init, const void *init
                                          float *centroids, uint32_t *assignments, float *average_distance,
                                          double *inertia /* NULL = not wanted */);
 
+/* Bisecting k-means, scikit-learn's BisectingKMeans: the K clusters are made by splitting one cluster in two at a time
+ * with a 2-means run inside it, on one GPU (device: a mask of at most one bit, 0 = the first GPU), L2 only.  The
+ * parameters up to `weights` are those of kmcuda_b200_kmeans_minibatch().  strategy 0 splits the leaf of largest
+ * inertia sum w e, strategy 1 the leaf of most rows (scikit-learn's bisecting_strategy "biggest_inertia" and
+ * "largest_cluster"); equal scores take the leaf that comes first in the tree's depth-first, left-first order, which
+ * is also the order of the output clusters.  Each bisection runs n_init inits (kmcudaInitMethodRandom: the two rows of
+ * positive weight of smallest -ln(u) / w; kmcudaInitMethodGreedyPlusPlus, init_params a uint32_t number of trials L,
+ * 0 or NULL = 2: centre 0 the row of smallest -ln(u) / w, centre 1 the best of L d^2-sampled trial rows by the
+ * potential they leave, greedy k-means++ restricted to the node) with at most max_iter (0 = 300) Lloyd iterations, and
+ * keeps the first init
+ * whose inertia no later one beats by more than a factor 1 - 1e-6.  A 2-means run stops when its labels repeat or when
+ * sum ||dc||^2 <= tolerance * (the mean of the unweighted per-feature variances of the samples), scikit-learn's KMeans
+ * scaling (BisectingKMeans passes its tol unscaled).  A child left without weight takes the farthest row of positive
+ * weight of the other child.  The draws depend on (seed, node, init) only and every double total is added in a fixed
+ * order, so the result depends on no launch shape; with every weight 1 it is bit-identical to weights == NULL.
+ * *inertia (if not NULL) is sum w ||x - c||^2 of the result, average_distance as for kmeans_cuda().  Verbosity >= 1 logs
+ * one "bisecting: split" line per split in pick order and a final line with the waves, the nodes bisected and the
+ * inertia; verbosity >= 2 one line per (node, init) with its iterations, stop reason and inertia.
+ * kmcudaInvalidArguments: the cosine metric, more than one device, strategy not 0 or 1, n_init == 0, an init other
+ * than kmcudaInitMethodRandom or kmcudaInitMethodGreedyPlusPlus (at most 32 trials), KMCUDA_B200_STRICT_UPDATE=1, a
+ * non-finite sample, data from which fewer than K clusters can be made (too few distinct rows of positive weight), an
+ * n_init * K too large for the 32-bit segment indices, and everything kmeans_cuda() rejects. */
+KMCUDAResult kmcuda_b200_kmeans_bisecting(KMCUDAInitMethod init, const void *init_params, float tolerance,
+                                          KMCUDADistanceMetric metric, uint32_t samples_size, uint16_t features_size,
+                                          uint32_t clusters_size, uint32_t seed, uint32_t device, int32_t device_ptrs,
+                                          int32_t fp16x2, int32_t verbosity, const float *samples,
+                                          const float *weights /* NULL = unweighted */,
+                                          int32_t strategy /* 0 = biggest inertia, 1 = largest cluster */,
+                                          uint32_t n_init, uint32_t max_iter /* 0 = 300 */, float *centroids,
+                                          uint32_t *assignments, float *average_distance,
+                                          double *inertia /* NULL = not wanted */);
+
 /* Creates the per-shard workspace (fp16 centroid table, TMA descriptors, re-check queues, sort
  * buffers) for up to max_samples samples of features_size fp32 features and clusters_size clusters. */
 KMCUDAResult kmcuda_b200_shard_create(kmcuda_b200_shard **shard, KMCUDADistanceMetric metric,

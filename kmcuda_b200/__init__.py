@@ -7,7 +7,8 @@ Python surface = the reference's `libKMCUDA` module (reference src/python.cc:33-
                 sample_weight=None,                                           # extension: per-sample weights
                 batch_size=None, max_steps=0,                                 # extension: mini-batch k-means
                 relocate_empty_clusters=False,                                # extension: scikit-learn's relocation
-                n_init=1, inertia=False)                                      # extension: restarts, inertia
+                n_init=1, inertia=False,                                      # extension: restarts, inertia
+                bisecting=None, max_iter=0)                                   # extension: bisecting k-means
                 init="k-means||" / ("k-means||", rounds)                      # extension: k-means|| seeding
     knn_cuda(k, samples, centroids, assignments, metric="L2", device=0, verbosity=0)  # python.cc:412-632
     supports_fp16                                                             # python.cc:52
@@ -50,6 +51,10 @@ _lib.kmcuda_b200_kmeans_minibatch.argtypes = _lib.kmeans_cuda.argtypes[:3] + _li
 _lib.kmcuda_b200_kmeans_restarts.restype = ctypes.c_int
 _lib.kmcuda_b200_kmeans_restarts.argtypes = _lib.kmeans_cuda.argtypes[:14] + \
     [ctypes.c_void_p, ctypes.c_int32, ctypes.c_uint32] + _lib.kmeans_cuda.argtypes[14:] + [ctypes.c_void_p]
+_lib.kmcuda_b200_kmeans_bisecting.restype = ctypes.c_int
+_lib.kmcuda_b200_kmeans_bisecting.argtypes = _lib.kmcuda_b200_kmeans_minibatch.argtypes[:13] + \
+    [ctypes.c_void_p, ctypes.c_int32, ctypes.c_uint32, ctypes.c_uint32] + _lib.kmeans_cuda.argtypes[14:] + \
+    [ctypes.c_void_p]
 _lib.knn_cuda.restype = ctypes.c_int
 _lib.knn_cuda.argtypes = [
     ctypes.c_uint16, ctypes.c_int, ctypes.c_uint32, ctypes.c_uint16, ctypes.c_uint32, ctypes.c_uint32,
@@ -66,6 +71,7 @@ KMEANS_PARALLEL_MAX_ROUNDS = 32
 INIT_GREEDY_PLUSPLUS = 5   # include/kmcuda_b200.h: kmcudaInitMethodGreedyPlusPlus
 GREEDY_PLUSPLUS_MAX_TRIALS = 32
 METRIC_L2, METRIC_COSINE = range(2)
+BISECTING_STRATEGIES = {"biggest_inertia": 0, "largest_cluster": 1}   # kmcuda_b200_kmeans_bisecting's strategy
 
 _INIT_METHODS = {"kmeans++": INIT_PLUSPLUS, "k-means++": INIT_PLUSPLUS, "afkmc2": INIT_AFKMC2,
                  "afk-mc2": INIT_AFKMC2, "random": INIT_RANDOM, "k-means||": INIT_KMEANS_PARALLEL,
@@ -177,7 +183,7 @@ def _raise_for(result, fn):
 
 def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1, metric="L2",
                 average_distance=False, seed=None, device=0, verbosity=0, sample_weight=None, batch_size=None,
-                max_steps=0, relocate_empty_clusters=False, n_init=1, inertia=False):
+                max_steps=0, relocate_empty_clusters=False, n_init=1, inertia=False, bisecting=None, max_iter=0):
     """K-means on the GPU(s); see the module docstring.  Returns (centroids, assignments[, avg_distance][, inertia]).
 
     sample_weight: one non-negative weight per sample (include/kmcuda_b200.h, kmcuda_b200_kmeans_weighted), a 1-D
@@ -197,7 +203,29 @@ def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1
     restart would be the same run) nor with batch_size.
 
     inertia: True appends the returned run's inertia, sum w * ||x - c||^2 (angular: w * angle^2) as a float, to the
-    result; not with batch_size."""
+    result; not with batch_size.
+
+    bisecting: "biggest_inertia" or "largest_cluster" runs bisecting k-means (kmcuda_b200_kmeans_bisecting,
+    scikit-learn's BisectingKMeans with that bisecting_strategy) on one GPU, L2 only, with init "random",
+    "greedy-k-means++" or ("greedy-k-means++", L) (L = 0: 2 trials, scikit-learn's 2 + floor(ln 2)); n_init is then
+    the number of inits per bisection and max_iter (0 = 300) the Lloyd iterations per 2-means run; yinyang_t is
+    ignored.  Not with batch_size, max_steps or relocate_empty_clusters.  None = the other routes."""
+    if bisecting is not None:
+        if not isinstance(bisecting, str):
+            raise TypeError("\"bisecting\" must be None or a string, got %r" % (bisecting,))
+        if bisecting not in BISECTING_STRATEGIES:
+            raise ValueError("\"bisecting\" must be \"biggest_inertia\" or \"largest_cluster\", got %r" % (bisecting,))
+        if batch_size is not None or max_steps or relocate_empty_clusters:
+            raise ValueError("\"bisecting\" cannot be combined with \"batch_size\", \"max_steps\" or "
+                             "\"relocate_empty_clusters\"")
+        name = init[0] if isinstance(init, tuple) and len(init) > 0 else init
+        if not (isinstance(name, str) and _INIT_METHODS.get(name) in (INIT_RANDOM, INIT_GREEDY_PLUSPLUS)) or \
+                (isinstance(init, tuple) and _INIT_METHODS[name] == INIT_RANDOM):
+            raise ValueError("\"bisecting\" takes init=\"random\", \"greedy-k-means++\" or (\"greedy-k-means++\", L), "
+                             "got %r" % (init,))
+    max_iter = _count(max_iter, "max_iter", 0)
+    if max_iter and bisecting is None:
+        raise ValueError("\"max_iter\" applies to bisecting runs only: pass \"bisecting\" too")
     if not isinstance(relocate_empty_clusters, (bool, np.bool_)):
         raise TypeError("\"relocate_empty_clusters\" must be a bool, got %r" % (relocate_empty_clusters,))
     relocate_empty_clusters = bool(relocate_empty_clusters)
@@ -302,7 +330,13 @@ def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1
     common = (init_method, ctypes.byref(afkmc2_m), tolerance, yinyang_t, metric_id, n, d, clusters,
               int(seed) & 0xFFFFFFFF, int(device), device_ptrs, int(fp16x2), int(verbosity), samples_ptr)
     outputs = (centroids_ptr, assignments_ptr, ctypes.byref(avg) if average_distance else None)
-    if n_init != 1 or inertia:
+    if bisecting is not None:
+        if yinyang_t and verbosity > 0:
+            print("bisecting k-means: yinyang_t is ignored", flush=True)
+        result = _lib.kmcuda_b200_kmeans_bisecting(*common[:3], *common[4:], weights_ptr,
+                                                   BISECTING_STRATEGIES[bisecting], n_init, max_iter, *outputs,
+                                                   ctypes.byref(inertia_value) if inertia else None)
+    elif n_init != 1 or inertia:
         result = _lib.kmcuda_b200_kmeans_restarts(*common, weights_ptr, int(relocate_empty_clusters), n_init, *outputs,
                                                   ctypes.byref(inertia_value) if inertia else None)
     elif batch_size is not None:

@@ -21,7 +21,7 @@ LIB = os.path.join(HERE, "libKMCUDA.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
 CU_SOURCES = ["simt_kernels.cu", "knn_kernels.cu", "assign_tc.cu", "yinyang.cu", "shard.cu", "exchange.cu",
-              "kmeans_parallel.cu", "greedy_plusplus.cu", "minibatch.cu", "relocate.cu", "transfer.cu", "job.cu", "seeding.cu",
+              "kmeans_parallel.cu", "greedy_plusplus.cu", "minibatch.cu", "bisecting.cu", "relocate.cu", "transfer.cu", "job.cu", "seeding.cu",
               "knn_driver.cu", "api.cu"]
 CC_SOURCES = ["py_module.cc"]
 

@@ -63,7 +63,7 @@ static KMCUDAResult print_memory_stats(const std::vector<int>& devs) {
 
 using namespace kmb;
 
-// kmeans_cuda, kmcuda_b200_kmeans_weighted, _relocate, _minibatch and _restarts (weights == nullptr: the unweighted run)
+// kmeans_cuda, kmcuda_b200_kmeans_weighted, _relocate, _minibatch, _restarts and _bisecting (weights == nullptr: the unweighted run)
 static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, float tolerance,
                                 float yinyang_t, KMCUDADistanceMetric metric, uint32_t samples_size,
                                 uint16_t features_size, uint32_t clusters_size, uint32_t seed,
@@ -71,7 +71,8 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
                                 const float* samples, const float* weights, float* centroids,
                                 uint32_t* assignments, float* average_distance, bool minibatch = false,
                                 uint32_t batch_size = 0, uint32_t max_steps = 0, bool relocate = false,
-                                uint32_t n_init = 1, double* inertia = nullptr) {
+                                uint32_t n_init = 1, double* inertia = nullptr, bool bisecting = false,
+                                int32_t strategy = 0, uint32_t max_iter = 0) {
   KMB_DEBUG("arguments: %d %p %.3f %.2f %d %" PRIu32 " %" PRIu16 " %" PRIu32 " %" PRIu32 " %" PRIu32
             " %d %" PRIi32 " %p %p %p %p\n", init, init_params, tolerance, yinyang_t, metric, samples_size,
             features_size, clusters_size, seed, device, fp16x2, verbosity, samples, centroids, assignments,
@@ -103,6 +104,18 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
     if (batch_size == 0 || metric == kmcudaDistanceMetricCosine || (device & (device - 1)) != 0 ||
         (su && su[0] == '1')) {
       KMB_INFO("mini-batch k-means takes batch_size >= 1, the L2 metric, one device and no strict update mode\n");
+      return kmcudaInvalidArguments;
+    }
+    if (device == 0) device = 1;
+  }
+  if (bisecting) {
+    // one GPU, L2; the 2-means runs start from a random or greedy k-means++ pair; strict mode replays a Lloyd update
+    // that bisection does not have
+    const char* su = getenv("KMCUDA_B200_STRICT_UPDATE");
+    if (metric == kmcudaDistanceMetricCosine || (device & (device - 1)) != 0 || (strategy != 0 && strategy != 1) ||
+        (init != kmcudaInitMethodRandom && init != kmcudaInitMethodGreedyPlusPlus) || (su && su[0] == '1')) {
+      KMB_INFO("bisecting k-means takes the L2 metric, one device, strategy 0 or 1, the random or greedy k-means++ "
+               "init and no strict update mode\n");
       return kmcudaInvalidArguments;
     }
     if (device == 0) device = 1;
@@ -152,7 +165,15 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
     g_prof.mark("weight check");
   }
   if (verbosity > 1) KMB_RET(print_memory_stats(dev_ids));
-  if (minibatch) {
+  if (bisecting) {
+    // greedy k-means++: 0 trials = scikit-learn's 2 + floor(ln 2) for the two centres of a bisection
+    uint32_t trials = 0;
+    if (init == kmcudaInitMethodGreedyPlusPlus) {
+      trials = init_params ? *static_cast<const uint32_t*>(init_params) : 0;
+      if (trials == 0) trials = 2 + static_cast<uint32_t>(std::log(2.0));
+    }
+    KMB_RET(job.bisecting(seed, tolerance, strategy, n_init, max_iter, trials, inertia));
+  } else if (minibatch) {
     KMB_RET(job.init_centroids(init, init_params, seed, device_ptrs, fp16x2 != 0, centroids));
     g_prof.mark("init centroids");
     KMB_RET(job.minibatch(batch_size, max_steps, tolerance, seed));
@@ -236,6 +257,18 @@ KMCUDAResult kmcuda_b200_kmeans_restarts(KMCUDAInitMethod init, const void* init
   return kmeans_impl(init, init_params, tolerance, yinyang_t, metric, samples_size, features_size, clusters_size, seed,
                      device, device_ptrs, fp16x2, verbosity, samples, weights, centroids, assignments,
                      average_distance, false, 0, 0, relocate_empty_clusters != 0, n_init, inertia);
+}
+
+KMCUDAResult kmcuda_b200_kmeans_bisecting(KMCUDAInitMethod init, const void* init_params, float tolerance,
+                                          KMCUDADistanceMetric metric, uint32_t samples_size,
+                                          uint16_t features_size, uint32_t clusters_size, uint32_t seed,
+                                          uint32_t device, int32_t device_ptrs, int32_t fp16x2, int32_t verbosity,
+                                          const float* samples, const float* weights, int32_t strategy,
+                                          uint32_t n_init, uint32_t max_iter, float* centroids,
+                                          uint32_t* assignments, float* average_distance, double* inertia) {
+  return kmeans_impl(init, init_params, tolerance, 0.f, metric, samples_size, features_size, clusters_size, seed,
+                     device, device_ptrs, fp16x2, verbosity, samples, weights, centroids, assignments,
+                     average_distance, false, 0, 0, false, n_init, inertia, true, strategy, max_iter);
 }
 
 KMCUDAResult knn_cuda(uint16_t k, KMCUDADistanceMetric metric, uint32_t samples_size,

@@ -9,6 +9,7 @@
 #include <dlfcn.h>
 
 #include <map>
+#include <set>
 
 #include "job.h"
 
@@ -932,6 +933,323 @@ KMCUDAResult Job::average_distance(float* out) {
   double sum = 0;
   for (double part : parts) sum += part;
   *out = static_cast<float>(sum / (weighted ? wtotal : N));   // weighted: sum w d / sum w
+  return kmcudaSuccess;
+}
+// Bisecting k-means (DESIGN.md §4o): scikit-learn's BisectingKMeans with this library's draws and fixed-order sums, on
+// one GPU.  The leaves are ranges of perm; each round splits the pickable leaf of largest score (lowest lo on ties).  A
+// node's bisection depends on its rows and range only, so the host bisects ahead: when the top pickable leaf has no
+// cached result, one wave bisects every uncached leaf among the top K - #leaves, all n_init inits of all of them in the
+// same launches, and the rounds then apply cached results in pick order.  Nodes bisected but never picked are the waste;
+// a wave holds at most K - #leaves nodes.  Every wave-iteration reads the status records back in one copy.
+KMCUDAResult Job::bisecting(uint32_t seed, float tolerance, int strategy, uint32_t n_init, uint32_t max_iter,
+                            uint32_t trials, double* inertia_out) {
+  static const char* const kStop[] = {"equal labels", "tolerance", "max_iter"};
+  Dev& d = devs[0];
+  KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+  if (max_iter == 0) max_iter = 300;
+  Drain drain{*this};
+  // scikit-learn's KMeans _tolerance (BisectingKMeans 1.9 passes tol unscaled): tolerance times the mean of the
+  // unweighted per-feature variances; a non-finite sample makes that mean non-finite
+  double tol_abs = 0;
+  {
+    DevBuf<double> work, var;
+    KMB_CU(work.alloc(mb_variance_doubles(D)), kmcudaMemoryAllocationFailure);
+    KMB_CU(var.alloc(D), kmcudaMemoryAllocationFailure);
+    KMB_CU(launch_mb_variance(d.X, N, D, work, var, d.st), kmcudaRuntimeError);
+    std::vector<double> hv(D);
+    KMB_CU(cudaMemcpyAsync(hv.data(), var.get(), sizeof(double) * D, cudaMemcpyDeviceToHost, d.st),
+           kmcudaMemoryCopyError);
+    KMB_CU(cudaStreamSynchronize(d.st), kmcudaRuntimeError);
+    double m = 0;
+    for (int f = 0; f < D; f++) m += hv[f];
+    if (!std::isfinite(m)) {
+      KMB_INFO("bisecting k-means takes finite samples\n");
+      return kmcudaInvalidArguments;
+    }
+    tol_abs = m / D * static_cast<double>(tolerance);
+  }
+  // a wave's segments of one init are disjoint ranges; segment, slot and chunk indices are 32-bit and the chunks are one
+  // grid, so a call whose n_init * K does not fit is rejected
+  const size_t nch_max = static_cast<size_t>(n_init) * (cdiv(N, kBkChunk) + static_cast<size_t>(K));
+  const size_t nseg_max = static_cast<size_t>(n_init) * K;
+  if (2 * nseg_max > UINT32_MAX || nch_max > INT32_MAX) {
+    KMB_INFO("bisecting k-means: n_init * clusters is too large\n");
+    return kmcudaInvalidArguments;
+  }
+  DevBuf<uint32_t> perm, perm2, flags, excl, leaf_lo;
+  DevBuf<uint8_t> lab;
+  DevBuf<BkSeg> segs;
+  DevBuf<uint2> work;
+  DevBuf<float> cbuf, csq;
+  DevBuf<double> part;
+  DevBuf<BkChunkStat> cstat;
+  DevBuf<BkKey> keys;
+  DevBuf<BkStatus> status;
+  DevBuf<char> tmp;
+  DevBuf<float> dist;
+  DevBuf<BkKey> tkeys;
+  DevBuf<double> phi;
+  DevBuf<uint32_t> trows;
+  if (trials) {   // greedy init
+    KMB_CU(dist.alloc(static_cast<size_t>(n_init) * N), kmcudaMemoryAllocationFailure);
+    KMB_CU(tkeys.alloc(nch_max * kGppMaxTrials), kmcudaMemoryAllocationFailure);
+    KMB_CU(phi.alloc(nch_max * kGppMaxTrials), kmcudaMemoryAllocationFailure);
+    KMB_CU(trows.alloc(nseg_max * kGppMaxTrials), kmcudaMemoryAllocationFailure);
+  }
+  const size_t tmp_bytes = bk_split_bytes(N);
+  KMB_CU(perm.alloc(N), kmcudaMemoryAllocationFailure);
+  KMB_CU(perm2.alloc(N), kmcudaMemoryAllocationFailure);
+  KMB_CU(flags.alloc(N + 1), kmcudaMemoryAllocationFailure);
+  KMB_CU(excl.alloc(N + 1), kmcudaMemoryAllocationFailure);
+  KMB_CU(leaf_lo.alloc(K), kmcudaMemoryAllocationFailure);
+  KMB_CU(lab.alloc(static_cast<size_t>(n_init) * N), kmcudaMemoryAllocationFailure);
+  KMB_CU(segs.alloc(nseg_max), kmcudaMemoryAllocationFailure);
+  KMB_CU(work.alloc(nch_max), kmcudaMemoryAllocationFailure);
+  KMB_CU(cbuf.alloc(static_cast<size_t>(nseg_max) * 4 * D), kmcudaMemoryAllocationFailure);
+  KMB_CU(csq.alloc(static_cast<size_t>(nseg_max) * 4), kmcudaMemoryAllocationFailure);
+  KMB_CU(part.alloc(static_cast<size_t>(nch_max) * bk_partial_doubles(D)), kmcudaMemoryAllocationFailure);
+  KMB_CU(cstat.alloc(nch_max), kmcudaMemoryAllocationFailure);
+  KMB_CU(keys.alloc(2 * static_cast<size_t>(nch_max)), kmcudaMemoryAllocationFailure);
+  KMB_CU(status.alloc(nseg_max), kmcudaMemoryAllocationFailure);
+  KMB_CU(tmp.alloc(tmp_bytes), kmcudaMemoryAllocationFailure);
+  KMB_CU(launch_bk_iota(perm, N, d.st), kmcudaRuntimeError);
+  BkLaunch la;
+  la.X = d.X;
+  la.D = D;
+  la.N = N;
+  la.w = d.w.get();
+  la.lab = lab;
+  la.segs = segs;
+  la.work = work;
+  la.cbuf = cbuf;
+  la.csq = csq;
+  la.part = part;
+  la.cstat = cstat;
+  la.keys = keys;
+  la.dist = dist.get();
+  la.tkeys = tkeys.get();
+  la.phi = phi.get();
+  la.trows = trows.get();
+  la.status = status;
+  uint32_t* cur_perm = perm.get();
+  uint32_t* alt_perm = perm2.get();
+  g_prof.mark("bisecting: setup");
+
+  struct Result {
+    bool splittable;
+    uint32_t r, n0;
+    double score[2];
+    std::vector<float> C;   // [2][D]
+  };
+  std::map<uint32_t, uint32_t> leaves;              // lo -> hi of every leaf, in perm order
+  std::map<uint32_t, std::vector<float>> centre;    // lo -> centre of the leaf
+  auto order = [](const std::pair<double, uint32_t>& a, const std::pair<double, uint32_t>& b) {
+    return a.first > b.first || (a.first == b.first && a.second < b.second);
+  };
+  std::set<std::pair<double, uint32_t>, decltype(order)> pickable(order);   // (score, lo)
+  std::map<uint32_t, Result> cache;                  // lo of a leaf -> its bisection
+  std::vector<BkSeg> pending;                        // splits decided but not yet applied to perm
+  leaves[0] = N;
+  pickable.insert({0.0, 0u});
+  uint32_t waves = 0, bisected = 0;
+  std::vector<BkSeg> hs;
+  std::vector<uint2> hw;
+  std::vector<BkStatus> hst;
+  // the table of CTAs for the segments hs: {segment, chunk} pairs
+  auto upload = [&](bool with_work) -> KMCUDAResult {
+    if (with_work) {
+      hw.clear();
+      for (uint32_t s = 0; s < hs.size(); s++)
+        for (uint32_t c = 0; c < cdiv(hs[s].hi - hs[s].lo, kBkChunk); c++) hw.push_back({s, c});
+      KMB_CU(cudaMemcpyAsync(work.get(), hw.data(), sizeof(uint2) * hw.size(), cudaMemcpyHostToDevice, d.st),
+             kmcudaMemoryCopyError);
+    }
+    KMB_CU(cudaMemcpyAsync(segs.get(), hs.data(), sizeof(BkSeg) * hs.size(), cudaMemcpyHostToDevice, d.st),
+           kmcudaMemoryCopyError);
+    la.nseg = static_cast<uint32_t>(hs.size());
+    la.nwork = static_cast<uint32_t>(hw.size());
+    la.perm = cur_perm;
+    return kmcudaSuccess;
+  };
+  auto read_status = [&]() -> KMCUDAResult {
+    hst.resize(hs.size());
+    KMB_CU(cudaMemcpyAsync(hst.data(), status.get(), sizeof(BkStatus) * hs.size(), cudaMemcpyDeviceToHost, d.st),
+           kmcudaMemoryCopyError);
+    KMB_CU(cudaStreamSynchronize(d.st), kmcudaRuntimeError);
+    return kmcudaSuccess;
+  };
+  auto apply_pending = [&]() -> KMCUDAResult {
+    if (pending.empty()) return kmcudaSuccess;
+    hs = pending;
+    pending.clear();
+    KMB_RET(upload(true));
+    KMB_CU(launch_bk_split(la, flags, excl, tmp.get(), tmp_bytes, alt_perm, d.st), kmcudaRuntimeError);
+    std::swap(cur_perm, alt_perm);
+    g_prof.mark("bisecting: split");
+    return kmcudaSuccess;
+  };
+  // bisects the nodes [lo, hi) of `nodes` (one segment per node and init) into the cache
+  auto wave = [&](const std::vector<std::pair<uint32_t, uint32_t>>& nodes) -> KMCUDAResult {
+    waves++;
+    bisected += static_cast<uint32_t>(nodes.size());
+    hs.clear();
+    uint32_t pbase = 0;
+    for (auto& nd : nodes)
+      for (uint32_t r = 0; r < n_init; r++) {
+        const uint32_t s = static_cast<uint32_t>(hs.size());
+        hs.push_back({nd.first, nd.second, r, kBkRun, 2 * s, 2 * s + 1, pbase, seed,
+                      bk_node_key(seed, nd.first, nd.second, r, 0)});
+        pbase += cdiv(nd.second - nd.first, kBkChunk);
+      }
+    const std::vector<BkSeg> all = hs;
+    KMB_RET(upload(true));
+    KMB_CU(launch_bk_init(la, trials, d.st), kmcudaRuntimeError);
+    KMB_RET(read_status());
+    g_prof.mark("bisecting: init");
+    const size_t ns = all.size();
+    std::vector<BkStatus> fin(ns);
+    std::vector<uint32_t> iters(ns, 0), cur_slot(ns), stop(ns, 0);
+    std::vector<char> done(ns, 0), noinit(ns, 0);
+    std::vector<uint32_t> active;
+    for (uint32_t s = 0; s < ns; s++) {
+      cur_slot[s] = all[s].cur;
+      if (hst[s].init_row[1] == UINT32_MAX) {
+        noinit[s] = 1;
+        done[s] = 1;
+      } else {
+        active.push_back(s);
+      }
+    }
+    std::vector<uint32_t> mode(ns, kBkRun);
+    while (!active.empty()) {
+      hs.clear();
+      for (uint32_t s : active) {
+        BkSeg g = all[s];
+        g.mode = mode[s];
+        g.cur = cur_slot[s];
+        g.nxt = cur_slot[s] ^ 1u;
+        hs.push_back(g);
+      }
+      KMB_RET(upload(true));
+      KMB_CU(launch_bk_step(la, d.st), kmcudaRuntimeError);
+      KMB_RET(read_status());
+      std::vector<uint32_t> next;
+      for (size_t a = 0; a < active.size(); a++) {
+        const uint32_t s = active[a];
+        const BkStatus& st = hst[a];
+        if (mode[s] == kBkFinal) {
+          fin[s] = st;
+          done[s] = 1;
+          continue;
+        }
+        const uint32_t i = iters[s]++;
+        if (i > 0 && st.changed == 0) {   // strict convergence: the labels and centres of this E step stand
+          fin[s] = st;
+          done[s] = 1;
+          stop[s] = 0;
+          continue;
+        }
+        cur_slot[s] ^= 1u;
+        if (st.shift <= tol_abs) {
+          mode[s] = kBkFinal;
+          stop[s] = 1;
+        } else if (iters[s] == max_iter) {
+          mode[s] = kBkFinal;
+          stop[s] = 2;
+        }
+        next.push_back(s);
+      }
+      active.swap(next);
+    }
+    g_prof.mark("bisecting: 2-means");
+    std::vector<float> hc(static_cast<size_t>(ns) * 4 * D);
+    KMB_CU(cudaMemcpyAsync(hc.data(), cbuf.get(), sizeof(float) * hc.size(), cudaMemcpyDeviceToHost, d.st),
+           kmcudaMemoryCopyError);
+    KMB_CU(cudaStreamSynchronize(d.st), kmcudaRuntimeError);
+    for (size_t b = 0; b < ns; b += n_init) {
+      const uint32_t lo = all[b].lo, hi = all[b].hi;
+      Result res{false, 0, 0, {0, 0}, {}};
+      if (noinit[b]) {
+        KMB_DEBUG("bisecting: node [%" PRIu32 ", %" PRIu32 ") has no init\n", lo, hi);
+      } else {
+        uint32_t best = 0;
+        for (uint32_t r = 0; r < n_init; r++) {
+          const BkStatus& st = fin[b + r];
+          KMB_DEBUG("bisecting: node [%" PRIu32 ", %" PRIu32 ") init %" PRIu32 ": %" PRIu32
+                    " iterations, stopped on %s, inertia %.17g\n", lo, hi, r, iters[b + r], kStop[stop[b + r]],
+                    st.inertia);
+          if (r > 0 && st.inertia < fin[b + best].inertia * (1 - 1e-6)) best = r;   // scikit-learn's _bisect
+        }
+        const BkStatus& st = fin[b + best];
+        res.splittable = st.W[0] > 0 && st.W[1] > 0;
+        res.r = best;
+        res.n0 = st.cnt[0];
+        for (int j = 0; j < 2; j++) res.score[j] = strategy == 0 ? st.I[j] : static_cast<double>(st.cnt[j]);
+        const float* c = hc.data() + static_cast<size_t>(cur_slot[b + best]) * 2 * D;
+        res.C.assign(c, c + 2 * D);
+      }
+      cache[lo] = std::move(res);
+    }
+    return kmcudaSuccess;
+  };
+
+  uint32_t nleaves = 1;
+  while (nleaves < K) {
+    if (pickable.empty()) {
+      KMB_INFO("bisecting: only %" PRIu32 " of %" PRIu32 " clusters can be made from these samples\n", nleaves, K);
+      return kmcudaInvalidArguments;
+    }
+    const auto top = *pickable.begin();
+    const uint32_t lo = top.second, hi = leaves[lo];
+    auto it = cache.find(lo);
+    if (it == cache.end()) {
+      KMB_RET(apply_pending());
+      std::vector<std::pair<uint32_t, uint32_t>> nodes;
+      uint32_t taken = 0;
+      for (auto p = pickable.begin(); p != pickable.end() && taken < K - nleaves; ++p, ++taken)
+        if (!cache.count(p->second)) nodes.push_back({p->second, leaves[p->second]});
+      KMB_RET(wave(nodes));
+      continue;
+    }
+    Result res = std::move(it->second);
+    cache.erase(it);
+    pickable.erase(pickable.begin());
+    if (!res.splittable) {
+      KMB_INFO("bisecting: [%" PRIu32 ", %" PRIu32 ") is not split\n", lo, hi);
+      continue;
+    }
+    const uint32_t mid = lo + res.n0;
+    KMB_INFO("bisecting: split [%" PRIu32 ", %" PRIu32 ") into %" PRIu32 " + %" PRIu32 " rows, scores %.17g %.17g\n", lo,
+             hi, res.n0, hi - mid, res.score[0], res.score[1]);
+    pending.push_back({lo, hi, res.r, 0, 0, 0, 0, 0, 0});
+    leaves[lo] = mid;
+    leaves[mid] = hi;
+    centre[lo].assign(res.C.begin(), res.C.begin() + D);
+    centre[mid].assign(res.C.begin() + D, res.C.end());
+    pickable.insert({res.score[0], lo});
+    pickable.insert({res.score[1], mid});
+    nleaves++;
+  }
+  KMB_RET(apply_pending());
+  std::vector<uint32_t> hlo;
+  std::vector<float> hC;
+  hlo.reserve(K);
+  hC.reserve(static_cast<size_t>(K) * D);
+  for (auto& lf : leaves) {
+    hlo.push_back(lf.first);
+    hC.insert(hC.end(), centre[lf.first].begin(), centre[lf.first].end());
+  }
+  KMB_CU(cudaMemcpyAsync(leaf_lo.get(), hlo.data(), sizeof(uint32_t) * K, cudaMemcpyHostToDevice, d.st),
+         kmcudaMemoryCopyError);
+  KMB_CU(cudaMemcpyAsync(d.C.get(), hC.data(), sizeof(float) * hC.size(), cudaMemcpyHostToDevice, d.st),
+         kmcudaMemoryCopyError);
+  KMB_CU(launch_bk_assign(cur_perm, N, leaf_lo, K, d.assign, d.st), kmcudaRuntimeError);
+  KMB_CU(cudaStreamSynchronize(d.st), kmcudaRuntimeError);
+  g_prof.mark("bisecting: labels");
+  double e = 0;
+  if (inertia_out || verbosity > 0) KMB_RET(inertia(&e));
+  KMB_INFO("bisecting: %" PRIu32 " waves, %" PRIu32 " nodes bisected, inertia %.17g\n", waves, bisected, e);
+  if (inertia_out) *inertia_out = e;
   return kmcudaSuccess;
 }
 }  // namespace kmb

@@ -192,6 +192,10 @@ class Job {
   KMCUDAResult restarts(KMCUDAInitMethod method, const void* init_params, uint32_t seed, uint32_t n_init,
                         int device_ptrs, bool fp16x2, const float* user_centroids, float tolerance, uint32_t G,
                         double* inertia_out);
+  // bisecting k-means (kmcuda_b200_kmeans_bisecting, DESIGN.md §4o) on the first device: C / assign, *inertia_out;
+  // trials = 0: random init, else greedy k-means++ with that many trials
+  KMCUDAResult bisecting(uint32_t seed, float tolerance, int strategy, uint32_t n_init, uint32_t max_iter,
+                         uint32_t trials, double* inertia_out);
   KMCUDAResult inertia(double* out);
   KMCUDAResult average_distance(float* out);
 };

@@ -245,6 +245,71 @@ cudaError_t launch_mb_stats(const float* Cold, const float* Cnew, const double* 
 size_t mb_variance_doubles(int D);
 cudaError_t launch_mb_variance(const float* X, uint32_t n, int D, double* work, double* var, cudaStream_t st);
 
+// ---- bisecting k-means (bisecting.cu) -----------------------------------------------------------------------------------
+// The draws of a node [lo, hi) of perm: row i of init r in stage s draws u = unit_oo(mix(bk_node_key(seed, lo, hi, r, s)
+// ^ i)), so a node's bisection is the same whenever it is computed
+constexpr uint64_t kBkTagNode = 0x6269736563742121ull;   // "bisect!!"
+constexpr uint32_t kBkChunk = 2048;   // positions per chunk of the fixed-order sums (and per CTA of the row kernels)
+constexpr uint32_t kBkRun = 0, kBkFinal = 1;   // segment modes: E + M step; the last E step (no M step)
+uint64_t bk_node_key(uint32_t seed, uint32_t lo, uint32_t hi, uint32_t r, uint32_t stage);
+// one (node, init r) of a wave: positions [lo, hi) of perm, label plane r, centre slots cur / nxt of the centre buffer
+// ([slot][2][D] floats, squared norms [slot][2]), chunk partials from chunk index pbase on, draw key
+struct BkSeg {
+  uint32_t lo, hi, r, mode, cur, nxt, pbase, seed;
+  uint64_t key;
+};
+struct BkKey {
+  double key;
+  uint32_t row, pad;
+};
+struct BkChunkStat {
+  unsigned long long fk[2];   // per child: max of (bits of e) << 32 | ~row over the rows of positive weight
+  uint32_t cnt[2], npos[2], changed, pad;
+};
+// per segment, after a step: per child W = sum w, I = sum w e, row counts and rows of positive weight, over the labels
+// of this E step; inertia = sum w e over all rows; changed labels; relocated (init_row[0] = the row); shift = sum
+// ||c_new - c_old||^2.  After the init: init_row = the two centre rows (init_row[1] = UINT32_MAX: no init)
+struct BkStatus {
+  double W[2], I[2], inertia, shift;
+  uint32_t cnt[2], npos[2], changed, relocated, init_row[2];
+};
+struct BkLaunch {
+  const float* X;
+  int D;
+  uint32_t N;
+  const float* w;          // nullptr = unweighted
+  const uint32_t* perm;
+  uint8_t* lab;            // [n_init][N] label bytes by position
+  const BkSeg* segs;
+  uint32_t nseg;
+  const uint2* work;       // {segment, chunk} per CTA
+  uint32_t nwork;
+  float* cbuf;
+  float* csq;
+  double* part;            // [chunks][bk_partial_doubles(D)]
+  BkChunkStat* cstat;      // [chunks]
+  BkKey* keys;             // [chunks][2]
+  BkStatus* status;        // [nseg]
+  // greedy init only
+  float* dist;             // [n_init][N] distance to c0 by position
+  BkKey* tkeys;            // [chunks][kGppMaxTrials]
+  double* phi;             // [chunks][kGppMaxTrials]
+  uint32_t* trows;         // [nseg][kGppMaxTrials]
+};
+size_t bk_partial_doubles(int D);
+cudaError_t launch_bk_iota(uint32_t* perm, uint32_t n, cudaStream_t st);
+// init of every segment.  L == 0, random: centres = the two positive-weight rows of smallest -ln(u) / w.  L > 0, greedy
+// k-means++ with L trials: c0 = the first of them, c1 = §4m's round 1 restricted to the node
+cudaError_t launch_bk_init(const BkLaunch& a, uint32_t L, cudaStream_t st);
+// one E step (and M step in mode kBkRun) of every segment: labels, new centres in slot nxt, status records
+cudaError_t launch_bk_step(const BkLaunch& a, cudaStream_t st);
+// applies the splits listed as segments (label plane r): perm_out = perm with each range stably partitioned by label
+size_t bk_split_bytes(uint32_t N);
+cudaError_t launch_bk_split(const BkLaunch& a, uint32_t* flags, uint32_t* excl, void* tmp, size_t tmp_bytes,
+                            uint32_t* perm_out, cudaStream_t st);
+cudaError_t launch_bk_assign(const uint32_t* perm, uint32_t N, const uint32_t* leaf_lo, uint32_t K, uint32_t* assign,
+                             cudaStream_t st);
+
 // ---- relocation of empty clusters (relocate.cu) ------------------------------------------------------------------------
 // keys[i] of the shard rows i < n (global row off + i): orderable bits of d_i (L2: the Kahan sum of squared differences
 // to C[assign[i]] before the square root; angular: distance_exact<1>) << 32 | ~(off + i), so that a descending order is

@@ -165,14 +165,32 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
   float tolerance = .01f, yinyang_t = .1f;
   PyObject *samples_obj, *init_obj = Py_None, *metric_obj = Py_None, *weight_obj = Py_None, *batch_obj = Py_None;
   PyObject *steps_obj = nullptr, *relocate_obj = Py_False, *n_init_obj = nullptr, *inertia_obj = Py_False;
+  PyObject *bisecting_obj = Py_None, *max_iter_obj = nullptr;
   static const char* kwlist[] = {"samples", "clusters", "tolerance", "init", "yinyang_t", "metric",
                                  "average_distance", "seed", "device", "verbosity", "sample_weight", "batch_size",
-                                 "max_steps", "relocate_empty_clusters", "n_init", "inertia", nullptr};
-  if (!PyArg_ParseTupleAndKeywords(args, kwargs, "OI|fOfOpIIiOOOOOO", const_cast<char**>(kwlist), &samples_obj,
+                                 "max_steps", "relocate_empty_clusters", "n_init", "inertia", "bisecting",
+                                 "max_iter", nullptr};
+  if (!PyArg_ParseTupleAndKeywords(args, kwargs, "OI|fOfOpIIiOOOOOOOO", const_cast<char**>(kwlist), &samples_obj,
                                    &clusters, &tolerance, &init_obj, &yinyang_t, &metric_obj, &adflag, &seed,
                                    &device, &verbosity, &weight_obj, &batch_obj, &steps_obj, &relocate_obj,
-                                   &n_init_obj, &inertia_obj))
+                                   &n_init_obj, &inertia_obj, &bisecting_obj, &max_iter_obj))
     return nullptr;
+  // bisecting k-means (kmcuda_b200.h, kmcuda_b200_kmeans_bisecting): None or a strategy name
+  int32_t strategy = -1;
+  if (bisecting_obj != Py_None) {
+    if (!PyUnicode_Check(bisecting_obj)) {
+      PyErr_SetString(PyExc_TypeError, "\"bisecting\" must be None or a string");
+      return nullptr;
+    }
+    const char* b = PyUnicode_AsUTF8(bisecting_obj);
+    if (b && strcmp(b, "biggest_inertia") == 0) strategy = 0;
+    else if (b && strcmp(b, "largest_cluster") == 0) strategy = 1;
+    else {
+      PyErr_Clear();
+      PyErr_SetString(PyExc_ValueError, "\"bisecting\" must be \"biggest_inertia\" or \"largest_cluster\"");
+      return nullptr;
+    }
+  }
   // relocation of empty clusters (kmcuda_b200.h, kmcuda_b200_kmeans_relocate): a bool, not with mini-batch
   if (!(PyBool_Check(relocate_obj) || PyArray_IsScalar(relocate_obj, Bool))) {
     PyErr_SetString(PyExc_TypeError, "\"relocate_empty_clusters\" must be a bool");
@@ -205,6 +223,31 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
   if (relocate && batch_obj != Py_None) {
     PyErr_SetString(PyExc_ValueError, "\"relocate_empty_clusters\" applies to Lloyd / Yinyang runs: mini-batch "
                                       "k-means (\"batch_size\") reassigns its clusters itself");
+    return nullptr;
+  }
+  if (strategy >= 0) {
+    // "random", "greedy-k-means++" / "greedy-kmeans++", or a tuple whose first item is a greedy name
+    PyObject* name = init_obj;
+    const bool tuple = init_obj && PyTuple_Check(init_obj);
+    if (tuple) name = PyTuple_Size(init_obj) > 0 ? PyTuple_GetItem(init_obj, 0) : nullptr;
+    const char* i = name && PyUnicode_Check(name) ? PyUnicode_AsUTF8(name) : nullptr;
+    const bool greedy_name = i && (strcmp(i, "greedy-k-means++") == 0 || strcmp(i, "greedy-kmeans++") == 0);
+    if (batch_obj != Py_None || max_steps || relocate) {
+      PyErr_SetString(PyExc_ValueError, "\"bisecting\" cannot be combined with \"batch_size\", \"max_steps\" or "
+                                        "\"relocate_empty_clusters\"");
+      return nullptr;
+    }
+    if (!(greedy_name || (!tuple && i && strcmp(i, "random") == 0))) {
+      PyErr_Clear();
+      PyErr_SetString(PyExc_ValueError,
+                      "\"bisecting\" takes init=\"random\", \"greedy-k-means++\" or (\"greedy-k-means++\", L)");
+      return nullptr;
+    }
+  }
+  uint32_t max_iter = 0;
+  if (max_iter_obj && !take_count(max_iter_obj, "max_iter", 0, &max_iter)) return nullptr;
+  if (max_iter && strategy < 0) {
+    PyErr_SetString(PyExc_ValueError, "\"max_iter\" applies to bisecting runs only: pass \"bisecting\" too");
     return nullptr;
   }
   // restarts (kmcuda_b200.h, kmcuda_b200_kmeans_restarts): n_init an integer >= 1, inertia a bool; not with mini-batch
@@ -382,7 +425,12 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
     fflush(stdout);
   }
   Py_BEGIN_ALLOW_THREADS
-  if (n_init != 1 || want_inertia)
+  if (strategy >= 0)
+    result = kmcuda_b200_kmeans_bisecting(init, &afkmc2_m, tolerance, metric, n, static_cast<uint16_t>(d), clusters,
+                                          seed, device, device_ptrs, fp16x2, verbosity, samples, weights, strategy,
+                                          n_init, max_iter, centroids, assignments,
+                                          adflag ? &average_distance : nullptr, want_inertia ? &inertia : nullptr);
+  else if (n_init != 1 || want_inertia)
     result = kmcuda_b200_kmeans_restarts(init, &afkmc2_m, tolerance, yinyang_t, metric, n, static_cast<uint16_t>(d),
                                          clusters, seed, device, device_ptrs, fp16x2, verbosity, samples, weights,
                                          relocate ? 1 : 0, n_init, centroids, assignments,
@@ -537,7 +585,7 @@ PyObject* py_knn_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
 char module_doc[] = "K-means and K-nn on NVIDIA H100 (drop-in for src-d/kmcuda's libKMCUDA).";
 char kmeans_doc[] = "kmeans_cuda(samples, clusters, tolerance=.01, init=\"k-means++\", yinyang_t=.1, metric=\"L2\", "
                     "average_distance=False, seed=time(), device=0, verbosity=0, sample_weight=None, batch_size=None, "
-                    "max_steps=0, relocate_empty_clusters=False, n_init=1, inertia=False) -> "
+                    "max_steps=0, relocate_empty_clusters=False, n_init=1, inertia=False, bisecting=None, max_iter=0) -> "
                     "(centroids, assignments[, avg][, inertia])";
 char knn_doc[] = "knn_cuda(k, samples, centroids, assignments, metric=\"L2\", device=0, verbosity=0) -> neighbors";
 
