@@ -143,6 +143,38 @@ KMCUDAResult kmcuda_b200_kmeans_restarts(KMCUDAInitMethod init, const void *init
                                          float *centroids, uint32_t *assignments, float *average_distance,
                                          double *inertia /* NULL = not wanted */);
 
+/* k-means with scikit-learn's stopping rule, KMeans(tol=..., max_iter=...): kmcuda_b200_kmeans_restarts() with the
+ * reassignment `tolerance` replaced by the centre-shift `tol`, plus max_iter (0 = 300) and *n_iter.  It accepts what
+ * _restarts accepts and rejects what it rejects, and in addition a negative or non-finite tol.  The rule (DESIGN.md §4p):
+ *   tol_abs = tol * mean_f Var(X_f), the unweighted population variance of every feature in double (scikit-learn's
+ *     _tolerance), computed once per call; tol == 0 gives 0 without the variance pass.  With a non-finite sample tol_abs
+ *     is not finite and only equal labels or max_iter can stop a run.
+ *   Iteration i = 1, 2, ... is one assignment pass (pass i), the centroid update (with relocation if asked for), then
+ *     S_i = sum_c ||c_new - c_old||^2 in double in a fixed order; a centroid whose old or new coordinates are not finite
+ *     (a cluster that died under the reference's empty-cluster rule) adds 0.
+ *   The run stops when pass i (i > 1) makes no reassignment ("equal labels": its labels and the centroids they were
+ *     made against stand, n_iter = i); when S_i <= tol_abs ("tolerance") or i == max_iter ("max_iter"): pass i + 1 is
+ *     the final E step and n_iter = i.  The shift or the cap at i wins over equal labels at pass i + 1, as in
+ *     scikit-learn's _kmeans_single_lloyd.
+ * S_i is read back with pass i + 1's reassignment count, so an iteration keeps its one host round trip.  Yinyang runs
+ * make the same decisions at the same points; its Lloyd draft and the adaptive switch back to Lloyd are unchanged.
+ * Every restart runs this rule; *inertia is taken after the final E step and *n_iter (if not NULL) is the kept
+ * restart's.  tol == 0 with a large enough max_iter stops where _restarts(tolerance = 0) stops, with the same results.
+ * Log: the "iteration %d: %u reassignments" lines are those of every pass (the final E step is pass n_iter + 1), the
+ * "reassignments threshold" line becomes "center shift tolerance: %.17g, max_iter %u", verbosity >= 1 adds "stopped
+ * at iteration %d: <equal labels | tolerance | max_iter>" and verbosity >= 2 "center shift %d: %.17g (tolerance %.17g)"
+ * per update. */
+KMCUDAResult kmcuda_b200_kmeans_center_shift(KMCUDAInitMethod init, const void *init_params, float tol,
+                                             float yinyang_t, KMCUDADistanceMetric metric, uint32_t samples_size,
+                                             uint16_t features_size, uint32_t clusters_size, uint32_t seed,
+                                             uint32_t device, int32_t device_ptrs, int32_t fp16x2, int32_t verbosity,
+                                             const float *samples, const float *weights /* NULL = unweighted */,
+                                             int32_t relocate_empty_clusters, uint32_t n_init,
+                                             uint32_t max_iter /* 0 = 300 */, float *centroids,
+                                             uint32_t *assignments, float *average_distance,
+                                             double *inertia /* NULL = not wanted */,
+                                             uint32_t *n_iter /* NULL = not wanted */);
+
 /* Bisecting k-means, scikit-learn's BisectingKMeans: the K clusters are made by splitting one cluster in two at a time
  * with a 2-means run inside it, on one GPU (device: a mask of at most one bit, 0 = the first GPU), L2 only.  The
  * parameters up to `weights` are those of kmcuda_b200_kmeans_minibatch().  strategy 0 splits the leaf of largest

@@ -8,7 +8,8 @@ Python surface = the reference's `libKMCUDA` module (reference src/python.cc:33-
                 batch_size=None, max_steps=0,                                 # extension: mini-batch k-means
                 relocate_empty_clusters=False,                                # extension: scikit-learn's relocation
                 n_init=1, inertia=False,                                      # extension: restarts, inertia
-                bisecting=None, max_iter=0)                                   # extension: bisecting k-means
+                bisecting=None, max_iter=0,                                   # extension: bisecting k-means
+                tol=None, n_iter=False)                                       # extension: scikit-learn's stop rule
                 init="k-means||" / ("k-means||", rounds)                      # extension: k-means|| seeding
     knn_cuda(k, samples, centroids, assignments, metric="L2", device=0, verbosity=0)  # python.cc:412-632
     supports_fp16                                                             # python.cc:52
@@ -55,6 +56,9 @@ _lib.kmcuda_b200_kmeans_bisecting.restype = ctypes.c_int
 _lib.kmcuda_b200_kmeans_bisecting.argtypes = _lib.kmcuda_b200_kmeans_minibatch.argtypes[:13] + \
     [ctypes.c_void_p, ctypes.c_int32, ctypes.c_uint32, ctypes.c_uint32] + _lib.kmeans_cuda.argtypes[14:] + \
     [ctypes.c_void_p]
+_lib.kmcuda_b200_kmeans_center_shift.restype = ctypes.c_int
+_lib.kmcuda_b200_kmeans_center_shift.argtypes = _lib.kmcuda_b200_kmeans_restarts.argtypes[:-4] + [ctypes.c_uint32] + \
+    _lib.kmcuda_b200_kmeans_restarts.argtypes[-4:] + [ctypes.c_void_p]
 _lib.knn_cuda.restype = ctypes.c_int
 _lib.knn_cuda.argtypes = [
     ctypes.c_uint16, ctypes.c_int, ctypes.c_uint32, ctypes.c_uint16, ctypes.c_uint32, ctypes.c_uint32,
@@ -183,8 +187,10 @@ def _raise_for(result, fn):
 
 def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1, metric="L2",
                 average_distance=False, seed=None, device=0, verbosity=0, sample_weight=None, batch_size=None,
-                max_steps=0, relocate_empty_clusters=False, n_init=1, inertia=False, bisecting=None, max_iter=0):
-    """K-means on the GPU(s); see the module docstring.  Returns (centroids, assignments[, avg_distance][, inertia]).
+                max_steps=0, relocate_empty_clusters=False, n_init=1, inertia=False, bisecting=None, max_iter=0,
+                tol=None, n_iter=False):
+    """K-means on the GPU(s); see the module docstring.  Returns (centroids, assignments[, avg_distance][, inertia]
+    [, n_iter]).
 
     sample_weight: one non-negative weight per sample (include/kmcuda_b200.h, kmcuda_b200_kmeans_weighted), a 1-D
     array-like of length N, or an int device pointer when `samples` is the device-pointer tuple; None = unweighted.
@@ -209,7 +215,17 @@ def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1
     scikit-learn's BisectingKMeans with that bisecting_strategy) on one GPU, L2 only, with init "random",
     "greedy-k-means++" or ("greedy-k-means++", L) (L = 0: 2 trials, scikit-learn's 2 + floor(ln 2)); n_init is then
     the number of inits per bisection and max_iter (0 = 300) the Lloyd iterations per 2-means run; yinyang_t is
-    ignored.  Not with batch_size, max_steps or relocate_empty_clusters.  None = the other routes."""
+    ignored.  Not with batch_size, max_steps or relocate_empty_clusters.  None = the other routes.
+
+    tol: a real number >= 0 stops Lloyd / Yinyang runs by scikit-learn's KMeans rule (kmcuda_b200_kmeans_center_shift):
+    when the centroids of an update move by at most tol * (the mean per-feature variance of the samples) in total
+    squared distance, when an update is the max_iter-th (max_iter 0 = 300; one final assignment pass follows either),
+    or when a pass reassigns no sample.  `tolerance` is then ignored.  Works with sample_weight,
+    relocate_empty_clusters, n_init and inertia; not with batch_size or bisecting.  None = the reference's rule, a run
+    ends when at most tolerance * N samples were reassigned.
+
+    n_iter: True appends the number of iterations of the returned run (scikit-learn's n_iter_) as an int, last; needs
+    tol."""
     if bisecting is not None:
         if not isinstance(bisecting, str):
             raise TypeError("\"bisecting\" must be None or a string, got %r" % (bisecting,))
@@ -223,9 +239,23 @@ def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1
                 (isinstance(init, tuple) and _INIT_METHODS[name] == INIT_RANDOM):
             raise ValueError("\"bisecting\" takes init=\"random\", \"greedy-k-means++\" or (\"greedy-k-means++\", L), "
                              "got %r" % (init,))
+    if tol is not None:
+        if isinstance(tol, (bool, np.bool_)) or not isinstance(tol, (int, float, np.integer, np.floating)):
+            raise TypeError("\"tol\" must be None or a real number, got %r" % (tol,))
+        tol = float(tol)
+        if not (np.isfinite(tol) and tol >= 0):
+            raise ValueError("\"tol\" must be a finite number >= 0, got %r" % (tol,))
+        if batch_size is not None or bisecting is not None:
+            raise ValueError("\"tol\" applies to Lloyd / Yinyang runs: mini-batch (\"batch_size\") and bisecting runs "
+                             "scale \"tolerance\" themselves")
+    if not isinstance(n_iter, (bool, np.bool_)):
+        raise TypeError("\"n_iter\" must be a bool, got %r" % (n_iter,))
+    n_iter = bool(n_iter)
+    if n_iter and tol is None:
+        raise ValueError("\"n_iter\" needs \"tol\": only runs with scikit-learn's stopping rule count iterations")
     max_iter = _count(max_iter, "max_iter", 0)
-    if max_iter and bisecting is None:
-        raise ValueError("\"max_iter\" applies to bisecting runs only: pass \"bisecting\" too")
+    if max_iter and bisecting is None and tol is None:
+        raise ValueError("\"max_iter\" applies to bisecting runs and runs with \"tol\" only: pass one of them too")
     if not isinstance(relocate_empty_clusters, (bool, np.bool_)):
         raise TypeError("\"relocate_empty_clusters\" must be a bool, got %r" % (relocate_empty_clusters,))
     relocate_empty_clusters = bool(relocate_empty_clusters)
@@ -327,10 +357,16 @@ def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1
             _cuda_memcpy_h2d(device_ptrs, centroids_ptr, imp.ctypes.data, clusters * d * 4)
     avg = ctypes.c_float(0)
     inertia_value = ctypes.c_double(0)
+    n_iter_value = ctypes.c_uint32(0)
     common = (init_method, ctypes.byref(afkmc2_m), tolerance, yinyang_t, metric_id, n, d, clusters,
               int(seed) & 0xFFFFFFFF, int(device), device_ptrs, int(fp16x2), int(verbosity), samples_ptr)
     outputs = (centroids_ptr, assignments_ptr, ctypes.byref(avg) if average_distance else None)
-    if bisecting is not None:
+    if tol is not None:
+        result = _lib.kmcuda_b200_kmeans_center_shift(
+            init_method, ctypes.byref(afkmc2_m), tol, *common[3:], weights_ptr, int(relocate_empty_clusters), n_init,
+            max_iter, *outputs, ctypes.byref(inertia_value) if inertia else None,
+            ctypes.byref(n_iter_value) if n_iter else None)
+    elif bisecting is not None:
         if yinyang_t and verbosity > 0:
             print("bisecting k-means: yinyang_t is ignored", flush=True)
         result = _lib.kmcuda_b200_kmeans_bisecting(*common[:3], *common[4:], weights_ptr,
@@ -357,6 +393,8 @@ def kmeans_cuda(samples, clusters, tolerance=.01, init="k-means++", yinyang_t=.1
         out += (avg.value,)
     if inertia:
         out += (inertia_value.value,)
+    if n_iter:
+        out += (int(n_iter_value.value),)
     return out
 
 

@@ -63,7 +63,8 @@ static KMCUDAResult print_memory_stats(const std::vector<int>& devs) {
 
 using namespace kmb;
 
-// kmeans_cuda, kmcuda_b200_kmeans_weighted, _relocate, _minibatch, _restarts and _bisecting (weights == nullptr: the unweighted run)
+// kmeans_cuda, kmcuda_b200_kmeans_weighted, _relocate, _minibatch, _restarts, _bisecting and _center_shift (weights ==
+// nullptr: the unweighted run; center_shift: scikit-learn's stopping rule with `tol` replaces the reassignment tolerance)
 static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, float tolerance,
                                 float yinyang_t, KMCUDADistanceMetric metric, uint32_t samples_size,
                                 uint16_t features_size, uint32_t clusters_size, uint32_t seed,
@@ -72,7 +73,8 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
                                 uint32_t* assignments, float* average_distance, bool minibatch = false,
                                 uint32_t batch_size = 0, uint32_t max_steps = 0, bool relocate = false,
                                 uint32_t n_init = 1, double* inertia = nullptr, bool bisecting = false,
-                                int32_t strategy = 0, uint32_t max_iter = 0) {
+                                int32_t strategy = 0, uint32_t max_iter = 0, bool center_shift = false,
+                                float tol = 0, uint32_t* n_iter = nullptr) {
   KMB_DEBUG("arguments: %d %p %.3f %.2f %d %" PRIu32 " %" PRIu16 " %" PRIu32 " %" PRIu32 " %" PRIu32
             " %d %" PRIi32 " %p %p %p %p\n", init, init_params, tolerance, yinyang_t, metric, samples_size,
             features_size, clusters_size, seed, device, fp16x2, verbosity, samples, centroids, assignments,
@@ -88,6 +90,7 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
   }
   if (samples == nullptr || centroids == nullptr || assignments == nullptr) return kmcudaInvalidArguments;
   if (!(tolerance >= 0 && tolerance <= 1)) return kmcudaInvalidArguments;
+  if (center_shift && !(std::isfinite(tol) && tol >= 0)) return kmcudaInvalidArguments;
   if (!(yinyang_t >= 0 && yinyang_t <= 0.5)) return kmcudaInvalidArguments;
   if (static_cast<uint64_t>(features_size) * (fp16x2 ? 2 : 1) > 65535u) return kmcudaInvalidArguments;
   if (init == kmcudaInitMethodKMeansParallel && init_params &&
@@ -144,7 +147,7 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
       return kmcudaInvalidArguments;
     }
   }
-  KMB_INFO("reassignments threshold: %" PRIu32 "\n", static_cast<uint32_t>(tolerance * samples_size));
+  if (!center_shift) KMB_INFO("reassignments threshold: %" PRIu32 "\n", static_cast<uint32_t>(tolerance * samples_size));
   const uint32_t yy_groups_size = static_cast<uint32_t>(yinyang_t * clusters_size);
   KMB_DEBUG("yinyang groups: %" PRIu32 "\n", yy_groups_size);
   std::vector<int> dev_ids;
@@ -156,6 +159,8 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
   Job job(m, samples_size, D, clusters_size, verbosity);
   job.weighted = weights != nullptr;
   job.relocate_empty = relocate;
+  job.center_shift = center_shift;
+  if (max_iter) job.max_iter = max_iter;
   KMB_RET(job.setup(dev_ids));
   g_prof.mark("setup: exchange (peer / nccl)");
   KMB_RET(job.ingest(samples, weights, device_ptrs, fp16x2 != 0));
@@ -163,6 +168,11 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
   if (weights) {
     KMB_RET(job.check_weights());
     g_prof.mark("weight check");
+  }
+  if (center_shift) {
+    KMB_RET(job.shift_tolerance(tol));   // once per call: every restart stops by the same tolerance
+    g_prof.mark("center shift tolerance");
+    KMB_INFO("center shift tolerance: %.17g, max_iter %" PRIu32 "\n", job.shift_tol, job.max_iter);
   }
   if (verbosity > 1) KMB_RET(print_memory_stats(dev_ids));
   if (bisecting) {
@@ -178,8 +188,10 @@ static KMCUDAResult kmeans_impl(KMCUDAInitMethod init, const void* init_params, 
     g_prof.mark("init centroids");
     KMB_RET(job.minibatch(batch_size, max_steps, tolerance, seed));
   } else {
-    KMB_RET(job.restarts(init, init_params, seed, n_init, device_ptrs, fp16x2 != 0, centroids, tolerance,
-                         yy_groups_size, inertia));
+    // under the rule a negative reassignment tolerance: no pass count ends a run or sends Yinyang to Lloyd
+    KMB_RET(job.restarts(init, init_params, seed, n_init, device_ptrs, fp16x2 != 0, centroids,
+                         center_shift ? -1.f : tolerance, yy_groups_size, inertia));
+    if (n_iter) *n_iter = static_cast<uint32_t>(job.n_iter);
   }
   if (average_distance) KMB_RET(job.average_distance(average_distance));
   g_prof.mark("average distance");
@@ -269,6 +281,20 @@ KMCUDAResult kmcuda_b200_kmeans_bisecting(KMCUDAInitMethod init, const void* ini
   return kmeans_impl(init, init_params, tolerance, 0.f, metric, samples_size, features_size, clusters_size, seed,
                      device, device_ptrs, fp16x2, verbosity, samples, weights, centroids, assignments,
                      average_distance, false, 0, 0, false, n_init, inertia, true, strategy, max_iter);
+}
+
+KMCUDAResult kmcuda_b200_kmeans_center_shift(KMCUDAInitMethod init, const void* init_params, float tol,
+                                              float yinyang_t, KMCUDADistanceMetric metric, uint32_t samples_size,
+                                              uint16_t features_size, uint32_t clusters_size, uint32_t seed,
+                                              uint32_t device, int32_t device_ptrs, int32_t fp16x2, int32_t verbosity,
+                                              const float* samples, const float* weights,
+                                              int32_t relocate_empty_clusters, uint32_t n_init, uint32_t max_iter,
+                                              float* centroids, uint32_t* assignments, float* average_distance,
+                                              double* inertia, uint32_t* n_iter) {
+  return kmeans_impl(init, init_params, 0.f, yinyang_t, metric, samples_size, features_size, clusters_size, seed,
+                     device, device_ptrs, fp16x2, verbosity, samples, weights, centroids, assignments,
+                     average_distance, false, 0, 0, relocate_empty_clusters != 0, n_init, inertia, false, 0, max_iter,
+                     true, tol, n_iter);
 }
 
 KMCUDAResult knn_cuda(uint16_t k, KMCUDADistanceMetric metric, uint32_t samples_size,

@@ -55,11 +55,16 @@ __device__ __forceinline__ void chunk_range(uint32_t n, uint32_t& lo, uint32_t& 
   hi = min(n, lo + per);
 }
 
+// FINITE_ONLY: a term that is not finite adds 0 (the centre-shift total, where a dead centroid's NaN must not count)
+template <bool FINITE_ONLY = false>
 __device__ __forceinline__ double chunk_sum(const double* __restrict__ v, uint32_t n) {
   uint32_t lo, hi;
   chunk_range(n, lo, hi);
   double acc = 0.0;
-  for (uint32_t b = lo; b < hi; b++) acc += v[b];
+  for (uint32_t b = lo; b < hi; b++) {
+    if constexpr (FINITE_ONLY) acc += isfinite(v[b]) ? v[b] : 0.0;
+    else acc += v[b];
+  }
   return acc;
 }
 

@@ -115,6 +115,14 @@ KMCUDAResult Job::setup(const std::vector<int>& dev_ids) {
       KMB_CU(d.wsums.alloc(K), kmcudaMemoryAllocationFailure);
       KMB_CU(d.cweights.alloc(K), kmcudaMemoryAllocationFailure);
     }
+    if (center_shift) {
+      KMB_CU(d.d_shift.alloc(1), kmcudaMemoryAllocationFailure);
+      KMB_CU(cudaMemsetAsync(d.d_shift.get(), 0, sizeof(double), d.st), kmcudaRuntimeError);
+      if (i == 0) {
+        KMB_CU(d.Cold.alloc(static_cast<size_t>(K) * D), kmcudaMemoryAllocationFailure);
+        KMB_CU(d.dsq.alloc(K), kmcudaMemoryAllocationFailure);
+      }
+    }
     g_prof.mark("setup: stream + job buffers");
     d.shard.reset(new Shard(metric, d.dev, d.len, D, K, verbosity));
     KMB_RET(d.shard->create(true));
@@ -235,15 +243,22 @@ KMCUDAResult Job::load_host_weights() {
   return sync_all();
 }
 
-// one assignment pass over every shard; *changed = total reassignments
-KMCUDAResult Job::assign_pass(uint32_t* changed) {
+// one assignment pass over every shard; *changed = total reassignments, *shift (if wanted) = the first device's d_shift
+KMCUDAResult Job::assign_pass(uint32_t* changed, double* shift) {
   for (auto& d : devs) {
     KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
     KMB_CU(cudaMemsetAsync(d.d_changed.get(), 0, sizeof(uint32_t), d.st), kmcudaRuntimeError);
     KMB_RET(d.shard->assign(d.len, d.X, d.C, d.assign, d.prev, d.d_changed, d.st));
   }
   std::vector<uint32_t> mine;
-  KMB_RET(gather([&](size_t i) { return devs[i].d_changed.get(); }, &mine));
+  if (shift) {
+    std::vector<double> s;
+    KMB_RET(gather([&](size_t i) { return devs[i].d_changed.get(); }, &mine,
+                   [&](size_t i) { return devs[i].d_shift.get(); }, &s));
+    *shift = s[0];
+  } else {
+    KMB_RET(gather([&](size_t i) { return devs[i].d_changed.get(); }, &mine));
+  }
   uint32_t total = 0;
   for (size_t i = 0; i < devs.size(); i++) {
     total += mine[i];
@@ -503,8 +518,90 @@ KMCUDAResult Job::relocate(int iter) {
   return kmcudaSuccess;
 }
 
+// scikit-learn's _tolerance (DESIGN.md §4p): shift_tol = tol times the mean of the unweighted population variances of
+// the features, in double.  Each device sums its shard per feature (launch_col_sums); the host adds the devices in
+// device order and divides by N, sends the mean back for the second pass over (x - mean)^2, and adds those the same way.
+KMCUDAResult Job::shift_tolerance(float tol) {
+  shift_tol = 0;
+  if (tol == 0) return kmcudaSuccess;
+  const size_t nd = devs.size(), dd = static_cast<size_t>(D);
+  std::vector<DevBuf<double>> work(nd);
+  Drain drain{*this};
+  std::vector<double> sums(nd * dd), mean(dd), var(dd);
+  for (int pass = 0; pass < 2; pass++) {
+    for (size_t i = 0; i < nd; i++) {
+      Dev& d = devs[i];
+      KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+      if (pass == 0) KMB_CU(work[i].alloc(mb_variance_doubles(D)), kmcudaMemoryAllocationFailure);
+      double* mu = work[i].get() + mb_variance_doubles(D) - 2 * dd;   // the layout of launch_mb_variance
+      double* out = mu + dd;
+      if (pass == 1)
+        KMB_CU(cudaMemcpyAsync(mu, mean.data(), sizeof(double) * dd, cudaMemcpyHostToDevice, d.st), kmcudaMemoryCopyError);
+      KMB_CU(launch_col_sums(d.X, d.len, D, pass ? mu : nullptr, work[i], out, d.st), kmcudaRuntimeError);
+      KMB_CU(cudaMemcpyAsync(sums.data() + i * dd, out, sizeof(double) * dd, cudaMemcpyDeviceToHost, d.st),
+             kmcudaMemoryCopyError);
+    }
+    KMB_RET(sync_all());
+    std::vector<double>& res = pass ? var : mean;
+    for (size_t f = 0; f < dd; f++) {
+      double acc = 0;
+      for (size_t i = 0; i < nd; i++) acc += sums[i * dd + f];
+      res[f] = acc / N;
+    }
+  }
+  double m = 0;
+  for (size_t f = 0; f < dd; f++) m += var[f];
+  shift_tol = m / D * static_cast<double>(tol);
+  return kmcudaSuccess;
+}
+
+// the centre shift of the update that just ran, sum ||C - Cold||^2 on the first device into its d_shift (the host reads
+// it back with the next pass); every device holds the same centroids
+KMCUDAResult Job::shift_of(const float* Cold) {
+  Dev& d = devs[0];
+  KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+  KMB_CU(launch_center_shift(Cold, d.C, K, D, d.dsq, d.d_shift, d.st), kmcudaRuntimeError);
+  return kmcudaSuccess;
+}
+
+// a Lloyd update; with the rule, the centroids are kept aside first and the shift follows
+KMCUDAResult Job::lloyd_update(int iter) {
+  Dev& d0 = devs[0];
+  if (center_shift) {
+    KMB_CU(cudaSetDevice(d0.dev), kmcudaRuntimeError);
+    KMB_CU(cudaMemcpyAsync(d0.Cold.get(), d0.C.get(), sizeof(float) * static_cast<size_t>(K) * D,
+                           cudaMemcpyDeviceToDevice, d0.st), kmcudaMemoryCopyError);
+  }
+  KMB_RET(update(iter));
+  if (center_shift) KMB_RET(shift_of(d0.Cold));
+  g_prof.mark("centroid update");
+  return kmcudaSuccess;
+}
+
+// scikit-learn's stopping rule (_kmeans_single_lloyd), after pass `iter` with `changed` reassignments; `shift` is the
+// centre shift of update iter - 1 (iter > 1), read back with this pass.  The run stops when that update moved the
+// centroids by at most shift_tol or was update max_iter (this pass is the final E step, n_iter = iter - 1), else when
+// this pass changed no label (n_iter = iter).  Sets n_iter; false without the rule.
+bool Job::shift_stop(int iter, uint32_t changed, double shift) {
+  if (!center_shift || iter < 2) return false;
+  KMB_DEBUG("center shift %d: %.17g (tolerance %.17g)\n", iter - 1, shift, shift_tol);
+  const char* why = nullptr;
+  int at = iter - 1;
+  if (shift <= shift_tol) why = "tolerance";
+  else if (at == static_cast<int>(max_iter)) why = "max_iter";
+  else if (changed == 0) {
+    why = "equal labels";
+    at = iter;
+  }
+  if (!why) return false;
+  n_iter = at;
+  KMB_INFO("stopped at iteration %d: %s\n", at, why);
+  return true;
+}
+
 // reference kmeans_cuda_lloyd, kmeans.cu:934-1026 (resume == false)
 KMCUDAResult Job::lloyd(float tolerance, int* iter_out, uint32_t* changed_out) {
+  n_iter = 0;
   for (auto& d : devs) {
     KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
     KMB_CU(cudaMemsetAsync(d.ccounts.get(), 0, sizeof(uint32_t) * K, d.st), kmcudaRuntimeError);
@@ -516,7 +613,8 @@ KMCUDAResult Job::lloyd(float tolerance, int* iter_out, uint32_t* changed_out) {
   auto t_prev = std::chrono::steady_clock::now();
   for (int iter = 1;; iter++) {
     uint32_t changed = 0;
-    KMB_RET(assign_pass(&changed));
+    double shift = 0;
+    KMB_RET(assign_pass(&changed, center_shift && iter > 1 ? &shift : nullptr));
     g_prof.mark("assign pass");
     // iteration period (update of the previous iteration + this pass; assign_pass synchronises): what a Yinyang
     // iteration has to beat (Job::yinyang)
@@ -529,9 +627,9 @@ KMCUDAResult Job::lloyd(float tolerance, int* iter_out, uint32_t* changed_out) {
     KMB_INFO("iteration %d: %" PRIu32 " reassignments\n", iter, changed);
     if (iter_out) *iter_out = iter;
     if (changed_out) *changed_out = changed;
+    if (shift_stop(iter, changed, shift)) return kmcudaSuccess;
     if (changed <= tolerance * N) return kmcudaSuccess;  // float compare, kmeans.cu:707
-    KMB_RET(update(iter));
-    g_prof.mark("centroid update");
+    KMB_RET(lloyd_update(iter));
   }
 }
 
@@ -539,13 +637,14 @@ KMCUDAResult Job::lloyd(float tolerance, int* iter_out, uint32_t* changed_out) {
 // the Yinyang iterations of a run turn out slower than its Lloyd passes (Job::yinyang)
 KMCUDAResult Job::lloyd_continue(float tolerance, int iter) {
   for (;;) {
-    KMB_RET(update(iter));
-    g_prof.mark("centroid update");
+    KMB_RET(lloyd_update(iter));
     iter++;
     uint32_t changed = 0;
-    KMB_RET(assign_pass(&changed));
+    double shift = 0;
+    KMB_RET(assign_pass(&changed, center_shift ? &shift : nullptr));
     g_prof.mark("assign pass");
     KMB_INFO("iteration %d: %" PRIu32 " reassignments\n", iter, changed);
+    if (shift_stop(iter, changed, shift)) return kmcudaSuccess;
     if (changed <= tolerance * N) return kmcudaSuccess;
   }
 }
@@ -601,7 +700,7 @@ KMCUDAResult Job::yinyang(float tolerance, uint32_t G) {
   int iter = 0;
   uint32_t changed = 0;
   KMB_RET(lloyd(kYinyangDraftReassignments, &iter, &changed));
-  if (changed <= tolerance * N) return kmcudaSuccess;
+  if (n_iter || changed <= tolerance * N) return kmcudaSuccess;   // n_iter: the rule stopped the run in the draft
   std::vector<uint32_t> groups;
   KMB_RET(group_centroids(G, &groups));
   g_prof.mark("yinyang: group centroids");
@@ -626,8 +725,14 @@ KMCUDAResult Job::yinyang(float tolerance, uint32_t G) {
   for (;; iter++) {
     if (!refresh) {
       std::vector<uint32_t> c, p;
-      KMB_RET(gather([&](size_t i) { return devs[i].d_changed.get(); }, &c,
-                     [&](size_t i) { return devs[i].shard->yy_counters.get() + 1; }, &p));
+      std::vector<double> s(1, 0.0);
+      if (center_shift)
+        KMB_RET(gather([&](size_t i) { return devs[i].d_changed.get(); }, &c,
+                       [&](size_t i) { return devs[i].shard->yy_counters.get() + 1; }, &p,
+                       [&](size_t i) { return devs[i].d_shift.get(); }, &s));
+      else
+        KMB_RET(gather([&](size_t i) { return devs[i].d_changed.get(); }, &c,
+                       [&](size_t i) { return devs[i].shard->yy_counters.get() + 1; }, &p));
       uint32_t total_changed = 0, total_passed = 0;
       for (size_t i = 0; i < devs.size(); i++) {
         KMB_RET(devs[i].shard->check_pipeline());
@@ -635,6 +740,7 @@ KMCUDAResult Job::yinyang(float tolerance, uint32_t G) {
         total_passed += p[i];
       }
       KMB_INFO("iteration %d: %" PRIu32 " reassignments\n", iter, total_changed);
+      if (shift_stop(iter, total_changed, s[0])) return kmcudaSuccess;
       if (total_changed <= tolerance * N) return kmcudaSuccess;
       {
         const auto t_now = std::chrono::steady_clock::now();
@@ -669,6 +775,7 @@ KMCUDAResult Job::yinyang(float tolerance, uint32_t G) {
                              cudaMemcpyDeviceToDevice, d.st), kmcudaMemoryCopyError);
     }
     KMB_RET(update(iter));
+    if (center_shift) KMB_RET(shift_of(devs[0].shard->oldC.get()));
     g_prof.mark("centroid update");
     for (auto& d : devs) {
       KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
@@ -861,6 +968,7 @@ KMCUDAResult Job::restarts(KMCUDAInitMethod method, const void* init_params, uin
   }
   double best_inertia = 0;
   uint32_t best_r = 0;
+  int best_n_iter = 0;
   for (uint32_t r = 0; r < n_init; r++) {
     const uint32_t seed_r = seed + r * 0x9E3779B9u;
     lloyd_iter_ms = 0;
@@ -876,6 +984,7 @@ KMCUDAResult Job::restarts(KMCUDAInitMethod method, const void* init_params, uin
     if (r > 0 && !(e < best_inertia)) continue;
     best_inertia = e;
     best_r = r;
+    best_n_iter = n_iter;
     if (r + 1 == n_init) break;   // the last restart's state is already in place
     for (size_t i = 0; i < best.size(); i++) {
       Dev& d = devs[i];
@@ -897,6 +1006,7 @@ KMCUDAResult Job::restarts(KMCUDAInitMethod method, const void* init_params, uin
     }
   }
   if (n_init > 1) KMB_INFO("restarts: kept restart %" PRIu32 ", inertia %.17g\n", best_r, best_inertia);
+  n_iter = best_n_iter;
   if (inertia_out) *inertia_out = best_inertia;
   return kmcudaSuccess;
 }

@@ -55,6 +55,10 @@ struct Dev {
   DevBuf<float> rl_x;
   DevBuf<char> rl_tmp;
   uint32_t rl_cap = 0;
+  // scikit-learn's stopping rule (Job::center_shift): the centroids before a Lloyd update and the per-centroid squared
+  // moves (first device only), and the centre shift S read back with the next pass (every device, read from the first)
+  DevBuf<float> Cold;
+  DevBuf<double> dsq, d_shift;
   cudaEvent_t ev_partial = nullptr;   // this device's partial sums are complete
   cudaEvent_t ev_reduced = nullptr;   // this device has finished reading every peer's partial sums
   ncclComm_t comm = nullptr;          // owned by the per-process cache (Job::setup)
@@ -131,6 +135,12 @@ class Job {
   bool peer_exchange = false;   // multi-GPU update through peer memory (NVLink / NVSwitch) instead of NCCL
   bool weighted = false;        // per-sample weights (kmcuda_b200_kmeans_weighted); set before setup()
   bool relocate_empty = false;  // relocate empty clusters in update() (kmcuda_b200_kmeans_relocate)
+  // scikit-learn's stopping rule instead of the reference's (kmcuda_b200_kmeans_center_shift, DESIGN.md §4p); set before
+  // setup().  The runs are then given a negative reassignment tolerance, which never stops them.
+  bool center_shift = false;
+  double shift_tol = 0;         // tol times the mean per-feature variance (shift_tolerance)
+  uint32_t max_iter = 300;      // the last update of a run
+  int n_iter = 0;               // iterations of the last run (of the kept restart after restarts()), 0 while it runs
   uint32_t relocated = 0;       // rows relocated by the last relocate(), still in every device's rl_x / rl_meta
   double wtotal = 0;            // sum of the weights (check_weights)
   std::vector<float> host_w;    // host copy of the weights for the host-side seeding steps (load_host_weights)
@@ -178,8 +188,13 @@ class Job {
   KMCUDAResult init_afkmc2(uint32_t m, uint32_t seed);
   KMCUDAResult init_kmeans_parallel(uint32_t rounds, uint32_t seed);
   KMCUDAResult init_greedy_plusplus(uint32_t trials, uint32_t seed);
-  KMCUDAResult assign_pass(uint32_t* changed);
+  // *shift (with the rule): the centre shift of the update before this pass, read back in the same round trip
+  KMCUDAResult assign_pass(uint32_t* changed, double* shift = nullptr);
   KMCUDAResult update(int iter);
+  KMCUDAResult lloyd_update(int iter);
+  KMCUDAResult shift_of(const float* Cold);
+  KMCUDAResult shift_tolerance(float tol);
+  bool shift_stop(int iter, uint32_t changed, double shift);
   KMCUDAResult relocate(int iter);
   KMCUDAResult lloyd(float tolerance, int* iter_out, uint32_t* changed_out);
   KMCUDAResult lloyd_continue(float tolerance, int iter);

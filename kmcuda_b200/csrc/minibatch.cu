@@ -159,6 +159,16 @@ mb_stats_kernel(const double* __restrict__ dsq, const double* __restrict__ W, ui
   }
 }
 
+// out[0] = sum of dsq[K] with the non-finite terms as 0 (chunk_sum, fold_chunks): the centre shift of a Lloyd / Yinyang
+// update under scikit-learn's stopping rule, where a dead centroid (NaN) must not keep a run going
+__global__ void __launch_bounds__(1024)
+center_shift_fold_kernel(const double* __restrict__ dsq, uint32_t K, double* __restrict__ out) {
+  __shared__ double s_chunk[1024];
+  s_chunk[threadIdx.x] = chunk_sum<true>(dsq, K);
+  __syncthreads();
+  if (threadIdx.x == 0) out[0] = fold_chunks(s_chunk);
+}
+
 // per-feature variance, two passes in double: partial[b][f] over a contiguous row range per CTA, folded in CTA order
 constexpr int kVarBlocks = 256;
 __global__ void __launch_bounds__(256)
@@ -257,15 +267,32 @@ cudaError_t launch_mb_stats(const float* Cold, const float* Cnew, const double* 
   return cudaGetLastError();
 }
 
+cudaError_t launch_center_shift(const float* Cold, const float* Cnew, uint32_t K, int D, double* dsq, double* out,
+                                cudaStream_t st) {
+  mb_shift_kernel<<<K, 128, 0, st>>>(Cold, Cnew, D, dsq);
+  center_shift_fold_kernel<<<1, 1024, 0, st>>>(dsq, K, out);
+  return cudaGetLastError();
+}
+
 size_t mb_variance_doubles(int D) { return static_cast<size_t>(kVarBlocks) * D + 2 * static_cast<size_t>(D); }
 
+// out[f] = scale * (the column sum of x_f, or of (x_f - mean_f)^2), partials in work[kVarBlocks][D]
+static void col_pass(const float* X, uint32_t n, int D, const double* mean, double* work, double scale, double* out,
+                     cudaStream_t st) {
+  mb_colsum_kernel<<<kVarBlocks, 256, 0, st>>>(X, n, D, mean, work);
+  mb_colfold_kernel<<<cdiv(D, 256), 256, 0, st>>>(work, kVarBlocks, D, scale, out);
+}
+
 cudaError_t launch_mb_variance(const float* X, uint32_t n, int D, double* work, double* var, cudaStream_t st) {
-  double* partial = work;
   double* mean = work + static_cast<size_t>(kVarBlocks) * D;
-  mb_colsum_kernel<<<kVarBlocks, 256, 0, st>>>(X, n, D, nullptr, partial);
-  mb_colfold_kernel<<<cdiv(D, 256), 256, 0, st>>>(partial, kVarBlocks, D, 1.0 / n, mean);
-  mb_colsum_kernel<<<kVarBlocks, 256, 0, st>>>(X, n, D, mean, partial);
-  mb_colfold_kernel<<<cdiv(D, 256), 256, 0, st>>>(partial, kVarBlocks, D, 1.0 / n, var);
+  col_pass(X, n, D, nullptr, work, 1.0 / n, mean, st);
+  col_pass(X, n, D, mean, work, 1.0 / n, var, st);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_col_sums(const float* X, uint32_t n, int D, const double* mean, double* work, double* out,
+                            cudaStream_t st) {
+  col_pass(X, n, D, mean, work, 1.0, out, st);
   return cudaGetLastError();
 }
 

@@ -10,6 +10,7 @@
 #include <numpy/arrayobject.h>
 
 #include <cinttypes>
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <ctime>
@@ -158,6 +159,10 @@ bool take_weights(PyObject* obj, bool device_samples, uint32_t n, Ref* keep, con
   return true;
 }
 
+PyObject* build_kmeans_result(PyObject* centroids_arr, PyObject* assignments_arr, float* centroids,
+                              uint32_t* assignments, int device_ptrs, int adflag, float average_distance,
+                              bool want_inertia, double inertia);
+
 PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
   uint32_t clusters = 0, afkmc2_m = 0, seed = static_cast<uint32_t>(time(nullptr)), device = 0;
   int32_t verbosity = 0;
@@ -165,15 +170,15 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
   float tolerance = .01f, yinyang_t = .1f;
   PyObject *samples_obj, *init_obj = Py_None, *metric_obj = Py_None, *weight_obj = Py_None, *batch_obj = Py_None;
   PyObject *steps_obj = nullptr, *relocate_obj = Py_False, *n_init_obj = nullptr, *inertia_obj = Py_False;
-  PyObject *bisecting_obj = Py_None, *max_iter_obj = nullptr;
+  PyObject *bisecting_obj = Py_None, *max_iter_obj = nullptr, *tol_obj = Py_None, *n_iter_obj = Py_False;
   static const char* kwlist[] = {"samples", "clusters", "tolerance", "init", "yinyang_t", "metric",
                                  "average_distance", "seed", "device", "verbosity", "sample_weight", "batch_size",
                                  "max_steps", "relocate_empty_clusters", "n_init", "inertia", "bisecting",
-                                 "max_iter", nullptr};
-  if (!PyArg_ParseTupleAndKeywords(args, kwargs, "OI|fOfOpIIiOOOOOOOO", const_cast<char**>(kwlist), &samples_obj,
+                                 "max_iter", "tol", "n_iter", nullptr};
+  if (!PyArg_ParseTupleAndKeywords(args, kwargs, "OI|fOfOpIIiOOOOOOOOOO", const_cast<char**>(kwlist), &samples_obj,
                                    &clusters, &tolerance, &init_obj, &yinyang_t, &metric_obj, &adflag, &seed,
                                    &device, &verbosity, &weight_obj, &batch_obj, &steps_obj, &relocate_obj,
-                                   &n_init_obj, &inertia_obj, &bisecting_obj, &max_iter_obj))
+                                   &n_init_obj, &inertia_obj, &bisecting_obj, &max_iter_obj, &tol_obj, &n_iter_obj))
     return nullptr;
   // bisecting k-means (kmcuda_b200.h, kmcuda_b200_kmeans_bisecting): None or a strategy name
   int32_t strategy = -1;
@@ -244,10 +249,44 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
       return nullptr;
     }
   }
+  // scikit-learn's stopping rule (kmcuda_b200.h, kmcuda_b200_kmeans_center_shift): tol None or a real number >= 0,
+  // n_iter a bool that needs tol; not with mini-batch or bisecting
+  const bool center_shift = tol_obj != Py_None;
+  double tol = 0;
+  if (center_shift) {
+    if (PyBool_Check(tol_obj) || PyArray_IsScalar(tol_obj, Bool) ||
+        !(PyFloat_Check(tol_obj) || PyLong_Check(tol_obj) || PyArray_IsScalar(tol_obj, Floating) ||
+          PyArray_IsScalar(tol_obj, Integer))) {
+      PyErr_SetString(PyExc_TypeError, "\"tol\" must be None or a real number");
+      return nullptr;
+    }
+    tol = PyFloat_AsDouble(tol_obj);
+    if (PyErr_Occurred()) return nullptr;
+    if (!(std::isfinite(tol) && tol >= 0)) {
+      PyErr_SetString(PyExc_ValueError, "\"tol\" must be a finite number >= 0");
+      return nullptr;
+    }
+    if (batch_obj != Py_None || strategy >= 0) {
+      PyErr_SetString(PyExc_ValueError, "\"tol\" applies to Lloyd / Yinyang runs: mini-batch (\"batch_size\") and "
+                                        "bisecting runs scale \"tolerance\" themselves");
+      return nullptr;
+    }
+  }
+  if (!(PyBool_Check(n_iter_obj) || PyArray_IsScalar(n_iter_obj, Bool))) {
+    PyErr_SetString(PyExc_TypeError, "\"n_iter\" must be a bool");
+    return nullptr;
+  }
+  const bool want_n_iter = PyObject_IsTrue(n_iter_obj) == 1;
+  if (want_n_iter && !center_shift) {
+    PyErr_SetString(PyExc_ValueError, "\"n_iter\" needs \"tol\": only runs with scikit-learn's stopping rule count "
+                                      "iterations");
+    return nullptr;
+  }
   uint32_t max_iter = 0;
   if (max_iter_obj && !take_count(max_iter_obj, "max_iter", 0, &max_iter)) return nullptr;
-  if (max_iter && strategy < 0) {
-    PyErr_SetString(PyExc_ValueError, "\"max_iter\" applies to bisecting runs only: pass \"bisecting\" too");
+  if (max_iter && strategy < 0 && !center_shift) {
+    PyErr_SetString(PyExc_ValueError, "\"max_iter\" applies to bisecting runs and runs with \"tol\" only: pass one "
+                                      "of them too");
     return nullptr;
   }
   // restarts (kmcuda_b200.h, kmcuda_b200_kmeans_restarts): n_init an integer >= 1, inertia a bool; not with mini-batch
@@ -419,13 +458,20 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
   }
   float average_distance = 0;
   double inertia = 0;
+  uint32_t n_iter = 0;
   int result;
   if (batch_size && yinyang_t > 0 && verbosity > 0) {
     printf("mini-batch k-means: yinyang_t is ignored\n");
     fflush(stdout);
   }
   Py_BEGIN_ALLOW_THREADS
-  if (strategy >= 0)
+  if (center_shift)
+    result = kmcuda_b200_kmeans_center_shift(init, &afkmc2_m, static_cast<float>(tol), yinyang_t, metric, n,
+                                             static_cast<uint16_t>(d), clusters, seed, device, device_ptrs, fp16x2,
+                                             verbosity, samples, weights, relocate ? 1 : 0, n_init, max_iter, centroids,
+                                             assignments, adflag ? &average_distance : nullptr,
+                                             want_inertia ? &inertia : nullptr, want_n_iter ? &n_iter : nullptr);
+  else if (strategy >= 0)
     result = kmcuda_b200_kmeans_bisecting(init, &afkmc2_m, tolerance, metric, n, static_cast<uint16_t>(d), clusters,
                                           seed, device, device_ptrs, fp16x2, verbosity, samples, weights, strategy,
                                           n_init, max_iter, centroids, assignments,
@@ -453,18 +499,33 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
                          adflag ? &average_distance : nullptr);
   Py_END_ALLOW_THREADS
   if (result != kmcudaSuccess) return raise_for(result, "kmeans_cuda");
+  if (want_n_iter) {   // the result below with the iteration count appended
+    Ref head(build_kmeans_result(centroids_arr.p, assignments_arr.p, centroids, assignments, device_ptrs, adflag,
+                                 average_distance, want_inertia, inertia));
+    Ref tail(Py_BuildValue("(k)", static_cast<unsigned long>(n_iter)));
+    if (!head.p || !tail.p) return nullptr;
+    return PySequence_Concat(head.p, tail.p);
+  }
+  return build_kmeans_result(centroids_arr.p, assignments_arr.p, centroids, assignments, device_ptrs, adflag,
+                             average_distance, want_inertia, inertia);
+}
+
+// (centroids, assignments[, avg][, inertia]): arrays for host samples, raw device pointers for device samples
+PyObject* build_kmeans_result(PyObject* centroids_arr, PyObject* assignments_arr, float* centroids,
+                              uint32_t* assignments, int device_ptrs, int adflag, float average_distance,
+                              bool want_inertia, double inertia) {
   if (want_inertia) {
     if (device_ptrs < 0) {
-      if (!adflag) return Py_BuildValue("OOd", centroids_arr.p, assignments_arr.p, inertia);
-      return Py_BuildValue("OOfd", centroids_arr.p, assignments_arr.p, average_distance, inertia);
+      if (!adflag) return Py_BuildValue("OOd", centroids_arr, assignments_arr, inertia);
+      return Py_BuildValue("OOfd", centroids_arr, assignments_arr, average_distance, inertia);
     }
     const unsigned long long cp = reinterpret_cast<uintptr_t>(centroids), ap = reinterpret_cast<uintptr_t>(assignments);
     if (!adflag) return Py_BuildValue("KKd", cp, ap, inertia);
     return Py_BuildValue("KKfd", cp, ap, average_distance, inertia);
   }
   if (device_ptrs < 0) {
-    if (!adflag) return Py_BuildValue("OO", centroids_arr.p, assignments_arr.p);
-    return Py_BuildValue("OOf", centroids_arr.p, assignments_arr.p, average_distance);
+    if (!adflag) return Py_BuildValue("OO", centroids_arr, assignments_arr);
+    return Py_BuildValue("OOf", centroids_arr, assignments_arr, average_distance);
   }
   const unsigned long long cp = reinterpret_cast<uintptr_t>(centroids), ap = reinterpret_cast<uintptr_t>(assignments);
   if (!adflag) return Py_BuildValue("KK", cp, ap);
@@ -585,8 +646,10 @@ PyObject* py_knn_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
 char module_doc[] = "K-means and K-nn on NVIDIA H100 (drop-in for src-d/kmcuda's libKMCUDA).";
 char kmeans_doc[] = "kmeans_cuda(samples, clusters, tolerance=.01, init=\"k-means++\", yinyang_t=.1, metric=\"L2\", "
                     "average_distance=False, seed=time(), device=0, verbosity=0, sample_weight=None, batch_size=None, "
-                    "max_steps=0, relocate_empty_clusters=False, n_init=1, inertia=False, bisecting=None, max_iter=0) -> "
-                    "(centroids, assignments[, avg][, inertia])";
+                    "max_steps=0, relocate_empty_clusters=False, n_init=1, inertia=False, bisecting=None, max_iter=0, "
+                    "tol=None, n_iter=False) -> (centroids, assignments[, avg][, inertia][, n_iter]).  tol (a real "
+                    "number >= 0) stops Lloyd / Yinyang runs by scikit-learn's KMeans rule with max_iter (0 = 300) and "
+                    "ignores tolerance; n_iter=True (needs tol) appends the run's iteration count.";
 char knn_doc[] = "knn_cuda(k, samples, centroids, assignments, metric=\"L2\", device=0, verbosity=0) -> neighbors";
 
 PyMethodDef module_functions[] = {
