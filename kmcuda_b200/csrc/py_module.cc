@@ -118,8 +118,46 @@ PyObject* raise_for(int result, const char* fn) {
   return nullptr;
 }
 
-void* as_pointer(PyObject* o) {
-  return reinterpret_cast<void*>(static_cast<uintptr_t>(PyLong_AsUnsignedLongLong(o)));
+// the int members of the device-pointer tuples and of init=("afkmc2", m), Python ints or NumPy integers: false, with
+// the Python error set, when `o` is not one or is out of range (negative, except for the device)
+bool as_ull(PyObject* o, unsigned long long* out) {
+  Ref i(PyNumber_Index(o));
+  if (!i.p) return false;
+  *out = PyLong_AsUnsignedLongLong(i.p);
+  return !(*out == static_cast<unsigned long long>(-1) && PyErr_Occurred());
+}
+
+template <typename T>
+bool as_pointer(PyObject* o, T** p) {
+  unsigned long long v;
+  if (!as_ull(o, &v)) return false;
+  *p = reinterpret_cast<T*>(static_cast<uintptr_t>(v));
+  return true;
+}
+
+bool as_u32(PyObject* o, uint32_t* out) {
+  unsigned long long v;
+  if (!as_ull(o, &v)) return false;
+  *out = static_cast<uint32_t>(v);
+  return true;
+}
+
+bool as_int(PyObject* o, int* out) {
+  const long v = PyLong_AsLong(o);
+  if (v == -1 && PyErr_Occurred()) return false;
+  *out = static_cast<int>(v);
+  return true;
+}
+
+// the shape member of a device-pointer samples tuple: (n, d) or (n, d, fp16x2)
+bool take_shape(PyObject* shape, uint32_t* n, uint32_t* d, bool* fp16x2) {
+  if (!PyTuple_Check(shape) || (PyTuple_GET_SIZE(shape) != 2 && PyTuple_GET_SIZE(shape) != 3)) {
+    PyErr_SetString(PyExc_TypeError, "\"samples\"[2] must be a shape tuple");
+    return false;
+  }
+  if (!as_u32(PyTuple_GET_ITEM(shape, 0), n) || !as_u32(PyTuple_GET_ITEM(shape, 1), d)) return false;
+  if (PyTuple_GET_SIZE(shape) == 3) *fp16x2 = PyObject_IsTrue(PyTuple_GET_ITEM(shape, 2)) == 1;
+  return true;
 }
 
 // sample_weight intake: with ndarray samples a 1-D numeric array-like of length n (converted to float32, kept alive in
@@ -131,8 +169,7 @@ bool take_weights(PyObject* obj, bool device_samples, uint32_t n, Ref* keep, con
                                        "pointer tuple");
       return false;
     }
-    *data = static_cast<const float*>(as_pointer(obj));
-    if (PyErr_Occurred()) return false;
+    if (!as_pointer(obj, data)) return false;
     if (!*data) {
       PyErr_SetString(PyExc_ValueError, "\"sample_weight\" is null");
       return false;
@@ -164,7 +201,8 @@ PyObject* build_kmeans_result(PyObject* centroids_arr, PyObject* assignments_arr
                               bool want_inertia, double inertia);
 
 PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
-  uint32_t clusters = 0, afkmc2_m = 0, seed = static_cast<uint32_t>(time(nullptr)), device = 0;
+  long long clusters_arg = 0;   // range-checked below: "I" would wrap it modulo 2^32
+  uint32_t afkmc2_m = 0, seed = static_cast<uint32_t>(time(nullptr)), device = 0;
   int32_t verbosity = 0;
   int adflag = 0;
   float tolerance = .01f, yinyang_t = .1f;
@@ -175,8 +213,8 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
                                  "average_distance", "seed", "device", "verbosity", "sample_weight", "batch_size",
                                  "max_steps", "relocate_empty_clusters", "n_init", "inertia", "bisecting",
                                  "max_iter", "tol", "n_iter", nullptr};
-  if (!PyArg_ParseTupleAndKeywords(args, kwargs, "OI|fOfOpIIiOOOOOOOOOO", const_cast<char**>(kwlist), &samples_obj,
-                                   &clusters, &tolerance, &init_obj, &yinyang_t, &metric_obj, &adflag, &seed,
+  if (!PyArg_ParseTupleAndKeywords(args, kwargs, "OL|fOfOpIIiOOOOOOOOOO", const_cast<char**>(kwlist), &samples_obj,
+                                   &clusters_arg, &tolerance, &init_obj, &yinyang_t, &metric_obj, &adflag, &seed,
                                    &device, &verbosity, &weight_obj, &batch_obj, &steps_obj, &relocate_obj,
                                    &n_init_obj, &inertia_obj, &bisecting_obj, &max_iter_obj, &tol_obj, &n_iter_obj))
     return nullptr;
@@ -333,8 +371,9 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
       return nullptr;
     }
     if (!named_init(first)) return nullptr;
-    if (PyTuple_Size(init_obj) > 1 && init == kmcudaInitMethodAFKMC2)
-      afkmc2_m = static_cast<uint32_t>(PyLong_AsUnsignedLong(PyTuple_GetItem(init_obj, 1)));
+    if (PyTuple_Size(init_obj) > 1 && init == kmcudaInitMethodAFKMC2 &&
+        !as_u32(PyTuple_GetItem(init_obj, 1), &afkmc2_m))
+      return nullptr;
     const bool greedy = init == kmcudaInitMethodGreedyPlusPlus;
     if (PyTuple_Size(init_obj) > 1 && (init == kmcudaInitMethodKMeansParallel || greedy)) {
       // k-means|| rounds or greedy k-means++ trials: an integer in [0, 32]
@@ -365,10 +404,11 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
   }
   KMCUDADistanceMetric metric;
   if (!parse_metric(metric_obj, &metric)) return nullptr;
-  if (clusters < 2 || clusters == UINT32_MAX) {
+  if (clusters_arg < 2 || clusters_arg >= UINT32_MAX) {
     PyErr_SetString(PyExc_ValueError, "\"clusters\" must be greater than 1 and less than (1 << 32) - 1");
     return nullptr;
   }
+  const uint32_t clusters = static_cast<uint32_t>(clusters_arg);
   float *samples = nullptr, *centroids = nullptr;
   uint32_t* assignments = nullptr;
   uint32_t n = 0, d = 0;
@@ -381,29 +421,21 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
       PyErr_SetString(PyExc_ValueError, "len(\"samples\") must be either 3 or 5");
       return nullptr;
     }
-    PyObject* ptr = PyTuple_GetItem(samples_obj, 0);
-    PyObject* shape = PyTuple_GetItem(samples_obj, 2);
+    PyObject* ptr = PyTuple_GET_ITEM(samples_obj, 0);
     if (!PyLong_Check(ptr)) {
       PyErr_SetString(PyExc_ValueError, "\"samples\"[0] is not a pointer (integer)");
       return nullptr;
     }
-    samples = static_cast<float*>(as_pointer(ptr));
+    if (!as_pointer(ptr, &samples)) return nullptr;
     if (!samples) {
       PyErr_SetString(PyExc_ValueError, "\"samples\"[0] is null");
       return nullptr;
     }
-    device_ptrs = static_cast<int>(PyLong_AsLong(PyTuple_GetItem(samples_obj, 1)));
-    if (!PyTuple_Check(shape) || (PyTuple_GET_SIZE(shape) != 2 && PyTuple_GET_SIZE(shape) != 3)) {
-      PyErr_SetString(PyExc_TypeError, "\"samples\"[2] must be a shape tuple");
+    if (!as_int(PyTuple_GET_ITEM(samples_obj, 1), &device_ptrs)) return nullptr;
+    if (!take_shape(PyTuple_GET_ITEM(samples_obj, 2), &n, &d, &fp16x2)) return nullptr;
+    if (size == 5 && (!as_pointer(PyTuple_GET_ITEM(samples_obj, 3), &centroids) ||
+                      !as_pointer(PyTuple_GET_ITEM(samples_obj, 4), &assignments)))
       return nullptr;
-    }
-    n = static_cast<uint32_t>(PyLong_AsUnsignedLong(PyTuple_GetItem(shape, 0)));
-    d = static_cast<uint32_t>(PyLong_AsUnsignedLong(PyTuple_GetItem(shape, 1)));
-    if (PyTuple_GET_SIZE(shape) == 3) fp16x2 = PyObject_IsTrue(PyTuple_GetItem(shape, 2)) == 1;
-    if (size == 5) {
-      centroids = static_cast<float*>(as_pointer(PyTuple_GetItem(samples_obj, 3)));
-      assignments = static_cast<uint32_t*>(as_pointer(PyTuple_GetItem(samples_obj, 4)));
-    }
   } else if (!take_samples(samples_obj, &keep_samples, &samples, &fp16x2, &n, &d)) {
     return nullptr;
   }
@@ -460,43 +492,32 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
   double inertia = 0;
   uint32_t n_iter = 0;
   int result;
-  if (batch_size && yinyang_t > 0 && verbosity > 0) {
-    printf("mini-batch k-means: yinyang_t is ignored\n");
+  if ((batch_size || strategy >= 0) && yinyang_t > 0 && verbosity > 0) {
+    printf("%s k-means: yinyang_t is ignored\n", batch_size ? "mini-batch" : "bisecting");
     fflush(stdout);
   }
+  float* const avg = adflag ? &average_distance : nullptr;
+  double* const inertia_out = want_inertia ? &inertia : nullptr;
+  const uint16_t features = static_cast<uint16_t>(d);
   Py_BEGIN_ALLOW_THREADS
   if (center_shift)
-    result = kmcuda_b200_kmeans_center_shift(init, &afkmc2_m, static_cast<float>(tol), yinyang_t, metric, n,
-                                             static_cast<uint16_t>(d), clusters, seed, device, device_ptrs, fp16x2,
-                                             verbosity, samples, weights, relocate ? 1 : 0, n_init, max_iter, centroids,
-                                             assignments, adflag ? &average_distance : nullptr,
-                                             want_inertia ? &inertia : nullptr, want_n_iter ? &n_iter : nullptr);
+    result = kmcuda_b200_kmeans_center_shift(init, &afkmc2_m, static_cast<float>(tol), yinyang_t, metric, n, features,
+                                             clusters, seed, device, device_ptrs, fp16x2, verbosity, samples, weights,
+                                             relocate ? 1 : 0, n_init, max_iter, centroids, assignments, avg,
+                                             inertia_out, want_n_iter ? &n_iter : nullptr);
   else if (strategy >= 0)
-    result = kmcuda_b200_kmeans_bisecting(init, &afkmc2_m, tolerance, metric, n, static_cast<uint16_t>(d), clusters,
-                                          seed, device, device_ptrs, fp16x2, verbosity, samples, weights, strategy,
-                                          n_init, max_iter, centroids, assignments,
-                                          adflag ? &average_distance : nullptr, want_inertia ? &inertia : nullptr);
-  else if (n_init != 1 || want_inertia)
-    result = kmcuda_b200_kmeans_restarts(init, &afkmc2_m, tolerance, yinyang_t, metric, n, static_cast<uint16_t>(d),
-                                         clusters, seed, device, device_ptrs, fp16x2, verbosity, samples, weights,
-                                         relocate ? 1 : 0, n_init, centroids, assignments,
-                                         adflag ? &average_distance : nullptr, want_inertia ? &inertia : nullptr);
+    result = kmcuda_b200_kmeans_bisecting(init, &afkmc2_m, tolerance, metric, n, features, clusters, seed, device,
+                                          device_ptrs, fp16x2, verbosity, samples, weights, strategy, n_init, max_iter,
+                                          centroids, assignments, avg, inertia_out);
   else if (batch_size)
-    result = kmcuda_b200_kmeans_minibatch(init, &afkmc2_m, tolerance, metric, n, static_cast<uint16_t>(d), clusters,
-                                          seed, device, device_ptrs, fp16x2, verbosity, samples, weights, batch_size,
-                                          max_steps, centroids, assignments, adflag ? &average_distance : nullptr);
-  else if (relocate)
-    result = kmcuda_b200_kmeans_relocate(init, &afkmc2_m, tolerance, yinyang_t, metric, n, static_cast<uint16_t>(d),
-                                         clusters, seed, device, device_ptrs, fp16x2, verbosity, samples, weights,
-                                         centroids, assignments, adflag ? &average_distance : nullptr);
-  else if (weights)
-    result = kmcuda_b200_kmeans_weighted(init, &afkmc2_m, tolerance, yinyang_t, metric, n, static_cast<uint16_t>(d),
-                                         clusters, seed, device, device_ptrs, fp16x2, verbosity, samples, weights,
-                                         centroids, assignments, adflag ? &average_distance : nullptr);
-  else
-    result = kmeans_cuda(init, &afkmc2_m, tolerance, yinyang_t, metric, n, static_cast<uint16_t>(d), clusters, seed,
-                         device, device_ptrs, fp16x2, verbosity, samples, centroids, assignments,
-                         adflag ? &average_distance : nullptr);
+    result = kmcuda_b200_kmeans_minibatch(init, &afkmc2_m, tolerance, metric, n, features, clusters, seed, device,
+                                          device_ptrs, fp16x2, verbosity, samples, weights, batch_size, max_steps,
+                                          centroids, assignments, avg);
+  else   // Lloyd / Yinyang with any weights, relocation and n_init: with n_init 1 and no inertia the header documents
+         // this call as bit-identical to kmeans_cuda(), _weighted() and _relocate()
+    result = kmcuda_b200_kmeans_restarts(init, &afkmc2_m, tolerance, yinyang_t, metric, n, features, clusters, seed,
+                                         device, device_ptrs, fp16x2, verbosity, samples, weights, relocate ? 1 : 0,
+                                         n_init, centroids, assignments, avg, inertia_out);
   Py_END_ALLOW_THREADS
   if (result != kmcudaSuccess) return raise_for(result, "kmeans_cuda");
   if (want_n_iter) {   // the result below with the iteration count appended
@@ -533,16 +554,17 @@ PyObject* build_kmeans_result(PyObject* centroids_arr, PyObject* assignments_arr
 }
 
 PyObject* py_knn_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
-  uint32_t device = 0, k = 0;
+  uint32_t device = 0;
+  long long k = 0;   // range-checked below: "I" would wrap it modulo 2^32
   int32_t verbosity = 0;
   PyObject *samples_obj, *centroids_obj, *assignments_obj, *metric_obj = Py_None;
   static const char* kwlist[] = {"k", "samples", "centroids", "assignments", "metric", "device", "verbosity", nullptr};
-  if (!PyArg_ParseTupleAndKeywords(args, kwargs, "IOOO|OIi", const_cast<char**>(kwlist), &k, &samples_obj,
+  if (!PyArg_ParseTupleAndKeywords(args, kwargs, "LOOO|OIi", const_cast<char**>(kwlist), &k, &samples_obj,
                                    &centroids_obj, &assignments_obj, &metric_obj, &device, &verbosity))
     return nullptr;
   KMCUDADistanceMetric metric;
   if (!parse_metric(metric_obj, &metric)) return nullptr;
-  if (k == 0 || k > UINT16_MAX) {
+  if (k <= 0 || k > UINT16_MAX) {
     PyErr_SetString(PyExc_ValueError, "\"k\" must be greater than 0 and less than (1 << 16)");
     return nullptr;
   }
@@ -561,27 +583,22 @@ PyObject* py_knn_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
       PyErr_SetString(PyExc_ValueError, "\"centroids\" must be a tuple of length 2");
       return nullptr;
     }
-    samples = static_cast<float*>(as_pointer(PyTuple_GetItem(samples_obj, 0)));
-    device_ptrs = static_cast<int>(PyLong_AsLong(PyTuple_GetItem(samples_obj, 1)));
-    PyObject* shape = PyTuple_GetItem(samples_obj, 2);
-    if (!PyTuple_Check(shape) || (PyTuple_GET_SIZE(shape) != 2 && PyTuple_GET_SIZE(shape) != 3)) {
-      PyErr_SetString(PyExc_TypeError, "\"samples\"[2] must be a shape tuple");
+    if (!as_pointer(PyTuple_GET_ITEM(samples_obj, 0), &samples) ||
+        !as_int(PyTuple_GET_ITEM(samples_obj, 1), &device_ptrs) ||
+        !take_shape(PyTuple_GET_ITEM(samples_obj, 2), &n, &d, &fp16x2) ||
+        !as_pointer(PyTuple_GET_ITEM(centroids_obj, 0), &centroids) ||
+        !as_u32(PyTuple_GET_ITEM(centroids_obj, 1), &clusters))
       return nullptr;
-    }
-    n = static_cast<uint32_t>(PyLong_AsUnsignedLong(PyTuple_GetItem(shape, 0)));
-    d = static_cast<uint32_t>(PyLong_AsUnsignedLong(PyTuple_GetItem(shape, 1)));
-    if (PyTuple_GET_SIZE(shape) == 3) fp16x2 = PyObject_IsTrue(PyTuple_GetItem(shape, 2)) == 1;
-    centroids = static_cast<float*>(as_pointer(PyTuple_GetItem(centroids_obj, 0)));
-    clusters = static_cast<uint32_t>(PyLong_AsUnsignedLong(PyTuple_GetItem(centroids_obj, 1)));
     if (PyTuple_Check(assignments_obj)) {
       if (PyTuple_GET_SIZE(assignments_obj) != 2) {
         PyErr_SetString(PyExc_ValueError, "\"assignments\" must be a pointer or a tuple of length 2");
         return nullptr;
       }
-      assignments = static_cast<uint32_t*>(as_pointer(PyTuple_GetItem(assignments_obj, 0)));
-      neighbors = static_cast<uint32_t*>(as_pointer(PyTuple_GetItem(assignments_obj, 1)));
-    } else {
-      assignments = static_cast<uint32_t*>(as_pointer(assignments_obj));
+      if (!as_pointer(PyTuple_GET_ITEM(assignments_obj, 0), &assignments) ||
+          !as_pointer(PyTuple_GET_ITEM(assignments_obj, 1), &neighbors))
+        return nullptr;
+    } else if (!as_pointer(assignments_obj, &assignments)) {
+      return nullptr;
     }
     if (!samples || !centroids || !assignments) {
       PyErr_SetString(PyExc_ValueError, "null pointer");
@@ -647,9 +664,8 @@ char module_doc[] = "K-means and K-nn on NVIDIA H100 (drop-in for src-d/kmcuda's
 char kmeans_doc[] = "kmeans_cuda(samples, clusters, tolerance=.01, init=\"k-means++\", yinyang_t=.1, metric=\"L2\", "
                     "average_distance=False, seed=time(), device=0, verbosity=0, sample_weight=None, batch_size=None, "
                     "max_steps=0, relocate_empty_clusters=False, n_init=1, inertia=False, bisecting=None, max_iter=0, "
-                    "tol=None, n_iter=False) -> (centroids, assignments[, avg][, inertia][, n_iter]).  tol (a real "
-                    "number >= 0) stops Lloyd / Yinyang runs by scikit-learn's KMeans rule with max_iter (0 = 300) and "
-                    "ignores tolerance; n_iter=True (needs tol) appends the run's iteration count.";
+                    "tol=None, n_iter=False) -> (centroids, assignments[, avg][, inertia][, n_iter]).  The keywords "
+                    "are described in the kmcuda_b200 package's docstring.";
 char knn_doc[] = "knn_cuda(k, samples, centroids, assignments, metric=\"L2\", device=0, verbosity=0) -> neighbors";
 
 PyMethodDef module_functions[] = {
