@@ -117,6 +117,35 @@ KMCUDAResult kmcuda_b200_kmeans_minibatch(KMCUDAInitMethod init, const void *ini
                                           const float *weights, uint32_t batch_size, uint32_t max_steps,
                                           float *centroids, uint32_t *assignments, float *average_distance);
 
+/* init_size of kmcuda_b200_kmeans_minibatch_init(): scikit-learn's default, m = 3 b (b = min(batch_size,
+ * samples_size)), 3 clusters_size when that is below clusters_size, at most samples_size. */
+#define KMCUDA_B200_INIT_SIZE_AUTO 0xFFFFFFFFu
+
+/* Mini-batch k-means with scikit-learn's MiniBatchKMeans init stage (init_size, n_init): kmcuda_b200_kmeans_minibatch()
+ * whose seeding reads m = init_size rows instead of all of them, best of n_init inits.  The parameters are those of
+ * _minibatch, plus init_size (0 = seed on all rows, which with n_init == 1 is exactly _minibatch;
+ * KMCUDA_B200_INIT_SIZE_AUTO = scikit-learn's default above; else m = min(init_size, samples_size)) and n_init.  Init r
+ * (r = 0 .. n_init - 1) seeds with seed_r = seed + r * 0x9E3779B9 (mod 2^32), the schedule of _restarts.  When
+ * m < samples_size it seeds on the m rows row_j = floor(u * samples_size), u a counter hash of (seed, r, j) with its
+ * own tag, drawn with replacement (not by weight), each with its weight: exactly the seeding of a
+ * kmcuda_b200_kmeans_weighted() call on those rows with seed_r, for every init method but kmcudaInitMethodImport;
+ * otherwise on all rows with seed_r.  With n_init > 1, m validation rows are drawn the same way (their own tag, r = 0),
+ * assigned to each init's centroids by the reference's argmin, and the init is ranked by sum w e over them (duplicates
+ * included, e the Kahan sum of squared differences, 0 for a row without a centroid); init 0 is the first best and a
+ * later one replaces it only with a strictly lower value (NaN never wins).  The mini-batch steps then run from the kept
+ * centroids with `seed` exactly as in _minibatch.  Verbosity >= 1 with init_size != 0 adds, after each seeding's own
+ * lines, "mini-batch init r/n_init: seed s, m rows" (r from 1), with ", validation inertia %.17g" when n_init > 1, and
+ * then "mini-batch init: kept init r/n_init".  kmcudaInvalidArguments: what _minibatch rejects, n_init == 0, n_init > 1
+ * with init_size == 0, init_size != 0 with kmcudaInitMethodImport, an init_size below clusters_size other than 0 and
+ * KMCUDA_B200_INIT_SIZE_AUTO, and sampled rows whose weights sum to 0. */
+KMCUDAResult kmcuda_b200_kmeans_minibatch_init(KMCUDAInitMethod init, const void *init_params, float tolerance,
+                                               KMCUDADistanceMetric metric, uint32_t samples_size,
+                                               uint16_t features_size, uint32_t clusters_size, uint32_t seed,
+                                               uint32_t device, int32_t device_ptrs, int32_t fp16x2, int32_t verbosity,
+                                               const float *samples, const float *weights, uint32_t batch_size,
+                                               uint32_t max_steps, uint32_t init_size, uint32_t n_init,
+                                               float *centroids, uint32_t *assignments, float *average_distance);
+
 /* k-means restarts, scikit-learn's KMeans(n_init=...): n_init seedings and runs over one ingest of the samples, keeping
  * the run of lowest inertia.  The parameters up to `weights` are those of kmcuda_b200_kmeans_relocate(); restart r
  * (r = 0 .. n_init - 1) is exactly what one kmcuda_b200_kmeans_relocate() call (relocate_empty_clusters != 0) or one

@@ -9,7 +9,8 @@ Python surface = the reference's `libKMCUDA` module (reference src/python.cc:33-
                 relocate_empty_clusters=False,                                # extension: scikit-learn's relocation
                 n_init=1, inertia=False,                                      # extension: restarts, inertia
                 bisecting=None, max_iter=0,                                   # extension: bisecting k-means
-                tol=None, n_iter=False)                                       # extension: scikit-learn's stop rule
+                tol=None, n_iter=False,                                       # extension: scikit-learn's stop rule
+                init_size=None)                                               # extension: mini-batch init stage
                 init="k-means||" / ("k-means||", rounds)                      # extension: k-means|| seeding
     knn_cuda(k, samples, centroids, assignments, metric="L2", device=0, verbosity=0)  # python.cc:412-632
     supports_fp16                                                             # python.cc:52
@@ -33,6 +34,13 @@ batch_size: an int >= 1 runs mini-batch k-means (kmcuda_b200_kmeans_minibatch, s
 with batches of min(batch_size, N) rows for at most max_steps steps (0 = 100 * N // batch size) on one GPU, L2
 only; yinyang_t is ignored.  None = the Lloyd / Yinyang run.
 
+init_size: with batch_size, the number of rows the seeding reads (kmcuda_b200_kmeans_minibatch_init, scikit-learn's
+MiniBatchKMeans init_size): an int >= clusters, or "auto" for scikit-learn's default 3 * batch size (3 * clusters
+when that is smaller than clusters), at most N.  Init r seeds with (seed + r * 0x9E3779B9) mod 2^32 on that many rows
+drawn uniformly with replacement, with their weights, exactly as a call on those rows would seed; n_init such inits
+are ranked by their inertia on as many validation rows and the lowest is kept, then the mini-batch steps run as
+without init_size.  Not with an ndarray init or bisecting.  None = seed on all rows, and then n_init must be 1.
+
 relocate_empty_clusters: True moves every cluster that ends an update without members to one of the samples
 farthest from their centroids (kmcuda_b200_kmeans_relocate, scikit-learn's KMeans rule) instead of leaving a NaN
 centroid; not with batch_size (mini-batch has its own reassignment).
@@ -40,7 +48,7 @@ centroid; not with batch_size (mini-batch has its own reassignment).
 n_init: an int >= 1, the number of restarts (kmcuda_b200_kmeans_restarts, scikit-learn's KMeans n_init): restart r
 seeds with (seed + r * 0x9E3779B9) mod 2^32 and runs Lloyd / Yinyang as a fresh call would, on one ingest of the
 samples; the run of lowest inertia is returned (ties keep the earlier restart).  Not with an ndarray init (every
-restart would be the same run) nor with batch_size.
+restart would be the same run).  With batch_size it needs init_size and counts the inits of the mini-batch run.
 
 inertia: True appends the returned run's inertia, sum w * ||x - c||^2 (angular: w * angle^2) as a float, to the
 result; not with batch_size.
@@ -94,6 +102,9 @@ _lib.kmcuda_b200_kmeans_relocate.argtypes = _lib.kmcuda_b200_kmeans_weighted.arg
 _lib.kmcuda_b200_kmeans_minibatch.restype = ctypes.c_int
 _lib.kmcuda_b200_kmeans_minibatch.argtypes = _lib.kmeans_cuda.argtypes[:3] + _lib.kmeans_cuda.argtypes[4:14] + \
     [ctypes.c_void_p, ctypes.c_uint32, ctypes.c_uint32] + _lib.kmeans_cuda.argtypes[14:]
+_lib.kmcuda_b200_kmeans_minibatch_init.restype = ctypes.c_int
+_lib.kmcuda_b200_kmeans_minibatch_init.argtypes = _lib.kmcuda_b200_kmeans_minibatch.argtypes[:16] + \
+    [ctypes.c_uint32, ctypes.c_uint32] + _lib.kmeans_cuda.argtypes[14:]
 _lib.kmcuda_b200_kmeans_restarts.restype = ctypes.c_int
 _lib.kmcuda_b200_kmeans_restarts.argtypes = _lib.kmeans_cuda.argtypes[:14] + \
     [ctypes.c_void_p, ctypes.c_int32, ctypes.c_uint32] + _lib.kmeans_cuda.argtypes[14:] + [ctypes.c_void_p]
@@ -116,6 +127,7 @@ INIT_RANDOM, INIT_PLUSPLUS, INIT_AFKMC2, INIT_IMPORT = range(4)
 INIT_KMEANS_PARALLEL = 4   # kmcudaInitMethodKMeansParallel
 INIT_GREEDY_PLUSPLUS = 5   # kmcudaInitMethodGreedyPlusPlus
 METRIC_L2, METRIC_COSINE = range(2)
+INIT_SIZE_AUTO = 0xFFFFFFFF   # KMCUDA_B200_INIT_SIZE_AUTO
 
 # `import libKMCUDA` from the same file: one dlopen, so _lib and the extension share the library's state
 _loader = importlib.machinery.ExtensionFileLoader("libKMCUDA", LIB_PATH)

@@ -69,7 +69,7 @@ namespace {
 enum class Route { kLloyd, kMinibatch, kBisecting };
 
 // one k-means call, filled by name by each entry point (kmeans_cuda, kmcuda_b200_kmeans_weighted, _relocate,
-// _minibatch, _restarts, _bisecting and _center_shift); the defaults are those of a plain kmeans_cuda() call
+// _minibatch_init, _restarts, _bisecting and _center_shift); the defaults are those of a plain kmeans_cuda() call
 struct KMeansRequest {
   KMCUDAInitMethod init;
   const void* init_params;
@@ -92,8 +92,9 @@ struct KMeansRequest {
   Route route = Route::kLloyd;
   uint32_t batch_size = 0;           // mini-batch
   uint32_t max_steps = 0;            // mini-batch
+  uint32_t init_size = 0;            // mini-batch: rows the seeding reads (0 = all, KMCUDA_B200_INIT_SIZE_AUTO)
   bool relocate = false;             // Lloyd / Yinyang
-  uint32_t n_init = 1;               // Lloyd / Yinyang, bisecting
+  uint32_t n_init = 1;               // Lloyd / Yinyang, bisecting, mini-batch (with init_size)
   double* inertia = nullptr;         // Lloyd / Yinyang, bisecting
   int32_t strategy = 0;              // bisecting
   uint32_t max_iter = 0;             // bisecting, center shift
@@ -136,6 +137,14 @@ KMCUDAResult kmeans_impl(KMeansRequest r) {
     // one GPU, L2, a real batch; strict mode replays a Lloyd update that mini-batch steps do not have
     if (r.batch_size == 0 || r.metric == kmcudaDistanceMetricCosine || (r.device & (r.device - 1)) != 0 || strict) {
       KMB_INFO("mini-batch k-means takes batch_size >= 1, the L2 metric, one device and no strict update mode\n");
+      return kmcudaInvalidArguments;
+    }
+    // the init stage: an init size of at least K, on a seeding method; several inits only with an init size
+    if ((r.init_size != 0 && (r.init == kmcudaInitMethodImport ||
+                              (r.init_size != KMCUDA_B200_INIT_SIZE_AUTO && r.init_size < r.clusters_size))) ||
+        (r.n_init > 1 && r.init_size == 0)) {
+      KMB_INFO("mini-batch k-means takes an init size of at least the number of clusters with a seeding method, and "
+               "n_init > 1 only with an init size\n");
       return kmcudaInvalidArguments;
     }
     if (r.device == 0) r.device = 1;
@@ -206,8 +215,21 @@ KMCUDAResult kmeans_impl(KMeansRequest r) {
     }
     KMB_RET(job.bisecting(r.seed, r.tolerance, r.strategy, r.n_init, r.max_iter, trials, r.inertia));
   } else if (r.route == Route::kMinibatch) {
-    KMB_RET(job.init_centroids(r.init, r.init_params, r.seed, r.device_ptrs, fp16x2, r.centroids));
-    g_prof.mark("init centroids");
+    if (r.init_size == 0) {
+      KMB_RET(job.init_centroids(r.init, r.init_params, r.seed, r.device_ptrs, fp16x2, r.centroids));
+      g_prof.mark("init centroids");
+    } else {
+      // scikit-learn's MiniBatchKMeans._check_params_vs_input: 3 b, raised to 3 K, at most N (in 64 bits: 3 b > 2^32)
+      const uint64_t b = std::min(r.batch_size, r.samples_size);
+      uint64_t m = r.init_size;
+      if (r.init_size == KMCUDA_B200_INIT_SIZE_AUTO) {
+        m = 3 * b;
+        if (m < r.clusters_size) m = 3ull * r.clusters_size;
+      }
+      m = std::min<uint64_t>(m, r.samples_size);
+      KMB_RET(job.minibatch_init(r.init, r.init_params, r.seed, static_cast<uint32_t>(m), r.n_init, r.device_ptrs,
+                                 fp16x2));
+    }
     KMB_RET(job.minibatch(r.batch_size, r.max_steps, r.tolerance, r.seed));
   } else {
     // under the rule a negative reassignment tolerance: no pass count ends a run or sends Yinyang to Lloyd
@@ -285,12 +307,26 @@ KMCUDAResult kmcuda_b200_kmeans_minibatch(KMCUDAInitMethod init, const void* ini
                                           const float* samples, const float* weights, uint32_t batch_size,
                                           uint32_t max_steps, float* centroids, uint32_t* assignments,
                                           float* average_distance) {
+  return kmcuda_b200_kmeans_minibatch_init(init, init_params, tolerance, metric, samples_size, features_size,
+                                           clusters_size, seed, device, device_ptrs, fp16x2, verbosity, samples,
+                                           weights, batch_size, max_steps, 0, 1, centroids, assignments,
+                                           average_distance);
+}
+
+KMCUDAResult kmcuda_b200_kmeans_minibatch_init(KMCUDAInitMethod init, const void* init_params, float tolerance,
+                                               KMCUDADistanceMetric metric, uint32_t samples_size,
+                                               uint16_t features_size, uint32_t clusters_size, uint32_t seed,
+                                               uint32_t device, int32_t device_ptrs, int32_t fp16x2, int32_t verbosity,
+                                               const float* samples, const float* weights, uint32_t batch_size,
+                                               uint32_t max_steps, uint32_t init_size, uint32_t n_init,
+                                               float* centroids, uint32_t* assignments, float* average_distance) {
   return kmeans_impl({.init = init, .init_params = init_params, .tolerance = tolerance, .yinyang_t = 0.f,
                       .metric = metric, .samples_size = samples_size, .features_size = features_size,
                       .clusters_size = clusters_size, .seed = seed, .device = device, .device_ptrs = device_ptrs,
                       .fp16x2 = fp16x2, .verbosity = verbosity, .samples = samples, .weights = weights,
                       .centroids = centroids, .assignments = assignments, .average_distance = average_distance,
-                      .route = Route::kMinibatch, .batch_size = batch_size, .max_steps = max_steps});
+                      .route = Route::kMinibatch, .batch_size = batch_size, .max_steps = max_steps,
+                      .init_size = init_size, .n_init = n_init});
 }
 
 KMCUDAResult kmcuda_b200_kmeans_restarts(KMCUDAInitMethod init, const void* init_params, float tolerance,

@@ -946,6 +946,114 @@ KMCUDAResult Job::minibatch(uint32_t batch_size, uint64_t max_steps, float toler
   return kmcudaSuccess;
 }
 
+// The init stage of mini-batch k-means (DESIGN.md §4q), scikit-learn's MiniBatchKMeans init_size / n_init.  Init r seeds
+// with seed_r = seed + r * 0x9E3779B9 (mod 2^32), the restart schedule.  When m < N it seeds on the m rows
+// floor(u(seed, r, kMbTagInit) * N), drawn with replacement and gathered with their weights into a nested job, which
+// runs exactly the seeding of a kmcuda_b200_kmeans_weighted() call on them; otherwise on all rows.  With n_init > 1 the
+// inits are ranked by sum w e over m validation rows (kMbTagValid, step 0), assigned by the exact argmin; init 0 is the
+// first best, a later init replaces it only with a strictly lower inertia.  The kept centroids are left in C.
+KMCUDAResult Job::minibatch_init(KMCUDAInitMethod method, const void* init_params, uint32_t seed, uint32_t m,
+                                 uint32_t n_init, int device_ptrs, bool fp16x2) {
+  Dev& d = devs[0];
+  KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+  const size_t kd = static_cast<size_t>(K) * D;
+  const bool subset = m < N;
+  DevBuf<uint32_t> rows, vrows, result, row_result, keys;
+  DevBuf<float> gx, gw, bestC;
+  DevBuf<double> bsum, total;
+  std::unique_ptr<Shard> vs;   // the validation pass over m row entries
+  Drain drain{*this};
+  if (subset) {
+    KMB_CU(rows.alloc(m), kmcudaMemoryAllocationFailure);
+    KMB_CU(gx.alloc(static_cast<size_t>(m) * D), kmcudaMemoryAllocationFailure);
+    if (weighted) KMB_CU(gw.alloc(m), kmcudaMemoryAllocationFailure);
+  }
+  if (n_init > 1) {
+    vs.reset(new Shard(metric, d.dev, m, D, K, verbosity));
+    KMB_RET(vs->create(false));
+    KMB_CU(vrows.alloc(m), kmcudaMemoryAllocationFailure);
+    KMB_CU(result.alloc(m), kmcudaMemoryAllocationFailure);
+    KMB_CU(row_result.alloc(N), kmcudaMemoryAllocationFailure);
+    KMB_CU(keys.alloc(m), kmcudaMemoryAllocationFailure);
+    KMB_CU(bsum.alloc(mb_blocks(m)), kmcudaMemoryAllocationFailure);
+    KMB_CU(total.alloc(1), kmcudaMemoryAllocationFailure);
+    KMB_CU(bestC.alloc(kd), kmcudaMemoryAllocationFailure);
+    KMB_CU(launch_mb_draw(N, m, mb_step_key(seed, 0, kMbTagValid), vrows, d.st), kmcudaRuntimeError);
+  }
+  double best_inertia = 0;
+  uint32_t best_r = 0;
+  for (uint32_t r = 0; r < n_init; r++) {
+    const uint32_t seed_r = seed + r * 0x9E3779B9u;
+    // the seeding's own phases stay out of this call's profile
+    const bool prof = g_prof.on;
+    g_prof.on = false;
+    KMCUDAResult res = kmcudaSuccess;
+    if (!subset) {
+      res = init_centroids(method, init_params, seed_r, device_ptrs, fp16x2, nullptr);
+    } else {
+      // X (fp16x2 already widened on ingest) and w gathered to [m] rows; the nested job borrows them
+      if (cudaSetDevice(d.dev) != cudaSuccess ||
+          launch_mb_draw(N, m, mb_step_key(seed, r, kMbTagInit), rows, d.st) != cudaSuccess ||
+          launch_kmp_gather(d.X, D, rows, m, gx, d.st) != cudaSuccess ||
+          (weighted && launch_kmp_gather(d.w, 1, rows, m, gw, d.st) != cudaSuccess) ||
+          cudaStreamSynchronize(d.st) != cudaSuccess)
+        res = kmcudaRuntimeError;
+      Job sub(metric, m, D, K, verbosity);
+      sub.weighted = weighted;
+      if (res == kmcudaSuccess) res = sub.setup({d.dev});
+      if (res == kmcudaSuccess) {
+        sub.devs[0].X.borrow(gx.get());
+        if (weighted) {
+          sub.devs[0].w.borrow(gw.get());
+          res = sub.check_weights();   // (the weights are valid: only their sum over the rows can fail)
+          if (res == kmcudaInvalidArguments)
+            KMB_INFO("mini-batch init %" PRIu32 "/%" PRIu32 ": the weights of the %" PRIu32 " sampled rows sum to 0\n",
+                     r + 1, n_init, m);
+        }
+      }
+      if (res == kmcudaSuccess) res = sub.init_centroids(method, init_params, seed_r, -1, false, nullptr);
+      if (res == kmcudaSuccess) res = sub.sync_all();
+      if (res == kmcudaSuccess && (cudaSetDevice(d.dev) != cudaSuccess ||
+                                   cudaMemcpyAsync(d.C.get(), sub.devs[0].C.get(), sizeof(float) * kd,
+                                                   cudaMemcpyDeviceToDevice, d.st) != cudaSuccess ||
+                                   cudaStreamSynchronize(d.st) != cudaSuccess))
+        res = kmcudaMemoryCopyError;
+    }
+    g_prof.on = prof;
+    KMB_RET(res);
+    KMB_CU(cudaSetDevice(d.dev), kmcudaRuntimeError);
+    g_prof.mark("mini-batch init: seeding");
+    if (n_init == 1) {
+      KMB_INFO("mini-batch init %" PRIu32 "/%" PRIu32 ": seed %" PRIu32 ", %" PRIu32 " rows\n", r + 1, n_init, seed_r,
+               m);
+      break;
+    }
+    KMB_RET(vs->assign_rows(m, d.X, N, vrows, d.C, row_result, result, d.st));
+    KMB_CU(launch_mb_inertia(d.X, vrows, m, D, d.C, K, result, d.w.get(), keys, bsum, d.st), kmcudaRuntimeError);
+    KMB_CU(launch_fixed_sum(bsum, mb_blocks(m), total, d.st), kmcudaRuntimeError);
+    double e = 0;
+    KMB_CU(cudaMemcpyAsync(&e, total.get(), sizeof(double), cudaMemcpyDeviceToHost, d.st), kmcudaMemoryCopyError);
+    KMB_CU(cudaStreamSynchronize(d.st), kmcudaRuntimeError);
+    KMB_RET(vs->check_pipeline());
+    g_prof.mark("mini-batch init: validation");
+    KMB_INFO("mini-batch init %" PRIu32 "/%" PRIu32 ": seed %" PRIu32 ", %" PRIu32 " rows, validation inertia %.17g\n",
+             r + 1, n_init, seed_r, m, e);
+    if (r > 0 && !(e < best_inertia)) continue;
+    best_inertia = e;
+    best_r = r;
+    if (r + 1 < n_init)
+      KMB_CU(cudaMemcpyAsync(bestC.get(), d.C.get(), sizeof(float) * kd, cudaMemcpyDeviceToDevice, d.st),
+             kmcudaMemoryCopyError);
+  }
+  if (n_init > 1) {
+    if (best_r + 1 != n_init)
+      KMB_CU(cudaMemcpyAsync(d.C.get(), bestC.get(), sizeof(float) * kd, cudaMemcpyDeviceToDevice, d.st),
+             kmcudaMemoryCopyError);
+    KMB_INFO("mini-batch init: kept init %" PRIu32 "/%" PRIu32 "\n", best_r + 1, n_init);
+  }
+  return sync_all();
+}
+
 // Restarts (DESIGN.md §4n): restart r seeds with seed + r * 0x9E3779B9 (mod 2^32) and runs exactly what a fresh call
 // with that seed runs; the samples stay ingested.  State that outlives a run in this Job is reset before each one (the
 // per-device update state is reset by lloyd()).  Restart 0 is the first best and a later one replaces it only with a

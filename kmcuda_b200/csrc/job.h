@@ -200,6 +200,10 @@ class Job {
   KMCUDAResult lloyd_continue(float tolerance, int iter);
   KMCUDAResult yinyang(float tolerance, uint32_t G);
   KMCUDAResult minibatch(uint32_t batch_size, uint64_t max_steps, float tolerance, uint32_t seed);
+  // the init stage of a mini-batch run (DESIGN.md §4q) on the first device: n_init seedings, init r on m rows drawn
+  // with seed_r (all rows when m >= N), the one of lowest inertia on m validation rows left in C
+  KMCUDAResult minibatch_init(KMCUDAInitMethod method, const void* init_params, uint32_t seed, uint32_t m,
+                              uint32_t n_init, int device_ptrs, bool fp16x2);
   double lloyd_iter_ms = 0;   // wall time of the fastest complete Lloyd iteration of this run (assign pass + update), 0 = none yet
   KMCUDAResult group_centroids(uint32_t G, std::vector<uint32_t>* groups);
   // n_init seedings + Lloyd / Yinyang runs, the one of lowest inertia left in C / assign (kmcuda_b200_kmeans_restarts);

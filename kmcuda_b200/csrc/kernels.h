@@ -174,6 +174,10 @@ cudaError_t launch_kmp_weights(const uint32_t* nearest, const float* w, uint32_t
 constexpr uint64_t kMbTagBatch = 0x6D696E6962617463ull;      // "minibatc"
 constexpr uint64_t kMbTagReassign = 0x7265617373696721ull;   // "reassig!"
 constexpr uint64_t kGppTagTrial = 0x677265656479212Bull;     // "greedy!+": the trial draws of greedy k-means++
+// the init stage of a mini-batch run (Job::minibatch_init): the seeding subset of init r (step = r) and the validation
+// rows (step 0)
+constexpr uint64_t kMbTagInit = 0x6D62696E69747375ull;       // "mbinitsu"
+constexpr uint64_t kMbTagValid = 0x6D6276616C696421ull;      // "mbvalid!"
 uint64_t mb_step_key(uint32_t seed, uint64_t step, uint64_t tag);
 
 // ---- greedy k-means++ seeding (greedy_plusplus.cu) ------------------------------------------------------------------

@@ -209,14 +209,16 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
   PyObject *samples_obj, *init_obj = Py_None, *metric_obj = Py_None, *weight_obj = Py_None, *batch_obj = Py_None;
   PyObject *steps_obj = nullptr, *relocate_obj = Py_False, *n_init_obj = nullptr, *inertia_obj = Py_False;
   PyObject *bisecting_obj = Py_None, *max_iter_obj = nullptr, *tol_obj = Py_None, *n_iter_obj = Py_False;
+  PyObject* init_size_obj = Py_None;
   static const char* kwlist[] = {"samples", "clusters", "tolerance", "init", "yinyang_t", "metric",
                                  "average_distance", "seed", "device", "verbosity", "sample_weight", "batch_size",
                                  "max_steps", "relocate_empty_clusters", "n_init", "inertia", "bisecting",
-                                 "max_iter", "tol", "n_iter", nullptr};
-  if (!PyArg_ParseTupleAndKeywords(args, kwargs, "OL|fOfOpIIiOOOOOOOOOO", const_cast<char**>(kwlist), &samples_obj,
+                                 "max_iter", "tol", "n_iter", "init_size", nullptr};
+  if (!PyArg_ParseTupleAndKeywords(args, kwargs, "OL|fOfOpIIiOOOOOOOOOOO", const_cast<char**>(kwlist), &samples_obj,
                                    &clusters_arg, &tolerance, &init_obj, &yinyang_t, &metric_obj, &adflag, &seed,
                                    &device, &verbosity, &weight_obj, &batch_obj, &steps_obj, &relocate_obj,
-                                   &n_init_obj, &inertia_obj, &bisecting_obj, &max_iter_obj, &tol_obj, &n_iter_obj))
+                                   &n_init_obj, &inertia_obj, &bisecting_obj, &max_iter_obj, &tol_obj, &n_iter_obj,
+                                   &init_size_obj))
     return nullptr;
   // bisecting k-means (kmcuda_b200.h, kmcuda_b200_kmeans_bisecting): None or a strategy name
   int32_t strategy = -1;
@@ -327,7 +329,42 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
                                       "of them too");
     return nullptr;
   }
-  // restarts (kmcuda_b200.h, kmcuda_b200_kmeans_restarts): n_init an integer >= 1, inertia a bool; not with mini-batch
+  // the init stage of mini-batch k-means (kmcuda_b200.h, kmcuda_b200_kmeans_minibatch_init): init_size None (seed on
+  // all rows), an integer >= 1 or "auto"; with batch_size only
+  uint32_t init_size = 0;
+  if (init_size_obj != Py_None) {
+    if (PyUnicode_Check(init_size_obj)) {
+      const char* a = PyUnicode_AsUTF8(init_size_obj);
+      if (!a || strcmp(a, "auto") != 0) {
+        PyErr_Clear();
+        PyErr_SetString(PyExc_ValueError, "\"init_size\" must be None, an integer >= 1 or \"auto\"");
+        return nullptr;
+      }
+      init_size = KMCUDA_B200_INIT_SIZE_AUTO;
+    } else {
+      if (PyBool_Check(init_size_obj) || !(PyLong_Check(init_size_obj) || PyArray_IsScalar(init_size_obj, Integer))) {
+        PyErr_SetString(PyExc_TypeError, "\"init_size\" must be None, an integer or \"auto\"");
+        return nullptr;
+      }
+      int overflow = 0;
+      const long long v = PyLong_AsLongLongAndOverflow(init_size_obj, &overflow);
+      if ((v == -1 && PyErr_Occurred()) || overflow < 0 || (!overflow && v < 1)) {
+        PyErr_Clear();
+        PyErr_SetString(PyExc_ValueError, "\"init_size\" must be None, an integer >= 1 or \"auto\"");
+        return nullptr;
+      }
+      // every size from the number of rows up seeds on all rows; the largest value is the "auto" constant
+      init_size = overflow || v >= KMCUDA_B200_INIT_SIZE_AUTO ? KMCUDA_B200_INIT_SIZE_AUTO - 1
+                                                              : static_cast<uint32_t>(v);
+    }
+    if (strategy >= 0 || batch_obj == Py_None) {
+      PyErr_SetString(PyExc_ValueError, "\"init_size\" applies to mini-batch runs only: pass \"batch_size\" and no "
+                                        "\"bisecting\"");
+      return nullptr;
+    }
+  }
+  // restarts (kmcuda_b200.h, kmcuda_b200_kmeans_restarts): n_init an integer >= 1, inertia a bool; with mini-batch
+  // n_init needs init_size (it is the number of inits ranked on a validation batch)
   uint32_t n_init = 1;
   if (n_init_obj && !take_count(n_init_obj, "n_init", 1, &n_init)) return nullptr;
   if (!(PyBool_Check(inertia_obj) || PyArray_IsScalar(inertia_obj, Bool))) {
@@ -335,8 +372,13 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
     return nullptr;
   }
   const bool want_inertia = PyObject_IsTrue(inertia_obj) == 1;
-  if ((n_init != 1 || want_inertia) && batch_obj != Py_None) {
-    PyErr_SetString(PyExc_ValueError, "\"n_init\" and \"inertia\" apply to Lloyd / Yinyang runs, not to mini-batch "
+  if ((n_init != 1 && !init_size) && batch_obj != Py_None) {
+    PyErr_SetString(PyExc_ValueError, "\"n_init\" > 1 with mini-batch k-means (\"batch_size\") needs \"init_size\": "
+                                      "the inits are ranked on a validation batch of that many rows");
+    return nullptr;
+  }
+  if (want_inertia && batch_obj != Py_None) {
+    PyErr_SetString(PyExc_ValueError, "\"inertia\" applies to Lloyd / Yinyang and bisecting runs, not to mini-batch "
                                       "k-means (\"batch_size\")");
     return nullptr;
   }
@@ -402,6 +444,10 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
                                       "is the same run");
     return nullptr;
   }
+  if (init == kmcudaInitMethodImport && init_size) {
+    PyErr_SetString(PyExc_ValueError, "\"init_size\" needs a seeding method: imported centroids read no rows");
+    return nullptr;
+  }
   KMCUDADistanceMetric metric;
   if (!parse_metric(metric_obj, &metric)) return nullptr;
   if (clusters_arg < 2 || clusters_arg >= UINT32_MAX) {
@@ -409,6 +455,10 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
     return nullptr;
   }
   const uint32_t clusters = static_cast<uint32_t>(clusters_arg);
+  if (init_size && init_size != KMCUDA_B200_INIT_SIZE_AUTO && init_size < clusters) {
+    PyErr_SetString(PyExc_ValueError, "\"init_size\" must be at least the number of clusters");
+    return nullptr;
+  }
   float *samples = nullptr, *centroids = nullptr;
   uint32_t* assignments = nullptr;
   uint32_t n = 0, d = 0;
@@ -509,10 +559,10 @@ PyObject* py_kmeans_cuda(PyObject*, PyObject* args, PyObject* kwargs) {
     result = kmcuda_b200_kmeans_bisecting(init, &afkmc2_m, tolerance, metric, n, features, clusters, seed, device,
                                           device_ptrs, fp16x2, verbosity, samples, weights, strategy, n_init, max_iter,
                                           centroids, assignments, avg, inertia_out);
-  else if (batch_size)
-    result = kmcuda_b200_kmeans_minibatch(init, &afkmc2_m, tolerance, metric, n, features, clusters, seed, device,
-                                          device_ptrs, fp16x2, verbosity, samples, weights, batch_size, max_steps,
-                                          centroids, assignments, avg);
+  else if (batch_size)   // init_size 0 and n_init 1: the documented equal of kmcuda_b200_kmeans_minibatch()
+    result = kmcuda_b200_kmeans_minibatch_init(init, &afkmc2_m, tolerance, metric, n, features, clusters, seed, device,
+                                               device_ptrs, fp16x2, verbosity, samples, weights, batch_size, max_steps,
+                                               init_size, n_init, centroids, assignments, avg);
   else   // Lloyd / Yinyang with any weights, relocation and n_init: with n_init 1 and no inertia the header documents
          // this call as bit-identical to kmeans_cuda(), _weighted() and _relocate()
     result = kmcuda_b200_kmeans_restarts(init, &afkmc2_m, tolerance, yinyang_t, metric, n, features, clusters, seed,
@@ -664,7 +714,7 @@ char module_doc[] = "K-means and K-nn on NVIDIA H100 (drop-in for src-d/kmcuda's
 char kmeans_doc[] = "kmeans_cuda(samples, clusters, tolerance=.01, init=\"k-means++\", yinyang_t=.1, metric=\"L2\", "
                     "average_distance=False, seed=time(), device=0, verbosity=0, sample_weight=None, batch_size=None, "
                     "max_steps=0, relocate_empty_clusters=False, n_init=1, inertia=False, bisecting=None, max_iter=0, "
-                    "tol=None, n_iter=False) -> (centroids, assignments[, avg][, inertia][, n_iter]).  The keywords "
+                    "tol=None, n_iter=False, init_size=None) -> (centroids, assignments[, avg][, inertia][, n_iter]).  The keywords "
                     "are described in the kmcuda_b200 package's docstring.";
 char knn_doc[] = "knn_cuda(k, samples, centroids, assignments, metric=\"L2\", device=0, verbosity=0) -> neighbors";
 
