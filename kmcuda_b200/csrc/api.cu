@@ -201,7 +201,10 @@ KMCUDAResult kmeans_impl(KMeansRequest r) {
     g_prof.mark("weight check");
   }
   if (r.center_shift) {
-    KMB_RET(job.shift_tolerance(r.tol));   // once per call: every restart stops by the same tolerance
+    if (r.tol != 0) {   // once per call: every restart stops by the same tolerance
+      KMB_RET(job.mean_variance(&job.shift_tol));
+      job.shift_tol *= static_cast<double>(r.tol);
+    }
     g_prof.mark("center shift tolerance");
     KMB_INFO("center shift tolerance: %.17g, max_iter %" PRIu32 "\n", job.shift_tol, job.max_iter);
   }
@@ -211,9 +214,9 @@ KMCUDAResult kmeans_impl(KMeansRequest r) {
     uint32_t trials = 0;
     if (r.init == kmcudaInitMethodGreedyPlusPlus) {
       trials = r.init_params ? *static_cast<const uint32_t*>(r.init_params) : 0;
-      if (trials == 0) trials = 2 + static_cast<uint32_t>(std::log(2.0));
+      if (trials == 0) trials = greedy_plusplus_trials(2);
     }
-    KMB_RET(job.bisecting(r.seed, r.tolerance, r.strategy, r.n_init, r.max_iter, trials, r.inertia));
+    KMB_RET(job.bisecting(r.seed, r.tolerance, r.strategy, r.n_init, trials, r.inertia));
   } else if (r.route == Route::kMinibatch) {
     if (r.init_size == 0) {
       KMB_RET(job.init_centroids(r.init, r.init_params, r.seed, r.device_ptrs, fp16x2, r.centroids));

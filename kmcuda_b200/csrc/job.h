@@ -26,6 +26,10 @@ static const float kYinyangRefreshEpsilon = 1e-4f;      // reference kmeans.cu:2
 static const uint32_t kKMeansParallelRounds = 5;        // k-means|| rounds when init_params gives none
 static const uint32_t kKMeansParallelMaxRounds = 32;    // the round number is 8 bits of the draw hash's key
 static const uint32_t kGreedyPlusPlusMaxTrials = 32;    // greedy k-means++ trials per round (kGppMaxTrials)
+// greedy k-means++ trials per round when init_params gives none: scikit-learn's 2 + floor(ln k) for k centres
+inline uint32_t greedy_plusplus_trials(uint32_t k) {
+  return 2 + static_cast<uint32_t>(std::log(static_cast<double>(k)));
+}
 
 // Device teardown (transfer.cu).  A buffer goes back to the pool only after its stream has been synchronised
 // (kernels.h), also when a call returns early on an error while work is still queued: the owner of several devices
@@ -138,8 +142,8 @@ class Job {
   // scikit-learn's stopping rule instead of the reference's (kmcuda_b200_kmeans_center_shift, DESIGN.md §4p); set before
   // setup().  The runs are then given a negative reassignment tolerance, which never stops them.
   bool center_shift = false;
-  double shift_tol = 0;         // tol times the mean per-feature variance (shift_tolerance)
-  uint32_t max_iter = 300;      // the last update of a run
+  double shift_tol = 0;         // tol times the mean per-feature variance (mean_variance)
+  uint32_t max_iter = 300;      // the last update of a run (of a 2-means run in bisecting())
   int n_iter = 0;               // iterations of the last run (of the kept restart after restarts()), 0 while it runs
   uint32_t relocated = 0;       // rows relocated by the last relocate(), still in every device's rl_x / rl_meta
   double wtotal = 0;            // sum of the weights (check_weights)
@@ -193,11 +197,12 @@ class Job {
   KMCUDAResult update(int iter);
   KMCUDAResult lloyd_update(int iter);
   KMCUDAResult shift_of(const float* Cold);
-  KMCUDAResult shift_tolerance(float tol);
+  // scikit-learn's _tolerance before its factor tol: the mean over the features of their population variances
+  KMCUDAResult mean_variance(double* out);
   bool shift_stop(int iter, uint32_t changed, double shift);
   KMCUDAResult relocate(int iter);
-  KMCUDAResult lloyd(float tolerance, int* iter_out, uint32_t* changed_out);
-  KMCUDAResult lloyd_continue(float tolerance, int iter);
+  // iter == 0: a fresh run; iter > 0: the run continues after pass `iter` (Job::yinyang)
+  KMCUDAResult lloyd(float tolerance, int iter = 0, int* iter_out = nullptr, uint32_t* changed_out = nullptr);
   KMCUDAResult yinyang(float tolerance, uint32_t G);
   KMCUDAResult minibatch(uint32_t batch_size, uint64_t max_steps, float tolerance, uint32_t seed);
   // the init stage of a mini-batch run (DESIGN.md §4q) on the first device: n_init seedings, init r on m rows drawn
@@ -213,8 +218,8 @@ class Job {
                         double* inertia_out);
   // bisecting k-means (kmcuda_b200_kmeans_bisecting, DESIGN.md §4o) on the first device: C / assign, *inertia_out;
   // trials = 0: random init, else greedy k-means++ with that many trials
-  KMCUDAResult bisecting(uint32_t seed, float tolerance, int strategy, uint32_t n_init, uint32_t max_iter,
-                         uint32_t trials, double* inertia_out);
+  KMCUDAResult bisecting(uint32_t seed, float tolerance, int strategy, uint32_t n_init, uint32_t trials,
+                         double* inertia_out);
   KMCUDAResult inertia(double* out);
   KMCUDAResult average_distance(float* out);
 };

@@ -245,11 +245,9 @@ cudaError_t launch_mb_reassign(const MbReassign& r, cudaStream_t st);
 // out[0] = sum_c ||Cnew_c - Cold_c||^2 (double, fixed order), out[1] = #{W_c == 0}; dsq: [K] scratch
 cudaError_t launch_mb_stats(const float* Cold, const float* Cnew, const double* W, uint32_t K, int D, double* dsq,
                             double* out, cudaStream_t st);
-// var[D] = per-feature variance of X[n][D] (population, two passes in double); work: mb_variance_doubles(D) doubles
-size_t mb_variance_doubles(int D);
-cudaError_t launch_mb_variance(const float* X, uint32_t n, int D, double* work, double* var, cudaStream_t st);
-// one shard's share of the variance across devices: out[D] = the column sums of x_f (mean == nullptr) or of
-// (x_f - mean_f)^2 over X[n][D], in double, in the same fixed order as launch_mb_variance; work as there
+// one shard's share of the per-feature variance (Job::mean_variance): out[D] = the column sums of x_f (mean == nullptr)
+// or of (x_f - mean_f)^2 over X[n][D], in double, in a fixed order; work: col_sums_doubles(D) doubles
+size_t col_sums_doubles(int D);
 cudaError_t launch_col_sums(const float* X, uint32_t n, int D, const double* mean, double* work, double* out,
                             cudaStream_t st);
 // out[0] = sum_c ||Cnew_c - Cold_c||^2 (double, fixed order, a centroid whose term is not finite adds 0); dsq: [K]

@@ -188,13 +188,12 @@ mb_colsum_kernel(const float* __restrict__ X, uint32_t n, int D, const double* _
   }
 }
 
-__global__ void mb_colfold_kernel(const double* __restrict__ partial, int nb, int D, double scale,
-                                  double* __restrict__ out) {
+__global__ void mb_colfold_kernel(const double* __restrict__ partial, int nb, int D, double* __restrict__ out) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= D) return;
   double acc = 0.0;
   for (int q = 0; q < nb; q++) acc += partial[static_cast<size_t>(q) * D + f];
-  out[f] = acc * scale;
+  out[f] = acc;
 }
 
 }  // namespace
@@ -274,25 +273,12 @@ cudaError_t launch_center_shift(const float* Cold, const float* Cnew, uint32_t K
   return cudaGetLastError();
 }
 
-size_t mb_variance_doubles(int D) { return static_cast<size_t>(kVarBlocks) * D + 2 * static_cast<size_t>(D); }
-
-// out[f] = scale * (the column sum of x_f, or of (x_f - mean_f)^2), partials in work[kVarBlocks][D]
-static void col_pass(const float* X, uint32_t n, int D, const double* mean, double* work, double scale, double* out,
-                     cudaStream_t st) {
-  mb_colsum_kernel<<<kVarBlocks, 256, 0, st>>>(X, n, D, mean, work);
-  mb_colfold_kernel<<<cdiv(D, 256), 256, 0, st>>>(work, kVarBlocks, D, scale, out);
-}
-
-cudaError_t launch_mb_variance(const float* X, uint32_t n, int D, double* work, double* var, cudaStream_t st) {
-  double* mean = work + static_cast<size_t>(kVarBlocks) * D;
-  col_pass(X, n, D, nullptr, work, 1.0 / n, mean, st);
-  col_pass(X, n, D, mean, work, 1.0 / n, var, st);
-  return cudaGetLastError();
-}
+size_t col_sums_doubles(int D) { return static_cast<size_t>(kVarBlocks) * D; }
 
 cudaError_t launch_col_sums(const float* X, uint32_t n, int D, const double* mean, double* work, double* out,
                             cudaStream_t st) {
-  col_pass(X, n, D, mean, work, 1.0, out, st);
+  mb_colsum_kernel<<<kVarBlocks, 256, 0, st>>>(X, n, D, mean, work);
+  mb_colfold_kernel<<<cdiv(D, 256), 256, 0, st>>>(work, kVarBlocks, D, out);
   return cudaGetLastError();
 }
 

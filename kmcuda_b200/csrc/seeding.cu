@@ -742,8 +742,7 @@ KMCUDAResult Job::init_centroids(KMCUDAInitMethod method, const void* init_param
     }
     case kmcudaInitMethodGreedyPlusPlus: {
       const uint32_t t = init_params ? *reinterpret_cast<const uint32_t*>(init_params) : 0;
-      // (t <= 32: kmeans_impl); 0 = scikit-learn's 2 + floor(ln K)
-      KMB_RET(init_greedy_plusplus(t ? t : 2 + static_cast<uint32_t>(std::log(static_cast<double>(K))), seed));
+      KMB_RET(init_greedy_plusplus(t ? t : greedy_plusplus_trials(K), seed));   // (t <= 32: kmeans_impl)
       break;
     }
     default:

@@ -157,7 +157,7 @@ def _final(lab, e, we, wd, C, it, stop, relocations):
 
 
 def tolerance_abs(X, tolerance):
-    """tolerance times the mean of the unweighted per-feature variances (launch_mb_variance's arithmetic is checked on
+    """tolerance times the mean of the unweighted per-feature variances (Job::mean_variance's arithmetic is checked on
     the GPU; numpy's two-pass variance agrees with it to rounding, so the CPU tests keep away from the boundary)"""
     Xd = X.astype(np.float64)
     var = ((Xd - Xd.mean(axis=0)) ** 2).mean(axis=0)

@@ -57,7 +57,7 @@ def _run(km, capfd, X, K, strategy, n_init=1, tolerance=1e-4, max_iter=0, w=None
 
 def _pin(km, capfd, X, K, strategy, n_init=1, tolerance=1e-4, max_iter=0, w=None, init="random"):
     C, A, e, lines = _run(km, capfd, X, K, strategy, n_init, tolerance, max_iter, w, init)
-    # the device's tolerance comes from launch_mb_variance; the model's numpy variance agrees with it to rounding, which
+    # the device's tolerance comes from Job::mean_variance; the model's numpy variance agrees with it to rounding, which
     # no stop decision of these cases lies within
     for waves in (True, False):
         mC, mA, mlines, me, _, _ = M.bisecting(X, K, SEED, strategy, n_init, tolerance, max_iter, w, waves, init=init)
