@@ -215,15 +215,22 @@ KMCUDAResult Shard::yy_refresh(uint32_t n, const float* X, const float* C, const
   return kmcudaSuccess;
 }
 
-// one Yinyang iteration after the centroid update: reference kmeans.cu:1180-1262 (drifts, global and local filter)
+// one Yinyang iteration after the centroid update: reference kmeans.cu:1180-1262 (drifts, global and local filter).
+// Routes of the local step: kYyRouteTc = tensor-core candidates (MODE 1) + yy_finish_kernel, the rows MODE 1 cannot
+// bound to yy_rows_cta_kernel; kYyRouteCta = every surviving row to yy_rows_cta_kernel; kYyRouteScan = every surviving
+// row to the reference-order scan (yy_local_scan_kernel).  The last two take the upper bounds from
+// yy_tight_scan_kernel.
 KMCUDAResult Shard::yy_step(uint32_t n, const float* X, const float* C, uint32_t* assignments, uint32_t* prev,
-                            uint32_t* d_changed, cudaStream_t st) {
+                            uint32_t* d_changed, cudaStream_t st, int route) {
   if (n > max_n) return kmcudaInvalidArguments;
+  if (route == kYyRouteAuto) route = tc ? kYyRouteTc : force_exact ? kYyRouteScan : kYyRouteCta;
+  if (route < kYyRouteTc || route > kYyRouteScan || (route == kYyRouteTc && !tc)) return kmcudaInvalidArguments;
+  TcPlan* plan = route == kYyRouteTc ? tc : nullptr;
   KMB_CU(launch_yy_drifts(metric, C, oldC, K, D, G, groups, drift, maxdrift, st), kmcudaRuntimeError);
-  if (tc) KMB_CU(launch_csqr(metric, C, K, D, csq, st), kmcudaRuntimeError);
+  if (plan) KMB_CU(launch_csqr(metric, C, K, D, csq, st), kmcudaRuntimeError);
   YyWorkspace ws{yy_minlb, yy_tight_rows, yy_tight_cand, yy_tight_score, passed, yy_gsize, yy_counters};
-  KMB_CU(launch_yy_step(metric, tc, X, C, csq, n, D, K, G, groups, drift, maxdrift, assignments, prev, bounds, ws,
-                        d_changed, force_exact, st), kmcudaRuntimeError);
+  KMB_CU(launch_yy_step(metric, plan, X, C, csq, n, D, K, G, groups, drift, maxdrift, assignments, prev, bounds, ws,
+                        d_changed, route == kYyRouteScan, st), kmcudaRuntimeError);
   return kmcudaSuccess;
 }
 
@@ -475,6 +482,52 @@ int32_t kmcuda_b200_debug_yy_bounds(kmcuda_b200_shard* shard, uint32_t n, const 
     return -9;
   if (cudaStreamSynchronize(st) != cudaSuccess) return -10;
   return (use_tc && kmb::tc_last_error(s->tc)) ? -11 : 0;
+}
+// One Yinyang iteration (Shard::yy_step, on the given route) from a given state, for tests.  Device: samples [n][D],
+// c_old / c_new [K][D], assignments [n] (in / out), prev [n] (out), bounds [n][G + 1] (in / out), drift_out [K],
+// maxdrift_out [G]; host: host_groups [K], counts_out [6] = changed, rows whose upper bound was recomputed (filter #1
+// failed), rows passed to the local step (filter #2 failed), and for the tensor-core route the MODE 1 pass's re-checked
+// rows, overflowed rows and pipeline error word (0 on the other routes).  Synchronous; 0 or a negative code.
+int32_t kmcuda_b200_debug_yy_step(kmcuda_b200_shard* shard, uint32_t n, const float* samples, const float* c_old,
+                                  const float* c_new, uint32_t* assignments, uint32_t* prev,
+                                  const uint32_t* host_groups, uint32_t G, float* bounds, int32_t route,
+                                  float* drift_out, float* maxdrift_out, uint32_t* counts_out) {
+  if (!shard || !samples || !c_old || !c_new || !assignments || !prev || !host_groups || !bounds || !drift_out ||
+      !maxdrift_out || !counts_out || G == 0)
+    return -1;
+  kmb::Shard* s = shard->impl;
+  if (n > s->max_n) return -2;
+  if (route == kmb::Shard::kYyRouteTc && !s->tc) return -3;
+  if (s->enable_yinyang(G) != kmcudaSuccess) return -4;
+  cudaStream_t st = nullptr;
+  const size_t kd = static_cast<size_t>(s->K) * s->D, nb = static_cast<size_t>(n) * (G + 1);
+  kmb::DevBuf<uint32_t> d_changed;
+  if (d_changed.alloc(1) != cudaSuccess) return -4;
+  if (cudaMemcpy(s->groups.get(), host_groups, sizeof(uint32_t) * s->K, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemsetAsync(d_changed.get(), 0, sizeof(uint32_t), st) != cudaSuccess ||
+      cudaMemsetAsync(s->yy_counters.get(), 0, sizeof(uint32_t) * 4, st) != cudaSuccess ||
+      cudaMemcpyAsync(s->oldC.get(), c_old, sizeof(float) * kd, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
+      cudaMemcpyAsync(s->bounds.get(), bounds, sizeof(float) * nb, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+    return -5;
+  if (s->yy_prepare(host_groups, st) != kmcudaSuccess) return -6;
+  if (s->yy_step(n, samples, c_new, assignments, prev, d_changed, st, route) != kmcudaSuccess) return -7;
+  if (cudaMemcpyAsync(bounds, s->bounds.get(), sizeof(float) * nb, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
+      cudaMemcpyAsync(drift_out, s->drift.get(), sizeof(float) * s->K, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
+      cudaMemcpyAsync(maxdrift_out, s->maxdrift.get(), sizeof(float) * G, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+    return -8;
+  uint32_t yc[4] = {0, 0, 0, 0}, changed = 0;
+  if (cudaStreamSynchronize(st) != cudaSuccess ||
+      cudaMemcpy(yc, s->yy_counters.get(), sizeof(yc), cudaMemcpyDeviceToHost) != cudaSuccess ||
+      cudaMemcpy(&changed, d_changed.get(), sizeof(uint32_t), cudaMemcpyDeviceToHost) != cudaSuccess)
+    return -9;
+  uint32_t rechecked = 0, overflowed = 0, err = 0;
+  if (route == kmb::Shard::kYyRouteTc || (route == kmb::Shard::kYyRouteAuto && s->tc)) {
+    kmb::tc_last_stats(s->tc, &rechecked, &overflowed);
+    err = kmb::tc_last_error(s->tc);
+  }
+  const uint32_t out[6] = {changed, yc[0], yc[1], rechecked, overflowed, err};
+  for (int i = 0; i < 6; i++) counts_out[i] = out[i];
+  return 0;
 }
 // the mini-batch assignment (Shard::assign_rows) of the n listed rows of samples [samples_size][D]: result [n] by list
 // position, row_scratch [samples_size]; device pointers, enqueued on `stream`.  0, or a negative code

@@ -104,8 +104,11 @@ class Shard {
   KMCUDAResult yy_prepare(const uint32_t* host_groups, cudaStream_t st);
   // (re)builds the bounds of every sample of the shard: reference kmeans_yy_init, kmeans.cu:431-485
   KMCUDAResult yy_refresh(uint32_t n, const float* X, const float* C, const uint32_t* assignments, cudaStream_t st);
+  // route of the local step: kYyRouteAuto = the shard's choice (kYyRouteTc with a tensor-core plan, kYyRouteScan under
+  // KMCUDA_B200_FORCE_EXACT, kYyRouteCta otherwise); the other three pick one (tests)
+  enum { kYyRouteAuto = -1, kYyRouteTc = 0, kYyRouteCta = 1, kYyRouteScan = 2 };
   KMCUDAResult yy_step(uint32_t n, const float* X, const float* C, uint32_t* assignments, uint32_t* prev,
-                       uint32_t* d_changed, cudaStream_t st);
+                       uint32_t* d_changed, cudaStream_t st, int route = kYyRouteAuto);
 
   // hot path
   KMCUDAResult assign(uint32_t n, const float* X, const float* C, uint32_t* assignments,

@@ -36,6 +36,9 @@ _lib.kmcuda_b200_debug_yy_bounds.restype = ctypes.c_int32
 _lib.kmcuda_b200_debug_yy_bounds.argtypes = [ctypes.c_void_p, ctypes.c_uint32, ctypes.c_void_p, ctypes.c_void_p,
                                              ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32, ctypes.c_int32,
                                              ctypes.c_void_p]
+_lib.kmcuda_b200_debug_yy_step.restype = ctypes.c_int32
+_lib.kmcuda_b200_debug_yy_step.argtypes = [ctypes.c_void_p, ctypes.c_uint32] + [ctypes.c_void_p] * 6 + \
+    [ctypes.c_uint32, ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
 _lib.kmcuda_b200_debug_assign_rows.restype = ctypes.c_int32
 _lib.kmcuda_b200_debug_assign_rows.argtypes = [ctypes.c_void_p, ctypes.c_uint32, ctypes.c_void_p, ctypes.c_uint32] + \
     [ctypes.c_void_p] * 5
@@ -145,6 +148,28 @@ class Shard:
         if rc != 0:
             raise RuntimeError("kmcuda_b200_debug_yy_bounds failed (%d)" % rc)
         return out
+
+    def debug_yy_step(self, X, C_old, C_new, assignments, groups, G, bounds, route=-1):
+        """One Yinyang iteration (Shard::yy_step) from the given state (diagnostics / parity tests): the drifts from C_old
+        to C_new, the global filter and the local step on `route` (-1 the library's choice, 0 tensor cores, 1 one CTA per
+        row, 2 the reference-order scan).  assignments (int32 [n]) and bounds (float32 [n][G + 1]) are updated in place;
+        groups: host uint32 [K].  Returns (prev, drift, maxdrift, counts) with counts = dict(changed, tight, passed,
+        rechecked, overflowed, error)."""
+        groups = np.ascontiguousarray(groups, dtype=np.uint32)
+        n, K = X.shape[0], C_new.shape[0]
+        prev = torch.empty(n, dtype=torch.int32, device=X.device)
+        drift = torch.empty(K, dtype=torch.float32, device=X.device)
+        maxdrift = torch.empty(G, dtype=torch.float32, device=X.device)
+        counts = np.zeros(6, np.uint32)
+        rc = _lib.kmcuda_b200_debug_yy_step(self._h, n, _ptr(X, torch.float32), _ptr(C_old, torch.float32),
+                                            _ptr(C_new, torch.float32), _ptr(assignments, torch.int32),
+                                            _ptr(prev, torch.int32), groups.ctypes.data, int(G),
+                                            _ptr(bounds, torch.float32), int(route), _ptr(drift, torch.float32),
+                                            _ptr(maxdrift, torch.float32), counts.ctypes.data)
+        if rc != 0:
+            raise RuntimeError("kmcuda_b200_debug_yy_step failed (%d)" % rc)
+        keys = ("changed", "tight", "passed", "rechecked", "overflowed", "error")
+        return prev, drift, maxdrift, dict(zip(keys, counts.tolist()))
 
     def debug_assign_rows(self, X, C, rows, out=None, scratch=None, sync=True):
         """the mini-batch assignment of the samples X[rows] (Shard::assign_rows, the row-list tensor-core pass): winners

@@ -318,6 +318,111 @@ static int ko_lloyd_loop(int metric, float tolerance, const float *X, uint32_t N
 }
 
 /* ------------------------------------------------------------------------------------------ */
+/* The three pieces of a Yinyang iteration, on the reference's bound planes: bounds[g * N + i], */
+/* plane 0 the upper bound, plane 1 + g the lower bound of group g.  ko_kmeans below calls      */
+/* them, so the whole-run oracle and the single-step oracle are the same code.                  */
+/* ------------------------------------------------------------------------------------------ */
+
+/* bounds refresh: kmeans_yy_init, kmeans.cu:431-485 */
+void ko_yy_init(int metric, const float *X, const float *C, uint32_t N, int D, uint32_t K, uint32_t G,
+                const uint32_t *groups, const uint32_t *assign, float *bounds) {
+#pragma omp parallel for schedule(static)
+  for (uint32_t i = 0; i < N; i++) {
+    for (uint32_t g = 0; g <= G; g++) bounds[(size_t)N * g + i] = FLT_MAX;
+    uint32_t nearest = assign[i];
+    for (uint32_t c = 0; c < K; c++) {
+      uint32_t g = groups[c];
+      if (g >= G) continue;
+      float d = ko_distance(metric, X + (size_t)i * D, C + (size_t)c * D, D);
+      if (c != nearest) {
+        if (d < bounds[(size_t)N * (1 + g) + i]) bounds[(size_t)N * (1 + g) + i] = d;
+      } else {
+        bounds[i] = d;
+      }
+    }
+  }
+}
+
+/* drifts, kmeans_yy_calc_drifts, kmeans.cu:487-499, and the group maxima,
+ * kmeans_yy_find_group_max_drifts, kmeans.cu:501-538 (a group without members keeps -FLT_MAX) */
+void ko_yy_drifts(int metric, const float *C, const float *oldC, uint32_t K, int D, uint32_t G,
+                  const uint32_t *groups, float *drift, float *maxdrift) {
+  for (uint32_t c = 0; c < K; c++)
+    drift[c] = ko_distance(metric, C + (size_t)c * D, oldC + (size_t)c * D, D);
+  for (uint32_t g = 0; g < G; g++) {
+    float m = -FLT_MAX;
+    for (uint32_t c = 0; c < K; c++) if (groups[c] == g && m < drift[c]) m = drift[c];
+    maxdrift[g] = m;
+  }
+}
+
+/* Global filter, kmeans.cu:540-582, then local filter, kmeans.cu:584-672.  Returns the number of
+ * changed assignments; *tight_out = rows whose decayed lower bounds do not prune them (filter #1
+ * fails, the upper bound is recomputed), *passed_out = rows that also fail filter #2 (local step).
+ * Two guards are not in the reference, which reads or writes out of range there; both restate
+ * the library's own (yinyang.cu):
+ *   - a row assigned >= K ("insane", first feature NaN) gets prev = assign and keeps its bounds
+ *     (the reference reads drift[K]);
+ *   - no bound is written for a group >= G (the reference writes plane 1 + G, past the end). */
+uint32_t ko_yy_step(int metric, const float *X, const float *C, uint32_t N, int D, uint32_t K, uint32_t G,
+                    const uint32_t *groups, const float *drift, const float *maxdrift, uint32_t *assign,
+                    uint32_t *prev, float *bounds, uint32_t *tight_out, uint32_t *passed_out) {
+  uint32_t *passed = (uint32_t *)malloc(sizeof(uint32_t) * (N ? N : 1));
+  uint32_t npassed = 0, ntight = 0;
+  for (uint32_t i = 0; i < N; i++) {
+    uint32_t a = assign[i];
+    prev[i] = a;
+    if (a >= K) continue; /* deviation: the library's guard (yy_decay_kernel) */
+    float ub = bounds[i] + drift[a];
+    float minlb = FLT_MAX;
+    for (uint32_t g = 0; g < G; g++) {
+      float lb = bounds[(size_t)N * (1 + g) + i] - maxdrift[g];
+      bounds[(size_t)N * (1 + g) + i] = lb;
+      if (lb < minlb) minlb = lb;
+    }
+    if (minlb >= ub) { bounds[i] = ub; continue; }
+    ntight++;
+    ub = ko_distance(metric, X + (size_t)i * D, C + (size_t)a * D, D);
+    bounds[i] = ub;
+    if (minlb >= ub) continue;
+    passed[npassed++] = i;
+  }
+  uint32_t ch = 0;
+#pragma omp parallel for schedule(dynamic, 64) reduction(+ : ch)
+  for (uint32_t pi = 0; pi < npassed; pi++) {
+    uint32_t i = passed[pi];
+    float ub = bounds[i];
+    uint32_t a = assign[i];
+    float mn = ub, sec = FLT_MAX;
+    uint32_t near = a;
+    for (uint32_t c = 0; c < K; c++) {
+      if (c == a) continue;
+      uint32_t g = groups[c];
+      if (g >= G) continue;
+      float lb = bounds[(size_t)N * (1 + g) + i];
+      if (lb >= ub) { if (lb < sec) sec = lb; continue; }
+      lb += maxdrift[g] - drift[c];
+      if (sec < lb) continue;
+      float d = ko_distance(metric, X + (size_t)i * D, C + (size_t)c * D, D);
+      if (d < mn) { sec = mn; mn = d; near = c; }
+      else if (d < sec) sec = d;
+    }
+    uint32_t ng = groups[near], pg = groups[a];
+    if (ng < G) bounds[(size_t)N * (1 + ng) + i] = sec; /* deviation: ng < G, pg < G (yy_finish_kernel) */
+    if (ng != pg && pg < G) {
+      float pb = bounds[(size_t)N * (1 + pg) + i];
+      if (pb > ub) bounds[(size_t)N * (1 + pg) + i] = ub;
+    }
+    bounds[i] = mn;
+    if (a != near) { assign[i] = near; ch++; }
+  }
+  free(passed);
+  if (tight_out) *tight_out = ntight;
+  if (passed_out) *passed_out = npassed;
+  return ch;
+}
+
+/* ------------------------------------------------------------------------------------------ */
 /* Whole k-means run from imported centroids: kmeans_cuda_yy, kmeans.cu:1028-1263.              */
 /* yy_groups==0 or tolerance>=0.11 -> pure Lloyd.  Returns total "iteration" lines emitted.     */
 /* ------------------------------------------------------------------------------------------ */
@@ -355,7 +460,6 @@ int ko_kmeans(int metric, float tolerance, uint32_t yy_groups, const float *X, u
   float *oldC = (float *)malloc(sizeof(float) * (size_t)K * D);
   float *drift = (float *)malloc(sizeof(float) * K);
   float *maxdrift = (float *)malloc(sizeof(float) * G);
-  uint32_t *passed = (uint32_t *)malloc(sizeof(uint32_t) * N);
   int refresh = 1;
   uint32_t npassed = 0;
   changed = 0; /* prepare_mem(resume=true) zeroes d_changed_number, kmeans.cu:1102-1103 */
@@ -369,85 +473,17 @@ int ko_kmeans(int metric, float tolerance, uint32_t yy_groups, const float *X, u
       if (1.f - (npassed + 0.f) / N < 1e-4f) refresh = 1;
       npassed = 0;
     }
-    if (refresh) { /* kmeans_yy_init, kmeans.cu:431-485 */
-#pragma omp parallel for schedule(static)
-      for (uint32_t i = 0; i < N; i++) {
-        for (uint32_t g = 0; g <= G; g++) bounds[(size_t)N * g + i] = FLT_MAX;
-        uint32_t nearest = assign[i];
-        for (uint32_t c = 0; c < K; c++) {
-          uint32_t g = groups[c];
-          if (g >= G) continue;
-          float d = ko_distance(metric, X + (size_t)i * D, C + (size_t)c * D, D);
-          if (c != nearest) {
-            if (d < bounds[(size_t)N * (1 + g) + i]) bounds[(size_t)N * (1 + g) + i] = d;
-          } else {
-            bounds[i] = d;
-          }
-        }
-      }
+    if (refresh) {
+      ko_yy_init(metric, X, C, N, D, K, G, groups, assign, bounds);
       refresh = 0;
     }
     memcpy(oldC, C, sizeof(float) * (size_t)K * D);
     ko_adjust(metric, X, N, D, K, prev, assign, C, ccounts);
-    for (uint32_t c = 0; c < K; c++) /* kmeans_yy_calc_drifts, kmeans.cu:487-499 */
-      drift[c] = ko_distance(metric, C + (size_t)c * D, oldC + (size_t)c * D, D);
-    for (uint32_t g = 0; g < G; g++) { /* kmeans_yy_find_group_max_drifts, kmeans.cu:501-538 */
-      float m = -FLT_MAX;
-      for (uint32_t c = 0; c < K; c++) if (groups[c] == g && m < drift[c]) m = drift[c];
-      maxdrift[g] = m;
-    }
-    /* global filter, kmeans.cu:540-582 */
-    npassed = 0;
-    for (uint32_t i = 0; i < N; i++) {
-      uint32_t a = assign[i];
-      prev[i] = a;
-      float ub = bounds[i] + drift[a];
-      float minlb = FLT_MAX;
-      for (uint32_t g = 0; g < G; g++) {
-        float lb = bounds[(size_t)N * (1 + g) + i] - maxdrift[g];
-        bounds[(size_t)N * (1 + g) + i] = lb;
-        if (lb < minlb) minlb = lb;
-      }
-      if (minlb >= ub) { bounds[i] = ub; continue; }
-      ub = ko_distance(metric, X + (size_t)i * D, C + (size_t)a * D, D);
-      bounds[i] = ub;
-      if (minlb >= ub) continue;
-      passed[npassed++] = i;
-    }
-    /* local filter, kmeans.cu:584-672 */
-    uint32_t ch = 0;
-#pragma omp parallel for schedule(dynamic, 64) reduction(+ : ch)
-    for (uint32_t pi = 0; pi < npassed; pi++) {
-      uint32_t i = passed[pi];
-      float ub = bounds[i];
-      uint32_t a = assign[i];
-      float mn = ub, sec = FLT_MAX;
-      uint32_t near = a;
-      for (uint32_t c = 0; c < K; c++) {
-        if (c == a) continue;
-        uint32_t g = groups[c];
-        if (g >= G) continue;
-        float lb = bounds[(size_t)N * (1 + g) + i];
-        if (lb >= ub) { if (lb < sec) sec = lb; continue; }
-        lb += maxdrift[g] - drift[c];
-        if (sec < lb) continue;
-        float d = ko_distance(metric, X + (size_t)i * D, C + (size_t)c * D, D);
-        if (d < mn) { sec = mn; mn = d; near = c; }
-        else if (d < sec) sec = d;
-      }
-      uint32_t ng = groups[near], pg = groups[a];
-      bounds[(size_t)N * (1 + ng) + i] = sec;
-      if (ng != pg) {
-        float pb = bounds[(size_t)N * (1 + pg) + i];
-        if (pb > ub) bounds[(size_t)N * (1 + pg) + i] = ub;
-      }
-      bounds[i] = mn;
-      if (a != near) { assign[i] = near; ch++; }
-    }
-    changed = ch;
+    ko_yy_drifts(metric, C, oldC, K, D, G, groups, drift, maxdrift);
+    changed = ko_yy_step(metric, X, C, N, D, K, G, groups, drift, maxdrift, assign, prev, bounds, NULL, &npassed);
   }
   free(prev); free(ccounts); free(GC); free(groups); free(bounds); free(oldC); free(drift);
-  free(maxdrift); free(passed);
+  free(maxdrift);
   return lines;
 }
 

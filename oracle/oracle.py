@@ -60,6 +60,15 @@ def lib():
         L.ko_kmeans.restype = ctypes.c_int
         L.ko_kmeans.argtypes = [ctypes.c_int, ctypes.c_float, ctypes.c_uint32, _f32p, ctypes.c_uint32,
                                 ctypes.c_int, ctypes.c_uint32, _f32p, _u32p, ctypes.c_int, ctypes.c_int]
+        L.ko_yy_init.restype = None
+        L.ko_yy_init.argtypes = [ctypes.c_int, _f32p, _f32p, ctypes.c_uint32, ctypes.c_int, ctypes.c_uint32,
+                                 ctypes.c_uint32, _u32p, _u32p, _f32p]
+        L.ko_yy_drifts.restype = None
+        L.ko_yy_drifts.argtypes = [ctypes.c_int, _f32p, _f32p, ctypes.c_uint32, ctypes.c_int, ctypes.c_uint32,
+                                   _u32p, _f32p, _f32p]
+        L.ko_yy_step.restype = ctypes.c_uint32
+        L.ko_yy_step.argtypes = [ctypes.c_int, _f32p, _f32p, ctypes.c_uint32, ctypes.c_int, ctypes.c_uint32,
+                                 ctypes.c_uint32, _u32p, _f32p, _f32p, _u32p, _u32p, _f32p, _u32p, _u32p]
         L.ko_knn.restype = None
         L.ko_knn.argtypes = [ctypes.c_int, ctypes.c_int, _f32p, ctypes.c_uint32, ctypes.c_int, _f32p,
                              ctypes.c_uint32, _u32p, _u32p, ctypes.c_uint32, _u32p, _f64p]
@@ -149,6 +158,47 @@ def kmeans(X, C0, tolerance=0.01, yinyang_t=0.1, metric=0, log=False, max_iter=0
     G = int(np.float32(yinyang_t) * np.float32(K))
     lines = lib().ko_kmeans(metric, tolerance, G, _f(X), N, D, K, _f(C), _u(a), int(log), int(max_iter))
     return C, a, lines
+
+
+# Yinyang pieces (kmeans.cu:431-672).  Bounds are row-major [N][G + 1] here, the library's layout (column 0 the upper
+# bound, column 1 + g the lower bound of group g); the C side keeps the reference's [(G + 1)][N] planes.
+def yy_init(X, C, assign, groups, G, metric=0):
+    """bounds refresh (kmeans_yy_init): [N][G + 1] float32"""
+    X, C = _c32(X), _c32(C)
+    N, D = X.shape
+    a = np.ascontiguousarray(assign, dtype=np.uint32)
+    g = np.ascontiguousarray(groups, dtype=np.uint32)
+    planes = np.empty((G + 1, N), np.float32)
+    lib().ko_yy_init(metric, _f(X), _f(C), N, D, C.shape[0], G, _u(g), _u(a), _f(planes))
+    return np.ascontiguousarray(planes.T)
+
+
+def yy_drifts(C_new, C_old, groups, G, metric=0):
+    """(drift [K], maxdrift [G]): distance of each centroid from its old position, largest per group (-FLT_MAX if
+    the group has no member)"""
+    Cn, Co = _c32(C_new), _c32(C_old)
+    K, D = Cn.shape
+    g = np.ascontiguousarray(groups, dtype=np.uint32)
+    drift = np.empty(K, np.float32)
+    maxdrift = np.empty(max(G, 1), np.float32)
+    lib().ko_yy_drifts(metric, _f(Cn), _f(Co), K, D, G, _u(g), _f(drift), _f(maxdrift))
+    return drift, maxdrift[:G]
+
+
+def yy_step(X, C, groups, G, drift, maxdrift, assign, bounds, metric=0):
+    """global + local filter after a centroid update.  Returns (assign, prev, bounds, changed, tight, passed); the
+    inputs are not modified"""
+    X, C = _c32(X), _c32(C)
+    N, D = X.shape
+    g = np.ascontiguousarray(groups, dtype=np.uint32)
+    a = np.array(assign, dtype=np.uint32)
+    prev = np.empty(N, np.uint32)
+    planes = np.ascontiguousarray(np.asarray(bounds, np.float32).reshape(N, G + 1).T)
+    dr, md = _c32(drift), _c32(maxdrift)
+    tight, passed = ctypes.c_uint32(0), ctypes.c_uint32(0)
+    changed = lib().ko_yy_step(metric, _f(X), _f(C), N, D, C.shape[0], G, _u(g), _f(dr), _f(md), _u(a), _u(prev),
+                               _f(planes), ctypes.byref(tight), ctypes.byref(passed))
+    return a, prev, np.ascontiguousarray(planes.T), int(changed), tight.value, passed.value
 
 
 def knn(k, X, C, assign, metric=0, queries=None):
